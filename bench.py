@@ -7,13 +7,17 @@ Workload at N=1: BASELINE configs[1], 32 clips x 10 s (300 frames each, 9 600 fr
 N>1 each rank runs its own 32 clips (weak scaling, configs[4]); weights are broadcast from rank 0 once
 at load (NCCL) and there is no collective inside the step.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
 
 Prints ONE JSON line (rank 0).  `value` = device-timed frames/s with inputs resident in HBM; `e2e` = the
 same span through the public API with pinned HOST buffers (H2D audio + D2H results inside the timed
 region, wall clock).  `roofline` = the dominant kernel (tap-GEMM) against the measured bf16 peak,
 `roofline_vq` = the VQ lookup kernel against the measured HBM bandwidth on 2^21 rows, `extra` = the other
 BASELINE configs (bs = 1 latency, CaMN bs 64, DisCo bs 32).
+
+`--dump-outputs DIR` writes what the timed path returned in its last timed step (the latent and prediction dicts of
+generate()) as DIR/<dict>_<key>.npy, float32 (float64 for integer arrays, exact), at most 64 MB in all: the inputs are
+seeded, so two builds can be compared output for output.
 
 `--impl reference` times the UNMODIFIED reference modules (byte-compiled into oracle/_ref by
 oracle/make_ref.py; falls back to the oracle port when that tree is absent) on the host cores, on the same
@@ -39,14 +43,10 @@ FLOP_PER_FRAME = 364.7e6              # SURVEY.md section 8(d): algorithmic work
 DTYPES = {"fp32": "f32", "fp16x3": "fp16x3 (two fp16 operand planes, 3 products, f32 accumulate)",
           "bf16x6": "bf16x6 (three bf16 operand planes, 6 products, f32 accumulate)",
           "bf16x3": "bf16x3 (two bf16 operand planes, 3 products, f32 accumulate)", "bf16": "bf16"}
-ENGINES = {"fp32": "fp32 SIMT tap-GEMM", "fp16x3": "tcgen05 tap-GEMM, 3 fp16 products per fp32 product",
-           "bf16x6": "tcgen05 tap-GEMM, 6 bf16 products per fp32 product",
-           "bf16x3": "tcgen05 tap-GEMM, 3 bf16 products per fp32 product", "bf16": "tcgen05 tap-GEMM, plain bf16"}
+ENGINES = {"fp32": "fp32 SIMT tap-GEMM", "fp16x3": "wgmma tap-GEMM, 3 fp16 products per fp32 product",
+           "bf16x6": "wgmma tap-GEMM, 6 bf16 products per fp32 product",
+           "bf16x3": "wgmma tap-GEMM, 3 bf16 products per fp32 product", "bf16": "wgmma tap-GEMM, plain bf16"}
 MMA_PER_PRODUCT = {"fp32": 0, "bf16": 1, "bf16x3": 3, "bf16x6": 6, "fp16x3": 3}
-# dram__bytes_read.sum + dram__bytes_write.sum of ONE representative launch from a committed `ncu --set full` capture
-# (a static number, not measured in this run): precision -> (bytes, source file under profiles/)
-NCU_TRAFFIC = {"bf16x6": (26.4e6, "profiles/ncu_full_r1_final.md"),
-               "fp16x3": (8.711e6, "profiles/r2/ncu_full.md (8.711 MB read + 0 B written; algorithmic operand bytes 8.65 MB)")}
 METRIC = "motion_frames_per_sec"
 UNIT = "frames/s"
 
@@ -58,11 +58,12 @@ def _peaks():
         return dict(hbm=float(p["hbm_gbs"]), bf16=float(p["bf16_tflops"]),
                     bf16_sustained=float(p.get("bf16_tflops_sustained", p["bf16_tflops"])), source="measured")
     except Exception:
-        return dict(hbm=6650.0, bf16=1590.0, bf16_sustained=1400.0, source="fallback")
+        # NVIDIA H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16 - not measured here
+        return dict(hbm=3350.0, bf16=989.0, bf16_sustained=989.0, source="H100 SXM data sheet")
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled during the timed region (read-only queries)."""
 
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -239,6 +240,33 @@ def instrumented_gemm_pass(run_step, ops):
                 weight_bytes=sum(r[3] for r in records), wall_ms=1e3 * wall)
 
 
+DUMP_BUDGET = 64 << 20
+
+
+def dump_outputs(out_dir, dicts):
+    """Every tensor of {prefix: {key: tensor}} as out_dir/<prefix>_<key>.npy.  Floating tensors are written as float32,
+    integer ones as float64 (exact).  If the whole set exceeds DUMP_BUDGET, each array keeps the same fixed, seeded
+    sample of its leading-axis rows (sorted), so that two runs stay comparable element for element."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {}
+    for prefix, d in dicts.items():
+        for k, v in d.items():
+            if torch.is_tensor(v):
+                t = v.detach().cpu()
+                arrays[f"{prefix}_{k.lstrip('_')}"] = t.float().numpy() if t.is_floating_point() else t.double().numpy()
+    total = sum(a.nbytes for a in arrays.values())
+    budget = DUMP_BUDGET - 4096 * len(arrays)                 # room for the .npy headers
+    frac = min(1.0, budget / total) if total else 1.0
+    for name, a in sorted(arrays.items()):
+        if frac < 1.0 and a.ndim >= 1 and a.shape[0] > 1:
+            keep = max(1, int(a.shape[0] * frac))
+            rows = np.sort(np.random.default_rng(0).choice(a.shape[0], keep, replace=False))
+            a = a[rows]
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+
+
 def _device_time(fn, steps, warmup, flush=None):
     """ms per call of fn(): CUDA events around each call, `flush` (a > L2 buffer) rewritten between calls."""
     import torch
@@ -348,7 +376,7 @@ def run_gpu(args):
     clips = CLIPS_PER_GPU
     host_audio = torch.from_numpy(synth_audio(clips, N_SAMPLES, 1234 + rank)).pin_memory()
     audio = host_audio.to(dev)
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)      # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)      # > the 50 MB L2
     frames_per_step = clips * FRAMES_PER_CLIP
 
     def sync_all():
@@ -364,8 +392,8 @@ def run_gpu(args):
         if cap is not None:
             cap.graph.replay()
             ops.launch_count += cap.kernels_per_replay
-        else:
-            generate(model, vqm, audio)
+            return cap.latent, cap.pred
+        return generate(model, vqm, audio)
 
     def step_e2e():
         if cap is not None:
@@ -385,13 +413,17 @@ def run_gpu(args):
     starts = [torch.cuda.Event(enable_timing=True) for _ in range(args.steps)]
     ends = [torch.cuda.Event(enable_timing=True) for _ in range(args.steps)]
     sync_all()
+    last = None
     for i in range(args.steps):
         flush.fill_(i & 0xFF)                   # evict L2 between timed iterations (outside the bracket)
         starts[i].record()
-        step_resident()
+        last = step_resident()
         ends[i].record()
     sync_all()
     launches = ops.launch_count - launches0
+    if args.dump_outputs and rank == 0 and last is not None:
+        dump_outputs(args.dump_outputs, {"latent": last[0], "pred": last[1]})
+    del last
     dev_ms = sum(s.elapsed_time(e) for s, e in zip(starts, ends))
 
     # ---- e2e: pinned host audio -> H2D -> public API -> D2H of the emitted SMPL-X parameters ----
@@ -425,7 +457,6 @@ def run_gpu(args):
         inst = instrumented_gemm_pass(lambda: generate(model, vqm, audio), ops)
         achieved = inst["flop"] / (inst["ms"] * 1e-3) / 1e12 if inst["ms"] > 0 else 0.0
         peak = peaks["bf16_sustained"]
-        traffic = NCU_TRAFFIC.get(args.precision)
         # ---- VQ lookup kernel against HBM, >= 10^6 rows (SURVEY.md section 8d)
         sys.path.insert(0, os.path.join(ROOT, "tools"))
         try:
@@ -458,9 +489,6 @@ def run_gpu(args):
             "gpu_launches": launches,
             "roofline": {"bound": "tensor", "kernel": "tapgemm_tc_kernel (conv1d + linear), all launches of one step",
                          "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak,
-                         "traffic": traffic[0] if traffic else None,
-                         "traffic_source": (f"static: one representative launch (M=2048, N=K=768 trunk GEMM) of the committed "
-                                            f"ncu --set full capture {traffic[1]}, not measured in this run") if traffic else None,
                          "launches_per_step": inst["launches"], "kernel_ms_sum": inst["ms"],
                          "kernel_ms_regime": "eager single-stream pass, one CUDA-event pair per launch; its own wall time is "
                                              f"{inst['wall_ms']:.1f} ms.  The graph-replayed step overlaps the face / body / part branches "
@@ -469,7 +497,7 @@ def run_gpu(args):
                          "tensor_pipe_frac": achieved * MMA_PER_PRODUCT[args.precision] / peak,
                          "note": "achieved = algorithmic FLOP (2*rows*cout*cin*taps) / summed launch durations; "
                                  "tensor_pipe_frac counts the 1/3/6 MMAs issued per fp32 product",
-                         "peak_source": f"{peaks['source']} bf16 sustained (MEASURED_PEAKS.json)",
+                         "peak_source": f"{peaks['source']} bf16 (MEASURED_PEAKS.json when present)",
                          "step_frac": FLOP_PER_FRAME * value / world / (peak * 1e12)},
             "roofline_vq": roofline_vq,
             "cpu_baseline": cpu_line,
@@ -494,6 +522,8 @@ def main():
     ap.add_argument("--extra", type=int, default=1, help="0 skips the other BASELINE configs (bs 1, CaMN, DisCo)")
     ap.add_argument("--body-priority", type=int, default=1, help="capture the critical (body) chain on a high-priority stream")
     ap.add_argument("--graph", type=int, default=1, help="replay the step as one CUDA graph (1) or launch eagerly (0)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the last timed step's outputs as DIR/<name>.npy (float32 / float64, <= 64 MB in all)")
     args = ap.parse_args()
     if args.impl == "reference":
         run_reference(args)

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Audio folder -> BEAT-format npz with CaMN or DisCo on the B200 path (reference test_camn_audio.py / test_disco_audio.py).
+"""Audio folder -> BEAT-format npz with CaMN or DisCo on the H100 path (reference test_camn_audio.py / test_disco_audio.py).
 
     python examples/camn_disco_demo.py --model camn --checkpoint /path/to/camn_audio --audio_folder ./wavs
     python examples/camn_disco_demo.py --model disco --synthetic --audio_folder ./wavs

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Audio folder -> BEAT-format motion npz files: the reference demo (test_emage_audio.py:71-105) on the B200 path.
+"""Audio folder -> BEAT-format motion npz files: the reference demo (test_emage_audio.py:71-105) on the H100 path.
 
     python examples/emage_audio_demo.py --checkpoint /path/to/emage_audio --audio_folder ./wavs --save_folder ./out
     python examples/emage_audio_demo.py --synthetic --audio_folder ./wavs            # seeded random weights (no network)
@@ -17,7 +17,7 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-from models.emage_audio import EmageAudioModel, EmageVAEConv, EmageVQModel, EmageVQVAEConv  # noqa: E402  (B200 drop-in)
+from models.emage_audio import EmageAudioModel, EmageVAEConv, EmageVQModel, EmageVQVAEConv  # noqa: E402  (GPU drop-in)
 from pantomatrix_b200.audio_io import load_audio  # noqa: E402
 from pantomatrix_b200.motion_io import beat_format_save  # noqa: E402
 from pantomatrix_b200.pipeline import generate  # noqa: E402

@@ -1,4 +1,4 @@
-/* pm_emage.h - C ABI of libpm_emage.so: the B200 (sm_100a) kernels of the EMAGE audio->motion
+/* pm_emage.h - C ABI of libpm_emage.so: the H100 (sm_90a) kernels of the EMAGE audio->motion
  * inference hot path.
  *
  * The reference (PantoMatrix) has no FFI for this path: every op below is a stock torch.nn /
@@ -51,12 +51,12 @@ int pm_tapgemm_f32(const float* A, long long a_bs, int lda, int batch, int rows_
                    int act, float slope,
                    float* out, long long o_bs, int ldo, void* stream);
 
-/* ---- tap-GEMM on the tcgen05 tensor cores (split-bf16 operands, fp32 TMEM accumulate) -------------
+/* ---- tap-GEMM on the wgmma tensor cores (split-bf16 operands, fp32 register accumulate) ----------
  * Same contract as pm_tapgemm_f32 with stride == 1 (strided convs are passed as stride-1 problems over the
  * (rows/s, s*cin) view of the input with zero-padded taps).  A and W are `nsplit` bf16 planes (x = p0+p1+p2),
  * plane strides a_ps / w_ps elements: nsplit 1 = plain bf16, 2 = bf16x3 (p0*p0 + p0*p1 + p1*p0), 3 = bf16x6
  * (all products down to 2^-24).  W planes are (taps, w_rows, ldw) with w_rows >= cout a multiple of the N
- * tile (64 if cout <= 64 else 128), zero rows beyond cout.  lda, ldw, a_bs, a_ps, w_ps must be multiples
+ * tile (64), zero rows beyond cout.  lda, ldw, a_bs, a_ps, w_ps must be multiples
  * of 8 elements (TMA 16-byte rule).  The activation is applied to columns < act_cols only (<=0: all).
  * The epilogue writes the fp32 result and/or its bf16 split planes (out_f32 / out_bf16 nullable).
  * Operands are staged by TMA (cp.async.bulk.tensor, zero fill for padding rows, tap shift folded into the
@@ -104,10 +104,10 @@ int pm_attention_f32(const float* Q, int ldq, const float* K, int ldk, const flo
                      float* O, int ldo, int batch, int heads, int tq, int tk, int head_dim,
                      uint16_t* planes, long long p_ps, int p_ld, int p_nsplit, void* stream);
 
-/* Same op on the tcgen05 tensor cores for the fp16x3 engine: Q, K, V are two-plane fp16 activations (x = (p0+p1)/64,
+/* Same op on the wgmma tensor cores for the fp16x3 engine: Q, K, V are two-plane fp16 activations (x = (p0+p1)/64,
  * plane stride *_ps, clip stride *_bs, row stride ld* elements, *_cols valid columns; head h of Q starts at column
  * q_col0 + h*hd, likewise K and V - so the packed q|k|v projection output is consumed in place through TMA).
- * S = Q K^T and O = P V run as 3-product fp16 UMMAs (M=64) with S and O in TMEM, softmax in fp32 registers.
+ * S = Q K^T and O = P V run as 3-product fp16 wgmma (M=64) with S and O in registers, softmax in fp32 registers.
  * Output: fp32 O (nullable) and / or two fp16 planes (p_nsplit = 2 | PM_FMT_F16). */
 int pm_attention_tc(const uint16_t* Q, long long q_ps, long long q_bs, int ldq, int q_cols, int q_col0,
                     const uint16_t* K, long long k_ps, long long k_bs, int ldk, int k_cols, int k_col0,
@@ -140,7 +140,7 @@ int pm_window_input_f32(const float* motion, const float* mask, const float* see
 /* index = argmin_k ( |z|^2 + |e_k|^2 - 2 z.e_k ) evaluated in fp32, first minimum wins (a row of NaNs yields 0, like
  * torch.argmin): EmageVQVAEConv.decode_from_latent M.py:60-65, Quantizer.map2index P.py:158-164.
  * e2 = precomputed |e_k|^2 (n_codes).  Writes int64 indices.  e_dim must be 256.
- *   pm_l2_argmin_tc      n_codes == 256: persistent tcgen05 kernel - fp16 UMMA screen of all 256 scores per row with a
+ *   pm_l2_argmin_tc      n_codes == 256: persistent wgmma kernel - fp16 tensor-core screen of all 256 scores per row with a
  *                        rigorous error bound, exact fp32 re-scoring of every row whose best two screened distances
  *                        are within that bound; each z row is read from HBM once (1 KB + 8 B written per row).
  *                        max_ctas > 0 caps the persistent grid (<= 0: one CTA per SM).

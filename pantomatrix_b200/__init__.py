@@ -1,3 +1,3 @@
-"""pantomatrix_b200: B200-native (sm_100a) implementation of PantoMatrix's EMAGE audio->motion
+"""pantomatrix_b200: H100-native (sm_90a) implementation of PantoMatrix's EMAGE audio->motion
 inference hot path behind the reference's `models.emage_audio` module API."""
 __version__ = "0.1.0"

@@ -1,4 +1,4 @@
-"""In-tree nvcc build of libpm_emage.so (sm_100a only; the built .so travels to the GPU box).
+"""In-tree nvcc build of libpm_emage.so (sm_90a: H100).
 
     python -m pantomatrix_b200.build [--force]
     python -m pantomatrix_b200.build --variant NAME -DMACRO[=V] ...   # instrumented / tuning build, see build_variant()
@@ -15,7 +15,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "csrc", "_build")
 LIB = os.path.join(HERE, "libpm_emage.so")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 # per-file extra flags
 EXTRA = {"pm_pose.cu": ["-fmad=false"]}

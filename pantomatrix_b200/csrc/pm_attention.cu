@@ -1,6 +1,6 @@
 // Whole-sequence multi-head attention for the EMAGE transformer layers: fp32 SIMT kernel of the fp32 / bf16-plane
 // engines (the default fp16x3 engine runs attention on the tensor cores, pm_attention_tc.cu; an mma.sync 3xTF32
-// variant of this kernel measured 1.3 % faster per step in round 2 and was removed in favour of the tcgen05 kernel).
+// variant of this kernel measured 1.3 % faster per step in round 2 and was removed in favour of the tensor-core kernel).
 // T <= 64 tokens, head_dim = 192, no masks: the full score tile lives on chip, so there is no
 // online-softmax pass.  One CTA per (clip, head).  Contract: include/pm_emage.h (pm_attention_f32).
 #include <stdlib.h>

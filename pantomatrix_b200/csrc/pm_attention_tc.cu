@@ -1,18 +1,18 @@
-// Multi-head attention core on the tcgen05 tensor cores (T <= 64 tokens, head_dim 192, no masks): the whole
-// 64 x 64 score tile of one (clip, head) lives in TMEM, softmax runs in registers, P goes back through shared
-// memory as the A operand of the P.V product.  Contract: include/pm_emage.h (pm_attention_tc); replaces
+// Multi-head attention core on the Hopper tensor cores (wgmma; T <= 64 tokens, head_dim 192, no masks): the whole
+// 64 x 64 score tile of one (clip, head) is one warpgroup's register accumulator, softmax runs in registers, P goes
+// back through shared memory as the A operand of the P.V product.  Contract: include/pm_emage.h (pm_attention_tc); replaces
 // scaled_dot_product_attention inside nn.MultiheadAttention of every transformer layer (M.py:238-250).
 //
 // Operands are the two-plane fp16 activations of the fp16x3 engine (x = (p0 + p1) / 64, pm_common.cuh), written
 // by the producing GEMM's epilogue, so Q, K, V arrive by TMA straight from the packed q|k|v projection output:
-//   S  = Q K^T            3 products (p0 p0 + p0 p1 + p1 p0), UMMA M=64 N=64 K=16, A and B K-major (dims contiguous)
-//   P  = exp(S/sqrt(hd) - rowmax)   fp32 in registers (thread = query row), split into two fp16 planes of 1024 P
-//   O  = P V              3 products, UMMA M=64 N=192 K=16, B = V as stored (keys x dims): MN-major descriptor
+//   S  = Q K^T            3 products (p0 p0 + p0 p1 + p1 p0), wgmma m64n64k16, A and B K-major (dims contiguous)
+//   P  = exp(S/sqrt(hd) - rowmax)   fp32 in registers (quad of threads = query row), split into two fp16 planes of 1024 P
+//   O  = P V              3 products, wgmma m64n192k16, B = V as stored (keys x dims): MN-major descriptor
 //   out = O / (rowsum * 64 * 1024)  -> fp32 and / or fp16 planes for the out-projection GEMM
 // Accuracy is that of the GEMM engine (2^-22 relative per product), so the fp32 parity gates hold.
 //
-// One CTA per (clip, head), 160 threads: warps 0-3 = softmax / epilogue (TMEM lane quarter = warp, 16 rows each:
-// a 64-row accumulator occupies lanes 0-15 of every quarter), warp 4 = TMA producer + MMA issuer.
+// One CTA per (clip, head), one warpgroup (128 threads): one elected thread issues the TMA loads, the warpgroup issues
+// the MMAs, and each thread owns two query rows of the accumulators for softmax and epilogue.
 #include "pm_common.cuh"
 #include "pm_tc_ptx.cuh"
 #include "../../include/pm_emage.h"
@@ -23,7 +23,7 @@ constexpr int T = 64;                   // tokens per tile (queries and keys)
 constexpr int HD = 192;                 // head dim
 constexpr int KB = HD / 64;             // 64-column blocks per head
 constexpr int BLK = T * 128;            // bytes of one 64 x 64 fp16 block (128-byte rows, 128B swizzle): 8 KB
-constexpr int NTHREADS = 160;
+constexpr int NTHREADS = 128;
 constexpr float P_SCALE = 1024.f;       // probabilities are split as fp16 planes of 1024 * p (second plane stays normal)
 
 struct Smem {
@@ -31,9 +31,8 @@ struct Smem {
   static constexpr int K = Q + 2 * KB * BLK;
   static constexpr int V = K + 2 * KB * BLK;
   static constexpr int P = V + 2 * KB * BLK;           // [2 planes] one block each
-  static constexpr int BARS = P + 2 * BLK;             // qk_full[KB], v_full, s_full, p_full, o_full
-  static constexpr int MISC = BARS + (KB + 4) * 8;
-  static constexpr int TOTAL = MISC + 16;
+  static constexpr int BARS = P + 2 * BLK;             // qk_full[KB], v_full
+  static constexpr int TOTAL = BARS + (KB + 1) * 8;
 };
 
 // Instrumented build only (-DPM_ATTN_TIMING, tools/bench_attention.py --timeline): clock64 stamps of CTA 0's phases.
@@ -52,16 +51,6 @@ struct AttnParams {
   PmPlanes planes;                      // fp16 planes of the output or ptr == null
 };
 
-__device__ __forceinline__ void tmem_ld64(uint32_t taddr, uint32_t (&r)[64]) {
-  uint32_t(&a)[32] = *reinterpret_cast<uint32_t(*)[32]>(&r[0]);
-  uint32_t(&b)[32] = *reinterpret_cast<uint32_t(*)[32]>(&r[32]);
-  tmem_ld32(taddr, a);
-  tmem_ld32(taddr + 32, b);
-}
-__device__ __forceinline__ void sts128u(uint32_t addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
-  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(a), "r"(b), "r"(c), "r"(d) : "memory");
-}
-
 __global__ void __launch_bounds__(NTHREADS, 1) attention_tc_kernel(const __grid_constant__ CUtensorMap map_q,
                                                                    const __grid_constant__ CUtensorMap map_k,
                                                                    const __grid_constant__ CUtensorMap map_v,
@@ -70,8 +59,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) attention_tc_kernel(const __grid_
   uint8_t* sm = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const uint32_t sm_u = smem_u32(sm);
   const uint32_t bars = sm_u + Smem::BARS;
-  const uint32_t qk_full = bars, v_full = bars + 8 * KB, s_full = v_full + 8, p_full = v_full + 16, o_full = v_full + 24;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(sm + Smem::MISC);
+  const uint32_t qk_full = bars, v_full = bars + 8 * KB;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int b = blockIdx.x / p.heads, h = blockIdx.x % p.heads;
   if (warp == 0) AT_STAMP(0);                              // kernel entry
@@ -79,29 +67,17 @@ __global__ void __launch_bounds__(NTHREADS, 1) attention_tc_kernel(const __grid_
   if (threadIdx.x == 0) {
     for (int kb = 0; kb < KB; ++kb) mbar_init(qk_full + 8 * kb, 1);
     mbar_init(v_full, 1);
-    mbar_init(s_full, 1);
-    mbar_init(p_full, 4);
-    mbar_init(o_full, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 4) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(256) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tmem_s = tmem_base, tmem_o = tmem_base + 64;
   if (warp == 0) AT_STAMP(1);                              // prologue done
-
-  if (warp == 4) {
-    // ===== TMA producer + MMA issuer =====
+  if (warp == 0) {
+    // ===== TMA: one barrier per 64-column block, so the first MMAs start on a third of Q, K =====
     if (elect_one()) {
       asm volatile("prefetch.tensormap [%0];" ::"l"(&map_q) : "memory");
       asm volatile("prefetch.tensormap [%0];" ::"l"(&map_k) : "memory");
       asm volatile("prefetch.tensormap [%0];" ::"l"(&map_v) : "memory");
-      for (int kb = 0; kb < KB; ++kb) {                   // one barrier per 64-column block: the first MMAs start on a third of Q, K
+      for (int kb = 0; kb < KB; ++kb) {
         mbar_expect_tx(qk_full + 8 * kb, 4 * BLK);
         for (int pl = 0; pl < 2; ++pl) {
           tma_load_4d(sm_u + Smem::Q + (pl * KB + kb) * BLK, &map_q, qk_full + 8 * kb, p.qc0 + h * HD + kb * 64, 0, b, pl);
@@ -114,170 +90,142 @@ __global__ void __launch_bounds__(NTHREADS, 1) attention_tc_kernel(const __grid_
           tma_load_4d(sm_u + Smem::V + (pl * KB + nb) * BLK, &map_v, v_full, p.vc0 + h * HD + nb * 64, 0, b, pl);
     }
     __syncwarp();
-    // ---- S = Q K^T : D = f32, A = B = f16, both K-major, N = 64, M = 64
-    {
-      constexpr uint32_t IDESC_S = (1u << 4) | ((uint32_t)(T >> 3) << 17) | ((uint32_t)(T >> 4) << 24);
-      const uint64_t q0 = UMMA_DESC_K_SW128 | (uint64_t)(((sm_u + Smem::Q) >> 4) & 0x3FFFu);
-      const uint64_t k0 = UMMA_DESC_K_SW128 | (uint64_t)(((sm_u + Smem::K) >> 4) & 0x3FFFu);
-      constexpr uint64_t PL = (uint64_t)(KB * BLK) >> 4, KBS = (uint64_t)BLK >> 4;
-      // per block: cross products first (small), the main product last: (A plane, B plane) = (0,1), (1,0), (0,0)
-      const int pa[3] = {0, 1, 0}, pb[3] = {1, 0, 0};
-      uint32_t acc = 0;
-#pragma unroll
-      for (int kb = 0; kb < KB; ++kb) {
-        mbar_wait(qk_full + 8 * kb, 0);
-        tc_fence_after();
-        AT_STAMP(8 + kb);                                  // Q | K block kb landed
-        if (elect_one()) {
-#pragma unroll
-          for (int t = 0; t < 3; ++t)
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              tc_mma_bf16(tmem_s, q0 + pa[t] * PL + kb * KBS + k * 2, k0 + pb[t] * PL + kb * KBS + k * 2, IDESC_S, acc);
-              acc = 1;
-            }
-          if (kb == KB - 1) tc_commit(s_full);
-        }
-        __syncwarp();
-      }
-    }
-    // ---- O = P V : B = V as stored, (keys x dims) = MN-major: 64-dim groups 8 KB apart (LBO), 8-key groups 1 KB (SBO)
-    mbar_wait(v_full, 0);
-    mbar_wait(p_full, 0);
-    tc_fence_after();
-    if (elect_one()) {
-      constexpr uint32_t IDESC_O = (1u << 4) | (1u << 16) | ((uint32_t)(HD >> 3) << 17) | ((uint32_t)(T >> 4) << 24);
-      constexpr uint64_t DESC_MN = ((uint64_t)(BLK >> 4) << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) | (2ull << 61);
-      const uint64_t p0 = UMMA_DESC_K_SW128 | (uint64_t)(((sm_u + Smem::P) >> 4) & 0x3FFFu);
-      const uint64_t v0 = DESC_MN | (uint64_t)(((sm_u + Smem::V) >> 4) & 0x3FFFu);
-      constexpr uint64_t PPL = (uint64_t)BLK >> 4, VPL = (uint64_t)(KB * BLK) >> 4;
-      const int pa[3] = {0, 1, 0}, pb[3] = {1, 0, 0};
-      uint32_t acc = 0;
-#pragma unroll
-      for (int t = 0; t < 3; ++t)
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {       // 16 keys per step: A advances 32 B inside the swizzled row, B by two 8-key groups
-          tc_mma_bf16(tmem_o, p0 + pa[t] * PPL + k * 2, v0 + pb[t] * VPL + k * (2048 >> 4), IDESC_O, acc);
-          acc = 1;
-        }
-      tc_commit(o_full);
-    }
-    __syncwarp();
-  } else {
-    // ===== softmax + epilogue: warp w owns query rows 16 w .. 16 w + 15 (TMEM lanes 32 w + 0..15) =====
-    const int row = warp * 16 + (lane & 15);
-    const bool active = lane < 16;
-    const uint32_t lane_addr = (uint32_t)(warp * 32) << 16;
-    float inv = 0.f;
-    {
-      mbar_wait(s_full, 0);
-      tc_fence_after();
-      if (warp == 0) AT_STAMP(2);                          // S complete
-      uint32_t sr[64];
-      tmem_ld64(tmem_s + lane_addr, sr);
-      // exp(s - m) = 2^((s - m) log2 e): log2 e is folded into the scale and the exponential is one MUFU.EX2
-      // (2 ulp); expf() costs ~25 instructions per element on 16 active lanes - the softmax was 5 400 of the kernel's
-      // 20 000 cycles (profiles/r2/attention_timeline.md)
-      const float sl2 = p.scale * 1.4426950408889634f;
-      float m = -INFINITY;
-#pragma unroll
-      for (int j = 0; j < 64; ++j) {
-        const float v = j < p.tk ? __uint_as_float(sr[j]) * sl2 : -INFINITY;
-        sr[j] = __float_as_uint(v);
-        m = fmaxf(m, v);
-      }
-      float sum = 0.f;
-#pragma unroll
-      for (int j = 0; j < 64; ++j) {
-        float e = 0.f;
-        if (j < p.tk) asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(__uint_as_float(sr[j]) - m));
-        sum += e;
-        sr[j] = __float_as_uint(e * P_SCALE);
-      }
-      inv = 1.f / (sum * (P_SCALE * PM_F16_ACT_SCALE));
-      if (active) {
-        const uint32_t dst = sm_u + Smem::P + (row >> 3) * 1024 + (row & 7) * 128;
-#pragma unroll
-        for (int c = 0; c < 8; ++c) {       // 8 keys per 16-byte chunk, two planes
-          uint32_t hi[4], lo[4];
-#pragma unroll
-          for (int u = 0; u < 4; ++u) {
-            const float a0 = __uint_as_float(sr[8 * c + 2 * u]), a1 = __uint_as_float(sr[8 * c + 2 * u + 1]);
-            const float f0 = pm_f16_head(a0), f1 = pm_f16_head(a1);       // exact in fp16: no conversion back (pm_common.cuh)
-            const __half2 h0 = __floats2half2_rn(f0, f1);
-            const __half2 h1 = __floats2half2_rn(a0 - f0, a1 - f1);
-            hi[u] = *reinterpret_cast<const uint32_t*>(&h0);
-            lo[u] = *reinterpret_cast<const uint32_t*>(&h1);
-          }
-          const uint32_t off = (uint32_t)((c ^ (row & 7)) << 4);
-          sts128u(dst + off, hi[0], hi[1], hi[2], hi[3]);
-          sts128u(dst + BLK + off, lo[0], lo[1], lo[2], lo[3]);
-        }
-      }
-      fence_proxy_async_smem();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(p_full);
-      if (warp == 0) AT_STAMP(3);                          // softmax done, P stored
-    }
-    // ---- O: normalise and write straight from registers (thread = query row): 16-byte vectors per plane / float4 for
-    // fp32.  (Staging the tile in shared memory and copying it out row-contiguously cost 9 600 of 20 000 cycles.)
-    mbar_wait(o_full, 0);
-    tc_fence_after();
-    if (warp == 0) AT_STAMP(4);                            // O complete
-    const bool live = active && row < p.tq;
-    const long long grow = (long long)b * p.tq + row;
-    const bool vec16 = p.planes.ptr && ((p.planes.ld & 7) == 0) && ((p.planes.ps & 7) == 0) &&
-                       ((reinterpret_cast<uintptr_t>(p.planes.ptr) & 15) == 0);
-    __half* const prow = reinterpret_cast<__half*>(p.planes.ptr) + grow * p.planes.ld + h * HD;
-    float* const frow = p.out ? p.out + grow * p.ldo + h * HD : nullptr;
-#pragma unroll 1
-    for (int c0 = 0; c0 < HD; c0 += 64) {
-      uint32_t orr[64];
-      tmem_ld64(tmem_o + lane_addr + c0, orr);
-      if (live) {
-#pragma unroll
-        for (int g8 = 0; g8 < 8; ++g8) {                   // 8 consecutive columns
-          float x[8];
-#pragma unroll
-          for (int u = 0; u < 8; ++u) x[u] = __uint_as_float(orr[8 * g8 + u]) * inv;
-          if (frow) {
-            *reinterpret_cast<float4*>(frow + c0 + 8 * g8) = make_float4(x[0], x[1], x[2], x[3]);
-            *reinterpret_cast<float4*>(frow + c0 + 8 * g8 + 4) = make_float4(x[4], x[5], x[6], x[7]);
-          }
-          if (p.planes.ptr) {
-            if (vec16) {
-              uint32_t h0[4], h1[4];
-#pragma unroll
-              for (int u = 0; u < 4; ++u) {
-                const float a0 = x[2 * u] * PM_F16_ACT_SCALE, a1 = x[2 * u + 1] * PM_F16_ACT_SCALE;
-                const float f0 = pm_f16_head(a0), f1 = pm_f16_head(a1);
-                const __half2 t0 = __floats2half2_rn(f0, f1);
-                const __half2 t1 = __floats2half2_rn(a0 - f0, a1 - f1);
-                h0[u] = *reinterpret_cast<const uint32_t*>(&t0);
-                h1[u] = *reinterpret_cast<const uint32_t*>(&t1);
-              }
-              *reinterpret_cast<uint4*>(prow + c0 + 8 * g8) = make_uint4(h0[0], h0[1], h0[2], h0[3]);
-              if (p.planes.nsplit > 1) *reinterpret_cast<uint4*>(prow + p.planes.ps + c0 + 8 * g8) = make_uint4(h1[0], h1[1], h1[2], h1[3]);
-            } else {
-#pragma unroll
-              for (int u = 0; u < 8; ++u) pm_store_planes_t<true>(p.planes, grow, h * HD + c0 + 8 * g8 + u, x[u]);
-            }
-          }
-        }
-      }
-    }
-    if (warp == 0) AT_STAMP(5);
   }
 
-  if (warp == 0) AT_STAMP(6);                              // outputs written
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) AT_STAMP(7);
-  if (warp == 4) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(256) : "memory");
+  // Fragment of this thread (pm_tc_ptx.cuh): query rows r0 = 16 warp + lane / 4 and r0 + 8; columns 8 i + 2 (lane % 4).
+  const int r0 = warp * 16 + (lane >> 2), t2 = 2 * (lane & 3);
+  // per block: cross products first (small), the main product last: (A plane, B plane) = (0,1), (1,0), (0,0)
+  const int pa[3] = {0, 1, 0}, pb[3] = {1, 0, 0};
+
+  // ---- S = Q K^T : A = Q, B = K, both K-major (dims contiguous), M = N = 64
+  float sr[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) sr[i] = 0.f;
+#pragma unroll
+  for (int kb = 0; kb < KB; ++kb) {
+    mbar_wait(qk_full + 8 * kb, 0);
+    if (warp == 0) AT_STAMP(8 + kb);                       // Q | K block kb landed
+    wgmma_fence();
+#pragma unroll
+    for (int t = 0; t < 3; ++t)
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        wgmma_m64n64k16<false>(sr, gmma_desc(GMMA_DESC_K_SW128, sm_u + Smem::Q + (pa[t] * KB + kb) * BLK + 32 * k),
+                               gmma_desc(GMMA_DESC_K_SW128, sm_u + Smem::K + (pb[t] * KB + kb) * BLK + 32 * k));
+    wgmma_commit();
   }
+  wgmma_wait<0>();
+  wgmma_fence_regs(sr);
+  if (warp == 0) AT_STAMP(2);                              // S complete
+
+  // ---- softmax in registers.  exp(s - m) = 2^((s - m) log2 e): log2 e is folded into the scale and the exponential
+  // is one MUFU.EX2 (2 ulp).  A row is spread over the four lanes of a quad: max and sum are reduced by two shuffles.
+  float inv[2];
+  {
+    const float sl2 = p.scale * 1.4426950408889634f;
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) {
+      float m = -INFINITY;
+#pragma unroll
+      for (int i = 0; i < 8; ++i)
+#pragma unroll
+        for (int u = 0; u < 2; ++u) {
+          const int j = 8 * i + t2 + u;
+          const float v = j < p.tk ? sr[4 * i + 2 * hr + u] * sl2 : -INFINITY;
+          sr[4 * i + 2 * hr + u] = v;
+          m = fmaxf(m, v);
+        }
+      m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 1));
+      m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, 2));
+      float sum = 0.f;
+#pragma unroll
+      for (int i = 0; i < 8; ++i)
+#pragma unroll
+        for (int u = 0; u < 2; ++u) {
+          const int j = 8 * i + t2 + u;
+          float e = 0.f;
+          if (j < p.tk) asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(sr[4 * i + 2 * hr + u] - m));
+          sum += e;
+          sr[4 * i + 2 * hr + u] = e * P_SCALE;
+        }
+      sum += __shfl_xor_sync(0xffffffffu, sum, 1);
+      sum += __shfl_xor_sync(0xffffffffu, sum, 2);
+      inv[hr] = 1.f / (sum * (P_SCALE * PM_F16_ACT_SCALE));
+    }
+    // P as two fp16 planes, K-major 128B-swizzled (query row = 128-byte row of 64 keys): the A operand of P V
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) {
+      const int row = r0 + 8 * hr;
+      const uint32_t dst = sm_u + Smem::P + (row >> 3) * 1024 + (row & 7) * 128;
+#pragma unroll
+      for (int i = 0; i < 8; ++i) {        // keys 8 i + t2, + 1: one 4-byte pair inside 16-byte chunk i
+        const float a0 = sr[4 * i + 2 * hr], a1 = sr[4 * i + 2 * hr + 1];
+        const float f0 = pm_f16_head(a0), f1 = pm_f16_head(a1);       // exact in fp16: no conversion back (pm_common.cuh)
+        const __half2 h0 = __floats2half2_rn(f0, f1);
+        const __half2 h1 = __floats2half2_rn(a0 - f0, a1 - f1);
+        const uint32_t off = (uint32_t)(((i ^ (row & 7)) << 4) + 2 * t2);
+        asm volatile("st.shared.b32 [%0], %1;" ::"r"(dst + off), "r"(*reinterpret_cast<const uint32_t*>(&h0)) : "memory");
+        asm volatile("st.shared.b32 [%0], %1;" ::"r"(dst + BLK + off), "r"(*reinterpret_cast<const uint32_t*>(&h1)) : "memory");
+      }
+    }
+    fence_proxy_async_smem();
+    __syncthreads();
+    if (warp == 0) AT_STAMP(3);                            // softmax done, P stored
+  }
+
+  // ---- O = P V : B = V as stored, (keys x dims) = MN-major: 64-dim blocks 8 KB apart (LBO), 8-key groups 1 KB (SBO)
+  float orr[96];
+#pragma unroll
+  for (int i = 0; i < 96; ++i) orr[i] = 0.f;
+  mbar_wait(v_full, 0);
+  wgmma_fence();
+  {
+    constexpr uint64_t DESC_MN = gmma_desc_mn_sw128(BLK);
+#pragma unroll
+    for (int t = 0; t < 3; ++t)
+#pragma unroll
+      for (int k = 0; k < 4; ++k)        // 16 keys per step: A advances 32 B inside the swizzled row, B by two 8-key groups
+        wgmma_m64n192k16<false, 1>(orr, gmma_desc(GMMA_DESC_K_SW128, sm_u + Smem::P + pa[t] * BLK + 32 * k),
+                                   gmma_desc(DESC_MN, sm_u + Smem::V + pb[t] * KB * BLK + 2048 * k));
+  }
+  wgmma_commit();
+  wgmma_wait<0>();
+  wgmma_fence_regs(orr);
+  if (warp == 0) AT_STAMP(4);                              // O complete
+
+  // ---- normalise and write straight from registers: 2 consecutive columns per store
+  const bool pair_ok = p.planes.ptr && ((p.planes.ld & 1) == 0) && ((p.planes.ps & 1) == 0) &&
+                       ((reinterpret_cast<uintptr_t>(p.planes.ptr) & 3) == 0);
+#pragma unroll
+  for (int hr = 0; hr < 2; ++hr) {
+    const int row = r0 + 8 * hr;
+    if (row >= p.tq) continue;
+    const long long grow = (long long)b * p.tq + row;
+    __half* const prow = reinterpret_cast<__half*>(p.planes.ptr) + grow * p.planes.ld + h * HD;
+    float* const frow = p.out ? p.out + grow * p.ldo + h * HD : nullptr;
+#pragma unroll
+    for (int i = 0; i < HD / 8; ++i) {
+      const int c = 8 * i + t2;
+      const float x0 = orr[4 * i + 2 * hr] * inv[hr], x1 = orr[4 * i + 2 * hr + 1] * inv[hr];
+      if (frow) *reinterpret_cast<float2*>(frow + c) = make_float2(x0, x1);
+      if (p.planes.ptr) {
+        if (pair_ok) {
+          const float a0 = x0 * PM_F16_ACT_SCALE, a1 = x1 * PM_F16_ACT_SCALE;
+          const float f0 = pm_f16_head(a0), f1 = pm_f16_head(a1);
+          *reinterpret_cast<__half2*>(prow + c) = __floats2half2_rn(f0, f1);
+          if (p.planes.nsplit > 1) *reinterpret_cast<__half2*>(prow + p.planes.ps + c) = __floats2half2_rn(a0 - f0, a1 - f1);
+        } else {
+          pm_store_planes_t<true>(p.planes, grow, h * HD + c, x0);
+          pm_store_planes_t<true>(p.planes, grow, h * HD + c + 1, x1);
+        }
+      }
+    }
+  }
+  if (warp == 0) AT_STAMP(5);                              // outputs written
+#ifdef PM_ATTN_TIMING
+  __syncthreads();
+#endif
+  if (warp == 0) AT_STAMP(7);                              // all warps done
 }
 
 constexpr size_t kSmem = Smem::TOTAL + 1024;

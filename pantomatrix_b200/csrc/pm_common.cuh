@@ -1,4 +1,4 @@
-// Shared helpers for the EMAGE hot-path kernels (sm_100a only).
+// Shared helpers for the EMAGE hot-path kernels (sm_90a).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -53,7 +53,7 @@ __device__ __forceinline__ float pm_warp_max(float v) {
   return v;
 }
 
-// ---- split-bf16 planes (operands of the tcgen05 engine): x ~ p0 + p1 + p2, round-to-nearest each ----
+// ---- split-bf16 planes (operands of the tensor-core engine): x ~ p0 + p1 + p2, round-to-nearest each ----
 struct PmPlanes {
   __nv_bfloat16* ptr;   // plane 0, element (row 0, channel 0); nullptr = no plane output
   long long ps;         // plane stride (elements)
@@ -71,14 +71,13 @@ __device__ __forceinline__ void pm_split3(float v, __nv_bfloat16 (&p)[3]) {
 
 // Plane element format.  bf16 (default) needs 3 planes / 6 products for an fp32-quality GEMM; IEEE fp16 reaches the
 // same accuracy with 2 planes / 3 products (11-bit mantissas) as long as magnitudes stay below 65504 - an overflow
-// turns into inf - inf = NaN in the consumer GEMM and is caught by the host (profiles/split_formats_r1.json).
+// turns into inf - inf = NaN in the consumer GEMM and is caught by the host.
 // Callers select it with bit 8 of an `nsplit` argument of the C ABI.
 #ifndef PM_FMT_F16
 #define PM_FMT_F16 0x100
 #endif
-// fp16 activation planes hold PM_F16_ACT_SCALE * x.  Measured on B200 (round 2): tcgen05.mma kind::f16 FLUSHES fp16
-// subnormal operands, so the second plane of an element below 2^-3 (|p1| < 2^-14) would be lost; the exact pre-scale
-// moves that threshold to 2^-9 (absolute error <= 2^-21 per element) and the overflow threshold to 65504 / 64 = 1023.
+// fp16 activation planes hold PM_F16_ACT_SCALE * x.  The second plane of an element below 2^-3 would be an fp16
+// subnormal (|p1| < 2^-14), which tensor cores may flush; the exact pre-scale moves that threshold to 2^-9 (absolute error <= 2^-21 per element) and the overflow threshold to 65504 / 64 = 1023.
 // The packed weights' acc_scale carries the matching 1 / 64 (ops.PackedW), so GEMM results are unchanged.
 #define PM_F16_ACT_SCALE 64.0f
 // host side: strip the format bit of an `nsplit` ABI argument into a flag
@@ -90,8 +89,7 @@ __device__ __forceinline__ void pm_split3(float v, __nv_bfloat16 (&p)[3]) {
 // Plane 0 is formed with integer ops on the fp32 bit pattern (add half an ulp of the 10-bit mantissa, clear the 13 low
 // bits: round-half-away, exponent carry included) - the result is exactly representable in fp16, so its conversion is
 // exact and the remainder v - f0 needs no conversion BACK from fp16.  Those back-conversions run at a fraction of the
-// FP32 rate and made every plane-writing epilogue conversion-bound (GEMM epilogue 7 500 cycles with planes against
-// 5 000 without, profiles/r2/gemm_timeline_fp16.txt).  (Below 2^-14 plane 0 would be an fp16 subnormal, which the
+// FP32 rate and would make every plane-writing epilogue conversion-bound.  (Below 2^-14 plane 0 would be an fp16 subnormal, which the
 // tensor core flushes anyway.)
 __device__ __forceinline__ float pm_f16_head(float v) {
   return __uint_as_float((__float_as_uint(v) + 0x00001000u) & 0xFFFFE000u);

@@ -1,19 +1,19 @@
-// tcgen05 tap-GEMM: Conv1d (stride 1, any taps / zero padding) and Linear on the Blackwell tensor cores.
+// Hopper tap-GEMM: Conv1d (stride 1, any taps / zero padding) and Linear on the sm_90a tensor cores (wgmma).
 //
 //   out[b,l,n] = act( bias[n] + sum_t sum_c A[b, l+t-pad, c] * W[t,n,c] + residual[b,l,n] )
 //
 // Operands are split-bf16 planes (x ~ p0 + p1 + p2, each plane bf16): nsplit 1 = plain bf16, 2 = bf16x3
-// (p0*p0 + p0*p1 + p1*p0), 3 = bf16x6 (every product down to 2^-24): all products accumulate in one fp32
-// TMEM accumulator, so the result has fp32-grade accuracy at tensor-core rates.
+// (p0*p0 + p0*p1 + p1*p0), 3 = bf16x6 (every product down to 2^-24): all products accumulate in fp32 registers, so
+// the result has fp32-grade accuracy at tensor-core rates.
 //
-// Structure (one 128 x BN output tile per CTA, 320 threads):
-//   warp 0   TMA producer  - cp.async.bulk.tensor: A box (64 ch x R rows x NB clips) per plane, with the tap
-//                            shift folded into the row coordinate (im2col-free; padding rows are TMA zero fill),
-//                            W box (64 ch x BN rows) per plane; 128B-swizzled K-major smem tiles; mbarrier ring
-//   warp 1   MMA issuer    - one elected lane issues tcgen05.mma.cta_group::1.kind::f16 (M=128, N=BN, K=16),
-//                            tcgen05.commit releases smem stages / publishes the accumulator; owns TMEM alloc
-//   warps 2-9 epilogue     - tcgen05.ld (32 lanes x 32 columns) -> smem transpose -> bias / residual /
-//                            activation -> coalesced fp32 store and/or bf16 split planes for the next GEMM
+// Structure (one 128 x BN output tile per CTA, 288 threads):
+//   warps 0-7  two consumer warpgroups - warpgroup g issues wgmma.m64nBNk16 for tile rows 64 g .. 64 g + 63 out of
+//                                        the shared operand stage, then runs the epilogue: registers -> smem tile ->
+//                                        bias / residual / activation -> coalesced fp32 store and/or split planes
+//   warp 8     TMA producer             - cp.async.bulk.tensor: A box (64 ch x R rows x NB clips) per plane, with the
+//                                        tap shift folded into the row coordinate (im2col-free; padding rows are TMA
+//                                        zero fill), W box (64 ch x 64 rows) per plane; 128B-swizzled K-major smem
+//                                        tiles; mbarrier ring
 // Contract and reference call sites: include/pm_emage.h (pm_tapgemm_tc).
 #include <cuda.h>
 #include <stdio.h>
@@ -26,15 +26,14 @@
 
 namespace {
 
-constexpr int BM = 128;             // tile rows (UMMA M)
+constexpr int BM = 128;             // tile rows (two 64-row warpgroups)
 constexpr int BK = 64;              // bf16 channels per k-block = one 128-byte swizzle row
-constexpr int UMMA_K = 16;
+constexpr int MMA_K = 16;
 constexpr int A_TILE_BYTES = BM * BK * 2;           // 16 KB per plane
-constexpr int NUM_THREADS = 320;   // TMA warp, MMA warp, 8 epilogue warps
+constexpr int CONSUMER_THREADS = 256;
+constexpr int NUM_THREADS = CONSUMER_THREADS + 32;  // two consumer warpgroups + the TMA warp
 constexpr int MAX_STAGES = 8;
-constexpr int OCC2_SMEM_KB = 100;   // operand ring per CTA when two CTAs share an SM (2 x (100 + 1.2) KB < 227 KB)
-constexpr int HALO_ROWS = 144;      // halo mode: 128 output rows + up to 16 neighbours, whole 8-row swizzle groups
-constexpr int HALO_BYTES = HALO_ROWS * BK * 2;      // 18 KB per plane
+constexpr int RING_KB = 200;        // operand ring per CTA (one CTA per SM; 227 KB is the sm_90 limit)
 
 struct TcParams {
   int taps, pad, nsplit, kblocks;   // kblocks = ceil(cin / 64)
@@ -65,58 +64,56 @@ __device__ unsigned long long pm_tc_stamps[4096 * 8];
 #define PM_STAMP(i) do {} while (0)
 #endif
 
-#include "pm_tc_ptx.cuh"   // PTX wrappers: mbarrier, TMA, tcgen05
+#include "pm_tc_ptx.cuh"   // PTX wrappers: mbarrier, TMA, wgmma
 
-// ---------------------------------------------------------------------------------------------------
-// CG2 = the CTA-pair form (tcgen05 cta_group::2): two CTAs of a 2-CTA cluster, neighbours along the row-tile axis, work
-// on one 256 x BN tile.  Each keeps its own 128 rows of A and its 128 x BN accumulators, but only HALF of the W tile
-// (BN / 2 weight rows); the leader's MMAs (M = 256) read both halves.  Why: with two fp16 planes a k-block brings
-// 64 KB into shared memory for 12 MMAs of 64 cycles - 83 B / cycle against the ~64 B / cycle an SM can take in from
-// L2, so the single-CTA mainloop is fill-bound (1 058 cycles per k-block instead of 768, profiles/r2/gemm_timeline_fp16.txt);
-// the pair needs 48 KB per CTA and k-block.
-//
-// OCC = CTAs per SM the kernel is compiled for.  2 (64-column tiles only: 256 TMEM columns, 96 registers, half the operand
-// ring) is for launches of many short tiles - the WavEncoder's 64-channel convs: 7 552 tiles of 15 k-blocks, where one
-// resident CTA spent more time in prologue, pipeline fill and epilogue than in its mainloop (13 us per tile against
-// 5.7 us of operand fill, profiles/r2/launches_fp16x3.md); with two, one CTA's epilogue overlaps the other's mainloop.
-//
-// HALO = one-k-block convs (cin <= 64) with several taps.  The tap-GEMM above re-stages the A tile for every tap although
-// consecutive taps read the same rows shifted by one: 15 x 32 KB of shared-memory fill per tile of the WavEncoder's
-// k = 15 convs, which made them fill-bound.  In halo mode the 128 + taps - 1 input rows of the tile are staged ONCE per
-// plane and tap t reads them through a descriptor whose start address is advanced by t rows (t x 128 B).  Measured on
-// B200 (profiles/r2/halo_mode_trial.md): the tensor core derives the 128B-swizzle phase from the ADDRESS bits 7-9, so a
-// start address that is not 1024-byte aligned needs nothing else - the descriptor's base-offset field must stay 0 (with
-// (start >> 7) & 7 in it, as the PTX text suggests for unaligned starts, every result was wrong).  Only the 8 KB W tiles
-// stream through the ring.  WavEncoder 64 -> 64, k = 15 conv over 0.97 M rows: 444 -> 420 us.
-template <int BN, bool F16, bool CG2, int OCC = 1, bool HALO = false>
-__global__ void __launch_bounds__(NUM_THREADS, OCC) tapgemm_tc_kernel(const __grid_constant__ CUtensorMap map_a,
-                                                                    const __grid_constant__ CUtensorMap map_w,
-                                                                    const TcParams p) {
-  constexpr int W_ROWS_CTA = CG2 ? BN / 2 : BN;     // weight rows this CTA stages per k-block and plane
-  constexpr int W_TILE_BYTES = W_ROWS_CTA * BK * 2;
-  // instruction descriptor: D = f32; A and B format field 1 = bf16, 0 = fp16; K-major A and B; N >> 3; M >> 4
-  constexpr uint32_t IDESC = (1u << 4) | (F16 ? 0u : ((1u << 7) | (1u << 10))) | ((uint32_t)(BN >> 3) << 17) |
-                             ((uint32_t)((CG2 ? 2 * BM : BM) >> 4) << 24);
-  // Three fp32 accumulators in TMEM: two "main" ones that take the p0*p0 products of alternate k-iterations
-  // and one "correction" accumulator for every cross product.  The tensor core aligns and TRUNCATES addends to
-  // the accumulator's exponent on every MMA, a biased error ~2^-25 |acc| per instruction; keeping the 2^-8-scaled
-  // cross terms apart and halving the chain length of the main sums brings the result back to fp32-FMA quality.
-  // The epilogue adds the three in fp32.
-  constexpr int TMEM_COLS = BN == 64 ? 256 : 512;   // 3 accumulators rounded up to a power of two
-  constexpr int ACC = BN;                           // column stride between the accumulators
+template <int BN, bool F16>
+__device__ __forceinline__ void mma_k16(float (&d)[BN / 2], uint64_t a, uint64_t b) {
+  static_assert(BN == 64, "64-column tiles (see pm_tapgemm_tc)");
+  wgmma_m64n64k16<!F16>(d, a, b);
+}
+
+// Three fp32 accumulators: two "main" ones that take the p0*p0 products of alternate k-iterations and one
+// "correction" accumulator for every cross product.  The tensor core aligns and truncates addends to the
+// accumulator's exponent, a biased error ~2^-25 |acc| per instruction; keeping the 2^-8-scaled cross terms apart and
+// halving the chain length of the main sums keeps the result at fp32-FMA quality.  The epilogue adds the three.
+template <int BN, bool F16, int NSPLIT>
+__device__ __forceinline__ void mma_kblock(float (&main)[BN / 2], float (&corr)[BN / 2], uint64_t a0, uint64_t w0) {
+  constexpr uint64_t A_PL = A_TILE_BYTES >> 4, W_PL = (BN * BK * 2) >> 4, K_ST = (MMA_K * 2) >> 4;   // descriptor units
+  // cross products first (small -> large), into the correction accumulator
+  if constexpr (NSPLIT == 3) {
+#pragma unroll
+    for (int k = 0; k < BK / MMA_K; ++k) mma_k16<BN, F16>(corr, a0 + k * K_ST, w0 + 2 * W_PL + k * K_ST);
+#pragma unroll
+    for (int k = 0; k < BK / MMA_K; ++k) mma_k16<BN, F16>(corr, a0 + A_PL + k * K_ST, w0 + W_PL + k * K_ST);
+#pragma unroll
+    for (int k = 0; k < BK / MMA_K; ++k) mma_k16<BN, F16>(corr, a0 + 2 * A_PL + k * K_ST, w0 + k * K_ST);
+  }
+  if constexpr (NSPLIT >= 2) {
+#pragma unroll
+    for (int k = 0; k < BK / MMA_K; ++k) mma_k16<BN, F16>(corr, a0 + k * K_ST, w0 + W_PL + k * K_ST);
+#pragma unroll
+    for (int k = 0; k < BK / MMA_K; ++k) mma_k16<BN, F16>(corr, a0 + A_PL + k * K_ST, w0 + k * K_ST);
+  }
+#pragma unroll
+  for (int k = 0; k < BK / MMA_K; ++k) mma_k16<BN, F16>(main, a0 + k * K_ST, w0 + k * K_ST);
+}
+
+template <int BN, bool F16, int NSPLIT>
+__global__ void __launch_bounds__(NUM_THREADS, 1) tapgemm_tc_kernel(const __grid_constant__ CUtensorMap map_a,
+                                                                  const __grid_constant__ CUtensorMap map_w,
+                                                                  const TcParams p) {
+  constexpr int W_TILE_BYTES = BN * BK * 2;
+  constexpr int NACC = BN / 2;                      // accumulator registers per thread (m64 x BN over 128 threads)
+  constexpr int ST = BN + 8;                        // epilogue staging row stride (floats)
 
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  // carve: [stages][nsplit A tiles][nsplit W tiles] (1024-aligned), then barriers
+  // carve: [stages][nsplit A tiles][nsplit W tiles] (1024-aligned), then barriers.  The epilogue reuses the ring.
   uint8_t* tiles = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  // halo mode: [nsplit A halo planes][stages][nsplit W tiles]
-  const int stage_bytes = HALO ? p.nsplit * W_TILE_BYTES : p.nsplit * (A_TILE_BYTES + W_TILE_BYTES);
-  uint8_t* ring = HALO ? tiles + p.nsplit * HALO_BYTES : tiles;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(ring + (size_t)p.stages * stage_bytes);
+  const int stage_bytes = p.nsplit * (A_TILE_BYTES + W_TILE_BYTES);
+  const int ring_bytes = p.stages * stage_bytes > BM * ST * 4 ? p.stages * stage_bytes : BM * ST * 4;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(tiles + ring_bytes);
   uint64_t* full_bar = bars;                       // [MAX_STAGES]
   uint64_t* empty_bar = bars + MAX_STAGES;         // [MAX_STAGES]
-  uint64_t* acc_bar = bars + 2 * MAX_STAGES;       // accumulator ready
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * MAX_STAGES + 1);
-  uint64_t* halo_bar = bars + 2 * MAX_STAGES + 2;  // halo mode: A planes landed
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (warp == 0) PM_STAMP(0);                                   // kernel entry
@@ -124,41 +121,25 @@ __global__ void __launch_bounds__(NUM_THREADS, OCC) tapgemm_tc_kernel(const __gr
   const int n0 = blockIdx.y * BN;
   const int b0 = blockIdx.z * p.NB;
   const int n_iter = p.taps * p.kblocks;
-  const uint32_t cta_rank = CG2 ? cluster_ctarank() : 0u;      // 0 = leader of the pair (issues the MMAs)
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == CONSUMER_THREADS) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_w) : "memory");
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(smem_u32(&full_bar[s]), 1);
-      mbar_init(smem_u32(&empty_bar[s]), 1);
+      mbar_init(smem_u32(&empty_bar[s]), 2);       // one arrival per consumer warpgroup
     }
-    mbar_init(smem_u32(acc_bar), 1);
-    if constexpr (HALO) mbar_init(smem_u32(halo_bar), 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    if constexpr (CG2) {                                       // one warp of EACH CTA of the pair, same shared-memory slot
-      asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(TMEM_COLS) : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-    } else {
-      asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(TMEM_COLS) : "memory");
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-  }
-  tc_fence_before();
   __syncthreads();
-  if constexpr (CG2) cluster_sync_all();     // the peer's barriers exist before any remote arrive / TMA completion
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  if (warp == 0) PM_STAMP(1);                                   // prologue done (barriers, TMEM, descriptors)
+  if (warp == 0) PM_STAMP(1);                                   // prologue done (barriers, descriptors)
 
-  if (warp == 0) {
+  if (warp == CONSUMER_THREADS / 32) {
     // ===== TMA producer =====
     if (lane == 1 && p.prefetch) {
-      // Weights are read once per window and the per-window set (0.6-0.8 GB) does not fit the 126 MB L2, so every
-      // GEMM would stream its W tiles from HBM at DRAM latency with only 2-3 stages in flight.  Each CTA instead
-      // prefetches its share of the NEXT GEMM's weights into L2 (cp.async.bulk.prefetch.L2) while this one computes.
+      // Weights are read once per window and the per-window set (0.6-0.8 GB) does not fit the 50 MB L2, so every
+      // GEMM would stream its W tiles from HBM at DRAM latency.  Each CTA instead prefetches its share of the NEXT
+      // GEMM's weights into L2 (cp.async.bulk.prefetch.L2) while this one computes.
       const long long ncta = (long long)gridDim.x * gridDim.y * gridDim.z;
       const long long cta = ((long long)blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x;
       long long share = ((p.prefetch_bytes + ncta - 1) / ncta + 127) & ~127LL;
@@ -170,290 +151,146 @@ __global__ void __launch_bounds__(NUM_THREADS, OCC) tapgemm_tc_kernel(const __gr
         asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(p.prefetch + off), "r"(n) : "memory");
       }
     }
-    if constexpr (HALO) {
+    __syncwarp();
+    const uint32_t tx = (uint32_t)stage_bytes;
+    int s = 0, tap = 0, kb = 0;
+    uint32_t ph = 0;
+    for (int it = 0; it < n_iter; ++it) {
+      mbar_wait_fast(smem_u32(&empty_bar[s]), ph ^ 1u);       // whole warp waits (uniform control flow)
       if (elect_one()) {
-        mbar_expect_tx(smem_u32(halo_bar), (uint32_t)(p.nsplit * HALO_BYTES));
-        for (int pl = 0; pl < p.nsplit; ++pl)
-          tma_load_4d(smem_u32(tiles + pl * HALO_BYTES), &map_a, smem_u32(halo_bar), 0, l0 - p.pad, b0, pl);
-      }
-      __syncwarp();
-      int s = 0;
-      uint32_t ph = 0;
-      for (int it = 0; it < n_iter; ++it) {                      // one W tile pair per tap
-        mbar_wait_fast(smem_u32(&empty_bar[s]), ph ^ 1u);
-        if (elect_one()) {
-          const uint32_t bar = smem_u32(&full_bar[s]);
-          mbar_expect_tx(bar, (uint32_t)(p.nsplit * W_TILE_BYTES));
-          for (int pl = 0; pl < p.nsplit; ++pl)
-            tma_load_3d(smem_u32(ring + (size_t)s * stage_bytes + pl * W_TILE_BYTES), &map_w, bar, 0, it * p.w_rows + n0, pl);
-        }
-        __syncwarp();
-        if (++s == p.stages) { s = 0; ph ^= 1u; }
-      }
-    } else {
-      const uint32_t tx = (uint32_t)(p.nsplit * (A_TILE_BYTES + W_TILE_BYTES));
-      int s = 0, tap = 0, kb = 0;
-      uint32_t ph = 0;
-      for (int it = 0; it < n_iter; ++it) {
-        mbar_wait_fast(smem_u32(&empty_bar[s]), ph ^ 1u);       // whole warp waits (uniform control flow)
         const uint32_t bar = smem_u32(&full_bar[s]);
         uint8_t* st = tiles + (size_t)s * stage_bytes;
-        if (elect_one()) {
-        if constexpr (CG2) {
-          // Both CTAs' bytes land on the LEADER's barrier, which expects 2 x tx; the peer's barrier is unused.  (The
-          // peer cannot run a phase ahead: it reuses a stage only after the leader's MMAs of the previous use have
-          // committed.  A cluster-scope release arrive from the peer per k-block was tried first and serialised the
-          // peer's producer: 1 430 cycles per k-block whatever the work.)
-          if (cta_rank == 0) mbar_expect_tx(bar, 2 * tx);
-        } else {
-          mbar_expect_tx(bar, tx);
-        }
+        mbar_expect_tx(bar, tx);
         for (int pl = 0; pl < p.nsplit; ++pl) {
-          const uint32_t a_dst = smem_u32(st + pl * A_TILE_BYTES);
-          const uint32_t w_dst = smem_u32(st + p.nsplit * A_TILE_BYTES + pl * W_TILE_BYTES);
-          if constexpr (CG2) {
-            tma_load_4d_cg2(a_dst, &map_a, bar, kb * BK, l0 + tap - p.pad, b0, pl);
-            tma_load_3d_cg2(w_dst, &map_w, bar, kb * BK, tap * p.w_rows + n0 + (int)cta_rank * W_ROWS_CTA, pl);
-          } else {
-            tma_load_4d(a_dst, &map_a, bar, kb * BK, l0 + tap - p.pad, b0, pl);
-            tma_load_3d(w_dst, &map_w, bar, kb * BK, tap * p.w_rows + n0, pl);
-          }
+          tma_load_4d(smem_u32(st + pl * A_TILE_BYTES), &map_a, bar, kb * BK, l0 + tap - p.pad, b0, pl);
+          tma_load_3d(smem_u32(st + p.nsplit * A_TILE_BYTES + pl * W_TILE_BYTES), &map_w, bar, kb * BK, tap * p.w_rows + n0, pl);
         }
-        }
-        __syncwarp();
-        if (++s == p.stages) { s = 0; ph ^= 1u; }
-        if (++kb == p.kblocks) { kb = 0; ++tap; }
       }
-    }
-  } else if (warp == 1) {
-    // ===== MMA issuer (pair: the leader CTA only; the peer's warp 1 only owns its TMEM allocation) =====
-    if (cta_rank == 0)
-    // One thread feeds the tensor core, so its own instruction stream must stay far below the 64 cycles a
-    // 128x128x16 MMA takes.  Measured: with per-MMA descriptor construction, runtime div/mod for the stage ring
-    // and a clock-reading wait loop this thread was THE bottleneck (the mainloop ran at the same speed with all TMA
-    // loads disabled, profiles/gemm_microbench_r1.md).  Hence: running stage/phase counters, descriptors advanced by
-    // adding to a precomputed 64-bit base, product loops specialised per split mode and fully unrolled.
-    {
-      const uint64_t desc_hi = (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) | (2ull << 61);
-      auto mma = [](uint32_t d, uint64_t a, uint64_t b, uint32_t idesc, uint32_t acc) {
-        if constexpr (CG2) tc_mma_cg2(d, a, b, idesc, acc);
-        else tc_mma_bf16(d, a, b, idesc, acc);
-      };
-      auto commit = [](uint32_t bar) {
-        if constexpr (CG2) tc_commit_cg2(bar);               // arrives in both CTAs of the pair
-        else tc_commit(bar);
-      };
-      const uint32_t tiles_u32 = smem_u32(tiles);
-      const uint32_t ring_u32 = smem_u32(ring);
-      const uint32_t d_corr = tmem_base + 2 * ACC;
-      if constexpr (HALO) {
-        mbar_wait_fast(smem_u32(halo_bar), 0);
-        tc_fence_after();
-      }
-      uint32_t first_main0 = 1, first_main1 = 1, first_corr = 1;     // 1 until the accumulator has been written once
-      int s = 0;
-      uint32_t ph = 0;
-      for (int it = 0; it < n_iter; ++it) {
-        mbar_wait_fast(smem_u32(&full_bar[s]), ph);               // whole warp waits (uniform control flow)
-        tc_fence_after();
-        if (it == 0) PM_STAMP(2);                                 // first operand stage landed
-        if (elect_one()) {
-        const uint32_t a_base = HALO ? tiles_u32 + (uint32_t)it * 128u                             // tap = row shift
-                                     : tiles_u32 + (uint32_t)s * (uint32_t)stage_bytes;
-        const uint32_t w_base = HALO ? ring_u32 + (uint32_t)s * (uint32_t)stage_bytes : a_base + p.nsplit * A_TILE_BYTES;
-        // halo: the start address sits (it % 8) rows into a 1024-byte swizzle atom; base offset (bits 49-51) stays 0
-        const uint64_t a0 = desc_hi | (uint64_t)((a_base >> 4) & 0x3FFFu);
-        const uint64_t w0 = desc_hi | (uint64_t)((w_base >> 4) & 0x3FFFu);
-        constexpr uint64_t A_PL = (HALO ? HALO_BYTES : A_TILE_BYTES) >> 4, W_PL = W_TILE_BYTES >> 4, K_ST = (UMMA_K * 2) >> 4;   // descriptor units
-        const bool odd = it & 1;
-        const uint32_t d_main = tmem_base + (odd ? ACC : 0);
-        // cross products first (small -> large), into the correction accumulator
-        if (p.nsplit == 3) {
-#pragma unroll
-          for (int k = 0; k < BK / UMMA_K; ++k) mma(d_corr, a0 + k * K_ST, w0 + 2 * W_PL + k * K_ST, IDESC, (k | (int)(first_corr ^ 1u)) != 0);
-#pragma unroll
-          for (int k = 0; k < BK / UMMA_K; ++k) mma(d_corr, a0 + A_PL + k * K_ST, w0 + W_PL + k * K_ST, IDESC, 1);
-#pragma unroll
-          for (int k = 0; k < BK / UMMA_K; ++k) mma(d_corr, a0 + 2 * A_PL + k * K_ST, w0 + k * K_ST, IDESC, 1);
-        }
-        if (p.nsplit >= 2) {
-          const uint32_t fresh = p.nsplit == 3 ? 0u : first_corr;      // with 3 planes the block above already wrote it
-#pragma unroll
-          for (int k = 0; k < BK / UMMA_K; ++k) mma(d_corr, a0 + k * K_ST, w0 + W_PL + k * K_ST, IDESC, (k | (int)(fresh ^ 1u)) != 0);
-#pragma unroll
-          for (int k = 0; k < BK / UMMA_K; ++k) mma(d_corr, a0 + A_PL + k * K_ST, w0 + k * K_ST, IDESC, 1);
-        }
-        {
-          const uint32_t first = odd ? first_main1 : first_main0;
-#pragma unroll
-          for (int k = 0; k < BK / UMMA_K; ++k) mma(d_main, a0 + k * K_ST, w0 + k * K_ST, IDESC, (k | (int)(first ^ 1u)) != 0);
-        }
-        commit(smem_u32(&empty_bar[s]));             // frees this smem stage when the MMAs have read it
-        }
-        __syncwarp();
-        if (p.nsplit >= 2) first_corr = 0;
-        if (it & 1) first_main1 = 0; else first_main0 = 0;
-        if (++s == p.stages) { s = 0; ph ^= 1u; }
-      }
-      if (n_iter > 0 && elect_one()) commit(smem_u32(acc_bar));      // accumulator complete
-      PM_STAMP(3);                                                // all MMAs issued
-    }
-  } else {
-    // ===== epilogue warps 2..9: TMEM lane quarter = warp % 4, column half = (warp - 2) / 4 =====
-    // tcgen05.ld hands each thread one accumulator ROW (32 consecutive columns).  The 32x32 chunk is transposed
-    // through shared memory (the operand ring is idle by now) so that each quarter-warp writes one contiguous
-    // 128-byte row segment.  Measured (profiles/gemm_microbench_r1.md): with 4 warps and branchy per-element code
-    // the epilogue cost 12 us of a 16 us GEMM - it is instruction-latency bound (one warp per scheduler), not
-    // memory bound - hence 8 warps, branch-free activation (identity == leaky with slope 1) and a warp-uniform
-    // fast path for full chunks.
-    const int q = warp & 3;
-    const int half = (warp - 2) >> 2;
-    constexpr int CW = 32;                                         // columns per tcgen05.ld chunk
-    constexpr int LPR = CW / 4;                                    // lanes per staged row (one float4 each)
-    constexpr int RPI = 32 / LPR;                                  // rows written per warp-wide store
-    constexpr int NIT = 32 / RPI;                                  // store rounds per chunk
-    constexpr int ST = CW + 4;                                     // staging row stride (floats): 16B aligned, conflict-free
-    const uint32_t stage = smem_u32(tiles) + (warp - 2) * 32 * ST * 4;   // <= 4.6 KB per warp (shared-space address)
-    const int sub_r = lane / LPR, c4 = (lane % LPR) * 4;           // this lane's row-in-group / first column of its float4
-    const int r_shift = 31 - __clz(p.R);                           // R is a power of two
-    const bool vec_f = p.out_f32 && ((p.ldo & 3) == 0) && ((reinterpret_cast<uintptr_t>(p.out_f32) & 15) == 0) && ((p.o_bs & 3) == 0);
-    const bool vec_r = p.residual && ((p.ldr & 3) == 0) && ((reinterpret_cast<uintptr_t>(p.residual) & 15) == 0) && ((p.r_bs & 3) == 0);
-    const bool vec_b = p.out_bf16 && ((p.ldob & 3) == 0) && ((reinterpret_cast<uintptr_t>(p.out_bf16) & 7) == 0) &&
-                       ((p.ob_bs & 3) == 0) && ((p.ob_ps & 3) == 0);
-    const bool all_vec = (!p.out_f32 || vec_f) && (!p.residual || vec_r) && (!p.out_bf16 || vec_b);
-    const float act_slope = p.act == PM_ACT_NONE ? 1.f : (p.act == PM_ACT_RELU ? 0.f : p.slope);
-    // rows this lane stores (NIT per chunk): offsets are chunk-invariant
-    long long off_f[NIT], off_r[NIT], off_b[NIT];
-    uint32_t row_ok = 0;
-#pragma unroll
-    for (int i = 0; i < NIT; ++i) {
-      const int rt = q * 32 + RPI * i + sub_r;
-      const int b = b0 + (rt >> r_shift), l = l0 + (rt & (p.R - 1));
-      if (b < p.batch && l < p.rows_out) row_ok |= 1u << i;
-      off_f[i] = (long long)b * p.o_bs + (long long)l * p.ldo;
-      off_r[i] = (long long)b * p.r_bs + (long long)l * p.ldr;
-      off_b[i] = (long long)b * p.ob_bs + (long long)l * p.ldob;
-    }
-#pragma unroll 1
-    for (int c0 = half * (BN / 2); c0 < (half + 1) * (BN / 2); c0 += CW) {
-      uint32_t acc[CW];
-      float v[CW];
-      const uint32_t lane_col = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)c0;
-      // Everything that does not depend on the accumulators - row offsets above, this chunk's bias and residual
-      // loads - is issued BEFORE the accumulator wait / TMEM loads, so their global latency overlaps the tail of the
-      // mainloop instead of sitting in the epilogue (measured round 2: 33.4 -> 30.6 ms per step in bf16x6 mode,
-      // 26.5 -> 23.9 ms in fp16x3, profiles/README.md).
-      const int nb = n0 + c0;                                                      // first column of this chunk
-      const int n = nb + c4;                                                       // this lane's first column
-      const bool fast = all_vec && nb + CW <= p.cout;                              // warp-uniform: whole chunk inside cout
-      float4 bias4 = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (p.bias) {
-        if (n < p.cout) bias4.x = __ldg(p.bias + n);
-        if (n + 1 < p.cout) bias4.y = __ldg(p.bias + n + 1);
-        if (n + 2 < p.cout) bias4.z = __ldg(p.bias + n + 2);
-        if (n + 3 < p.cout) bias4.w = __ldg(p.bias + n + 3);
-      }
-      float4 rres[NIT];
-      if (fast && p.residual) {
-#pragma unroll
-        for (int i = 0; i < NIT; ++i)
-          rres[i] = ((row_ok >> i) & 1u) ? *reinterpret_cast<const float4*>(p.residual + off_r[i] + n) : make_float4(0.f, 0.f, 0.f, 0.f);
-      }
-      if (c0 == half * (BN / 2)) {
-        mbar_wait(smem_u32(acc_bar), 0);
-        tc_fence_after();
-        if (warp == 2) PM_STAMP(4);                                 // accumulators complete
-      }
-      __syncwarp();                                                                // .sync.aligned: whole warp converged
-      tmem_ld(lane_col, acc);
-#pragma unroll
-      for (int j = 0; j < CW; ++j) v[j] = __uint_as_float(acc[j]);
-      if (n_iter > 1) {                                                            // second main accumulator in use
-        tmem_ld(lane_col + ACC, acc);
-#pragma unroll
-        for (int j = 0; j < CW; ++j) v[j] += __uint_as_float(acc[j]);
-      }
-      if (p.nsplit > 1) {                                                          // cross-product accumulator
-        tmem_ld(lane_col + 2 * ACC, acc);
-#pragma unroll
-        for (int j = 0; j < CW; ++j) v[j] += __uint_as_float(acc[j]);
-      }
-      if constexpr (F16) {                                                         // undo the weight pre-scale (exact)
-#pragma unroll
-        for (int j = 0; j < CW; ++j) v[j] *= p.acc_scale;
-      }
-      if (nb >= p.cout) continue;                                   // warp-uniform
-      // transpose: thread = row -> smem[row][0..CW)
-#pragma unroll
-      for (int j = 0; j < CW / 4; ++j) sts128(stage + (lane * ST + 4 * j) * 4, v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
       __syncwarp();
-      // identity == leaky with slope 1: one branch-free (select) formula for none / relu / leaky / partial activation
-      const float s0 = n < p.act_cols ? act_slope : 1.f, s1 = n + 1 < p.act_cols ? act_slope : 1.f;
-      const float s2 = n + 2 < p.act_cols ? act_slope : 1.f, s3 = n + 3 < p.act_cols ? act_slope : 1.f;
-      if (fast) {
-        // Hot path, kept contiguous and small: the ragged path below is rolled and placed after it, so the
-        // instructions actually executed do not straddle 200+ KB of cold unrolled code (in-kernel clock stamps,
-        // profiles/gemm_timeline_r1.txt: the epilogue was instruction-fetch bound).
-#pragma unroll
-        for (int i = 0; i < NIT; ++i) {
-          if (!((row_ok >> i) & 1u)) continue;
-          float4 x = lds128(stage + ((RPI * i + sub_r) * ST + c4) * 4);
-          x.x += bias4.x; x.y += bias4.y; x.z += bias4.z; x.w += bias4.w;
-          if (p.residual) {
-            const float4 t = rres[i];
-            x.x += t.x; x.y += t.y; x.z += t.z; x.w += t.w;
-          }
-          // compare-select, not fmaxf / fminf: those return the non-NaN operand and would turn the NaN an fp16 operand
-          // overflow leaves into 0, hiding it from the overflow guard (round 2: a 2e4x too loud input went unnoticed)
-          x.x = x.x < 0.f ? s0 * x.x : x.x;
-          x.y = x.y < 0.f ? s1 * x.y : x.y;
-          x.z = x.z < 0.f ? s2 * x.z : x.z;
-          x.w = x.w < 0.f ? s3 * x.w : x.w;
-          if (p.out_f32) *reinterpret_cast<float4*>(p.out_f32 + off_f[i] + n) = x;
-          if (p.out_bf16) {
-            const PmPlanes P{p.out_bf16 + off_b[i], p.ob_ps, p.ldob, p.out_nsplit};
-            pm_store_planes4_t<F16>(P, 0, n, x);
-          }
-        }
-      } else if (n < p.cout) {
-        // ragged / unaligned tail: per element, rolled (offsets recomputed so the arrays above stay in registers)
-#pragma unroll 1
-        for (int i = 0; i < NIT; ++i) {
-          const int rt = q * 32 + RPI * i + sub_r;
-          const int b = b0 + (rt >> r_shift), l = l0 + (rt & (p.R - 1));
-          if (b >= p.batch || l >= p.rows_out) continue;
-          const long long of = (long long)b * p.o_bs + (long long)l * p.ldo;
-          const long long orr = (long long)b * p.r_bs + (long long)l * p.ldr;
-          const PmPlanes P{p.out_bf16 ? p.out_bf16 + (long long)b * p.ob_bs + (long long)l * p.ldob : nullptr,
-                           p.ob_ps, p.ldob, p.out_nsplit};
-          const uint32_t src = stage + ((RPI * i + sub_r) * ST + c4) * 4;
-#pragma unroll 1
-          for (int k = 0; k < 4; ++k) {
-            if (n + k >= p.cout) break;
-            float y;
-            asm volatile("ld.shared.f32 %0, [%1];" : "=f"(y) : "r"(src + 4 * k) : "memory");
-            y += k == 0 ? bias4.x : (k == 1 ? bias4.y : (k == 2 ? bias4.z : bias4.w));
-            if (p.residual) y += p.residual[orr + n + k];
-            y = y < 0.f ? (k == 0 ? s0 : (k == 1 ? s1 : (k == 2 ? s2 : s3))) * y : y;
-            if (p.out_f32) p.out_f32[of + n + k] = y;
-            if (P.ptr) pm_store_planes_t<F16>(P, 0, n + k, y);
-          }
-        }
-      }
+      if (++s == p.stages) { s = 0; ph ^= 1u; }
+      if (++kb == p.kblocks) { kb = 0; ++tap; }
     }
+    return;                                        // the consumers' named barriers below do not count this warp
   }
 
-  if (warp == 2) PM_STAMP(5);                                     // this warp's share of the epilogue issued
-  // teardown: everyone done with TMEM before the owning warp frees it
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) PM_STAMP(6);                                     // all warps done
-  if constexpr (CG2) cluster_sync_all();    // neither CTA frees TMEM or leaves while the peer may still signal its barriers
-  if (warp == 1) {
-    tc_fence_after();
-    if constexpr (CG2) asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(TMEM_COLS) : "memory");
-    else asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(TMEM_COLS) : "memory");
+  // ===== consumer warpgroups =====
+  const int wg = threadIdx.x >> 7;                  // 0 / 1: tile rows 64 wg .. 64 wg + 63
+  float acc0[NACC], acc1[NACC], accc[NACC];
+#pragma unroll
+  for (int i = 0; i < NACC; ++i) { acc0[i] = 0.f; acc1[i] = 0.f; accc[i] = 0.f; }
+  {
+    const uint32_t tiles_u32 = smem_u32(tiles);
+    int s = 0;
+    uint32_t ph = 0;
+    int prev = -1;                                  // stage whose MMAs are still in flight
+    // one k-block: the even ones accumulate into acc0, the odd ones into acc1 (unrolled by two, so that every wgmma
+    // names its accumulator statically)
+    auto kblock = [&](float (&main)[NACC]) {
+      mbar_wait_fast(smem_u32(&full_bar[s]), ph);
+      if (prev < 0 && warp == 0) PM_STAMP(2);                     // first operand stage landed
+      const uint32_t a_base = tiles_u32 + (uint32_t)s * (uint32_t)stage_bytes + (uint32_t)wg * (64 * 128);
+      const uint32_t w_base = tiles_u32 + (uint32_t)s * (uint32_t)stage_bytes + (uint32_t)(NSPLIT * A_TILE_BYTES);
+      wgmma_fence();
+      mma_kblock<BN, F16, NSPLIT>(main, accc, gmma_desc(GMMA_DESC_K_SW128, a_base), gmma_desc(GMMA_DESC_K_SW128, w_base));
+      wgmma_commit();
+      // at most one k-block in flight: the previous one has finished reading its stage, hand it back to the producer
+      wgmma_wait<1>();
+      if (prev >= 0 && threadIdx.x % 128 == 0) mbar_arrive(smem_u32(&empty_bar[prev]));
+      prev = s;
+      if (++s == p.stages) { s = 0; ph ^= 1u; }
+    };
+    int it = 0;
+    for (; it + 1 < n_iter; it += 2) {
+      kblock(acc0);
+      kblock(acc1);
+    }
+    if (it < n_iter) kblock(acc0);
+    if (warp == 0) PM_STAMP(3);                                 // all MMAs issued
+    wgmma_wait<0>();
+    if (warp == 0) PM_STAMP(4);                                 // accumulators complete
+    wgmma_fence_regs(acc0);
+    wgmma_fence_regs(acc1);
+    wgmma_fence_regs(accc);
   }
+  // every MMA of both warpgroups has read its operands: the ring becomes the epilogue's staging tile
+  named_bar_sync(1, CONSUMER_THREADS);
+  {
+    const int wq = (threadIdx.x >> 5) & 3, t4 = lane & 3;
+    const int r0 = wg * 64 + wq * 16 + (lane >> 2);
+    float* stg = reinterpret_cast<float*>(tiles);
+#pragma unroll
+    for (int i = 0; i < NACC / 4; ++i) {
+      const int c = 8 * i + 2 * t4;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float v0 = acc0[4 * i + 2 * h] + acc1[4 * i + 2 * h];
+        float v1 = acc0[4 * i + 2 * h + 1] + acc1[4 * i + 2 * h + 1];
+        v0 += accc[4 * i + 2 * h];
+        v1 += accc[4 * i + 2 * h + 1];
+        if constexpr (F16) { v0 *= p.acc_scale; v1 *= p.acc_scale; }       // undo the weight pre-scale (exact)
+        *reinterpret_cast<float2*>(stg + (r0 + 8 * h) * ST + c) = make_float2(v0, v1);
+      }
+    }
+  }
+  named_bar_sync(1, CONSUMER_THREADS);
+
+  // ===== epilogue: one float4 of one row per thread and round; consecutive threads cover a row (coalesced) =====
+  const bool vec_f = p.out_f32 && ((p.ldo & 3) == 0) && ((reinterpret_cast<uintptr_t>(p.out_f32) & 15) == 0) && ((p.o_bs & 3) == 0);
+  const bool vec_r = p.residual && ((p.ldr & 3) == 0) && ((reinterpret_cast<uintptr_t>(p.residual) & 15) == 0) && ((p.r_bs & 3) == 0);
+  const bool vec_b = p.out_bf16 && ((p.ldob & 3) == 0) && ((reinterpret_cast<uintptr_t>(p.out_bf16) & 7) == 0) &&
+                     ((p.ob_bs & 3) == 0) && ((p.ob_ps & 3) == 0);
+  const bool all_vec = (!p.out_f32 || vec_f) && (!p.residual || vec_r) && (!p.out_bf16 || vec_b);
+  const float act_slope = p.act == PM_ACT_NONE ? 1.f : (p.act == PM_ACT_RELU ? 0.f : p.slope);
+  const int r_shift = 31 - __clz(p.R);                           // R is a power of two
+  constexpr int C4 = BN / 4;                                     // float4 columns per row
+  const float* stg = reinterpret_cast<const float*>(tiles);
+#pragma unroll 1
+  for (int item = threadIdx.x; item < BM * C4; item += CONSUMER_THREADS) {
+    const int rt = item / C4, c = (item % C4) * 4;
+    const int b = b0 + (rt >> r_shift), l = l0 + (rt & (p.R - 1));
+    const int n = n0 + c;
+    if (b >= p.batch || l >= p.rows_out || n >= p.cout) continue;
+    const float4 x4 = *reinterpret_cast<const float4*>(stg + rt * ST + c);
+    // identity == leaky with slope 1: one branch-free (select) formula for none / relu / leaky / partial activation.
+    // Compare-select, not fmaxf / fminf: those return the non-NaN operand and would turn the NaN an fp16 operand
+    // overflow leaves into 0, hiding it from the host's overflow guard.
+    const long long of = (long long)b * p.o_bs + (long long)l * p.ldo;
+    const long long orr = (long long)b * p.r_bs + (long long)l * p.ldr;
+    const PmPlanes P{p.out_bf16 ? p.out_bf16 + (long long)b * p.ob_bs + (long long)l * p.ldob : nullptr,
+                     p.ob_ps, p.ldob, p.out_nsplit};
+    if (all_vec && n + 4 <= p.cout) {
+      float4 x = x4;
+      if (p.bias) { x.x += __ldg(p.bias + n); x.y += __ldg(p.bias + n + 1); x.z += __ldg(p.bias + n + 2); x.w += __ldg(p.bias + n + 3); }
+      if (p.residual) {
+        const float4 t = *reinterpret_cast<const float4*>(p.residual + orr + n);
+        x.x += t.x; x.y += t.y; x.z += t.z; x.w += t.w;
+      }
+      x.x = x.x < 0.f ? (n < p.act_cols ? act_slope : 1.f) * x.x : x.x;
+      x.y = x.y < 0.f ? (n + 1 < p.act_cols ? act_slope : 1.f) * x.y : x.y;
+      x.z = x.z < 0.f ? (n + 2 < p.act_cols ? act_slope : 1.f) * x.z : x.z;
+      x.w = x.w < 0.f ? (n + 3 < p.act_cols ? act_slope : 1.f) * x.w : x.w;
+      if (p.out_f32) *reinterpret_cast<float4*>(p.out_f32 + of + n) = x;
+      if (P.ptr) pm_store_planes4_t<F16>(P, 0, n, x);
+    } else {
+      // ragged / unaligned tail: per element
+      const float xs[4] = {x4.x, x4.y, x4.z, x4.w};
+#pragma unroll
+      for (int k = 0; k < 4; ++k) {
+        if (n + k >= p.cout) break;
+        float y = xs[k];
+        if (p.bias) y += __ldg(p.bias + n + k);
+        if (p.residual) y += p.residual[orr + n + k];
+        y = y < 0.f ? (n + k < p.act_cols ? act_slope : 1.f) * y : y;
+        if (p.out_f32) p.out_f32[of + n + k] = y;
+        if (P.ptr) pm_store_planes_t<F16>(P, 0, n + k, y);
+      }
+    }
+  }
+  if (warp == 0) PM_STAMP(5);                                   // this warp's share of the epilogue issued
+#ifdef PM_TC_TIMING
+  named_bar_sync(1, CONSUMER_THREADS);
+#endif
+  if (warp == 0) PM_STAMP(6);                                   // all consumer warps done
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -486,42 +323,23 @@ __global__ void __launch_bounds__(256) split_bf16_kernel(const float* __restrict
 }
 
 // ---------------------------------------------------------------------------------------------------
-template <int BN, bool F16, bool CG2, int OCC = 1, bool HALO = false>
-int launch(const CUtensorMap& ma, const CUtensorMap& mw, TcParams& p, dim3 grid, cudaStream_t st, int pair_axis = 0) {
-  static_assert(OCC == 1 || (BN == 64 && !CG2), "two CTAs per SM: 64-column tiles only (TMEM columns, registers)");
-  static_assert(!HALO || (OCC == 2 && BN == 64), "halo mode is built for the 64-column, two-CTAs-per-SM form");
-  const int stage_bytes = HALO ? p.nsplit * BN * BK * 2 : p.nsplit * (A_TILE_BYTES + (CG2 ? BN / 2 : BN) * BK * 2);
-  const int fixed_bytes = HALO ? p.nsplit * HALO_BYTES : 0;
-  static const int env_kb = getenv("PM_TC_SMEM_KB") ? atoi(getenv("PM_TC_SMEM_KB")) : 200;   // tuning override
-  int stages = ((OCC == 2 ? OCC2_SMEM_KB : env_kb) * 1024 - fixed_bytes) / stage_bytes;
+template <int BN, bool F16, int NSPLIT>
+int launch(const CUtensorMap& ma, const CUtensorMap& mw, TcParams& p, dim3 grid, cudaStream_t st) {
+  const int stage_bytes = p.nsplit * (A_TILE_BYTES + BN * BK * 2);
+  int stages = RING_KB * 1024 / stage_bytes;
   if (stages > MAX_STAGES) stages = MAX_STAGES;
   if (stages < 2) return PM_EUNSUPPORTED;
   p.stages = stages;
-  const size_t smem = (size_t)fixed_bytes + (size_t)stages * stage_bytes + 1024 /*align slack*/ + (2 * MAX_STAGES + 3) * sizeof(uint64_t);
+  const int staging = BM * (BN + 8) * 4;
+  const size_t ring = (size_t)stages * stage_bytes > (size_t)staging ? (size_t)stages * stage_bytes : (size_t)staging;
+  const size_t smem = ring + 1024 /*align slack*/ + 2 * MAX_STAGES * sizeof(uint64_t);
   static unsigned long long configured = 0;       // per template instantiation, one bit per device
   if (pm_first_use_on_device(configured)) {
-    cudaError_t e = cudaFuncSetAttribute(tapgemm_tc_kernel<BN, F16, CG2, OCC, HALO>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    cudaError_t e = cudaFuncSetAttribute(tapgemm_tc_kernel<BN, F16, NSPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     if (e != cudaSuccess) { configured = 0; return (int)e; }
   }
-  if constexpr (CG2) {                      // CTA pairs: 2-CTA clusters along the row-tile axis
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = grid;
-    cfg.blockDim = dim3(NUM_THREADS);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = pair_axis == 0 ? 2 : 1;       // the pair: two row tiles (x) or two clip tiles (z) of one N tile
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = pair_axis == 2 ? 2 : 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    const cudaError_t e = cudaLaunchKernelEx(&cfg, tapgemm_tc_kernel<BN, F16, CG2, OCC, HALO>, ma, mw, p);
-    return e == cudaSuccess ? PM_OK : (int)e;
-  } else {
-    tapgemm_tc_kernel<BN, F16, CG2, OCC, HALO><<<grid, NUM_THREADS, smem, st>>>(ma, mw, p);
-    PM_LAUNCH_CHECK();
-  }
+  tapgemm_tc_kernel<BN, F16, NSPLIT><<<grid, NUM_THREADS, smem, st>>>(ma, mw, p);
+  PM_LAUNCH_CHECK();
 }
 
 }  // namespace
@@ -555,26 +373,10 @@ extern "C" int pm_tapgemm_tc(const uint16_t* A, long long a_ps, long long a_bs, 
   int R = 128;
   if (rows_out <= 64 && batch > 1) { R = 16; while (R < rows_out) R <<= 1; }
   const int NB = 128 / R;
-  // N tile: 128 columns (64 for narrow outputs).  Measured alternatives that lost and were removed: 64-column tiles for
-  // the M = 2048 GEMMs, 96-column tiles (34.2 vs 33.4 ms per step), 2x2 clusters with TMA multicast (10-25 % slower),
-  // programmatic dependent launch (35.2 vs 34.7 ms): profiles/README.md.
-  int BNsel = cout <= 64 ? 64 : 128;
+  // N tile: 64 columns.  Three m64n128 accumulators per thread (192 registers) do not fit the 168 registers a thread
+  // of a 288- or 384-thread CTA gets on sm_90 (ptxas spills them); three m64n64 ones take 96.
+  constexpr int BNsel = 64;
   PM_REQUIRE(w_rows % BNsel == 0);
-  // CTA pairs (cta_group::2) where the row-tile grid is even: two fp16 planes, 128-column tiles, 128-row tiles.
-  static const bool cg2_on = !(getenv("PM_TC_CG2") && atoi(getenv("PM_TC_CG2")) == 0);      // A/B switch (tools)
-  // Measured (profiles/r2/gemm_microbench_fp16_pairs.txt, M = 2048, N = 768): K = 768 12.4 vs 13.5 us, K = 1536 18.1 vs
-  // 20.8, K = 3072 29.0 vs 35.5 (906 instead of 1 184 cycles per k-block: MMA-bound); K <= 256 is a few hundred ns
-  // slower (cluster barriers in prologue and teardown), hence the k-block threshold.
-  // Pairs are formed along the row-tile axis only.  (Pairing clip tiles of the batch-tiled small-R convs along z was
-  // tried and failed the golden parity tests on the first run; it was not pursued - those convs are a few per cent
-  // of the step.)
-  const int pair_axis = 0;
-  const bool cg2 = cg2_on && f16 && nsplit == 2 && BNsel == 128 && R == 128 && pm_cdiv(rows_out, R) % 2 == 0 &&
-                   taps * ((cin + BK - 1) / BK) >= 6;
-
-  // Halo mode (see the kernel): one-k-block convs with >= 3 taps on 128-row tiles, two fp16 / bf16 planes.
-  static const bool halo_on = !(getenv("PM_TC_HALO") && atoi(getenv("PM_TC_HALO")) == 0);      // A/B switch (tools)
-  const bool halo = halo_on && BNsel == 64 && R == 128 && cin <= BK && taps >= 3 && BM + taps - 1 <= HALO_ROWS && nsplit == 2;
 
   TcParams p;
   p.taps = taps; p.pad = pad; p.nsplit = nsplit; p.kblocks = (cin + BK - 1) / BK;
@@ -594,35 +396,27 @@ extern "C" int pm_tapgemm_tc(const uint16_t* A, long long a_ps, long long a_bs, 
     const long long ps_el = nsplit > 1 ? a_ps : bs_el * batch;
     cuuint64_t dims[4] = {(cuuint64_t)cin, (cuuint64_t)rows_in, (cuuint64_t)batch, (cuuint64_t)nsplit};
     cuuint64_t strides[3] = {(cuuint64_t)lda * 2, (cuuint64_t)bs_el * 2, (cuuint64_t)ps_el * 2};
-    cuuint32_t box[4] = {(cuuint32_t)BK, (cuuint32_t)(halo ? HALO_ROWS : R), (cuuint32_t)NB, 1};
+    cuuint32_t box[4] = {(cuuint32_t)BK, (cuuint32_t)R, (cuuint32_t)NB, 1};
     if (!encode_map(&ma, A, 4, dims, strides, box, f16)) return PM_EBADARG;
   }
   {
     const long long ps_el = nsplit > 1 ? w_ps : (long long)taps * w_rows * ldw;
     cuuint64_t dims[3] = {(cuuint64_t)cin, (cuuint64_t)taps * w_rows, (cuuint64_t)nsplit};
     cuuint64_t strides[2] = {(cuuint64_t)ldw * 2, (cuuint64_t)ps_el * 2};
-    cuuint32_t box[3] = {(cuuint32_t)BK, (cuuint32_t)(cg2 ? BNsel / 2 : BNsel), 1};      // pair: each CTA stages half of the W tile
+    cuuint32_t box[3] = {(cuuint32_t)BK, (cuuint32_t)BNsel, 1};
     if (!encode_map(&mw, W, 3, dims, strides, box, f16)) return PM_EBADARG;
   }
   dim3 grid(pm_cdiv(rows_out, R), pm_cdiv(cout, BNsel), pm_cdiv(batch, NB));
   PM_REQUIRE(grid.z <= 65535 && grid.y <= 65535);
-  // Two CTAs per SM for 64-column launches with more tiles than two per SM, if half the ring still holds 2 stages.
-  static const bool occ2_on = !(getenv("PM_TC_OCC2") && atoi(getenv("PM_TC_OCC2")) == 0);      // A/B switch (tools)
-  const bool occ2 = occ2_on && BNsel == 64 && (long long)grid.x * grid.y * grid.z > 2 * 148 &&
-                    OCC2_SMEM_KB * 1024 / (nsplit * (A_TILE_BYTES + 64 * BK * 2)) >= 2;
-  if (halo) {
-    if (f16) return launch<64, true, false, 2, true>(ma, mw, p, grid, (cudaStream_t)stream);
-    return launch<64, false, false, 2, true>(ma, mw, p, grid, (cudaStream_t)stream);
-  }
+  const cudaStream_t st = (cudaStream_t)stream;
   if (f16) {
-    if (cg2) return launch<128, true, true>(ma, mw, p, grid, (cudaStream_t)stream, pair_axis);
-    if (occ2) return launch<64, true, false, 2>(ma, mw, p, grid, (cudaStream_t)stream);
-    if (BNsel == 64) return launch<64, true, false>(ma, mw, p, grid, (cudaStream_t)stream);
-    return launch<128, true, false>(ma, mw, p, grid, (cudaStream_t)stream);
+    if (nsplit == 1) return launch<BNsel, true, 1>(ma, mw, p, grid, st);
+    if (nsplit == 2) return launch<BNsel, true, 2>(ma, mw, p, grid, st);
+    return launch<BNsel, true, 3>(ma, mw, p, grid, st);
   }
-  if (occ2) return launch<64, false, false, 2>(ma, mw, p, grid, (cudaStream_t)stream);
-  if (BNsel == 64) return launch<64, false, false>(ma, mw, p, grid, (cudaStream_t)stream);
-  return launch<128, false, false>(ma, mw, p, grid, (cudaStream_t)stream);
+  if (nsplit == 1) return launch<BNsel, false, 1>(ma, mw, p, grid, st);
+  if (nsplit == 2) return launch<BNsel, false, 2>(ma, mw, p, grid, st);
+  return launch<BNsel, false, 3>(ma, mw, p, grid, st);
 }
 
 #ifdef PM_TC_TIMING
@@ -651,7 +445,7 @@ extern "C" int pm_split_bf16(const float* x, long long x_bs, int ldx, int batch,
                    (o_ps & 3) == 0 && (reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 7) == 0;
   const long long work = (long long)rows * (vec ? ch / 4 : ch);
   long long gx = (work + 255) / 256;
-  const long long cap = batch >= 148 * 4 ? 1 : (148 * 8 + batch - 1) / batch;
+  const long long cap = batch >= 132 * 4 ? 1 : (132 * 8 + batch - 1) / batch;
   if (gx > cap) gx = cap;
   dim3 grid((unsigned)gx, batch);
   __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(out);

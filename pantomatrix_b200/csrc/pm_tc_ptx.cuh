@@ -1,5 +1,5 @@
-// PTX wrappers shared by the tcgen05 kernels (tap-GEMM, VQ lookup, attention): mbarrier, TMA, tcgen05.mma /
-// commit / ld, UMMA descriptors.  sm_100a only.  Everything is static-inline: include from one .cu at a time.
+// PTX wrappers shared by the Hopper tensor-core kernels (tap-GEMM, VQ lookup, attention): mbarrier, TMA, wgmma and
+// its shared-memory descriptors.  sm_90a.  Everything is static-inline: include from one .cu at a time.
 #pragma once
 #include <cuda.h>
 #include <stdint.h>
@@ -17,7 +17,7 @@ __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
 }
 // Bounded wait: a protocol bug must become a trap (an error the host sees), never a hung GPU.  The spin body is kept to
 // the probe itself (try_wait suspends the thread for a hardware-defined slice): the watchdog clock is read only every
-// 4096 probes - with it in every iteration the waiting warps of the VQ kernel cost ~10 % of the SM's issue slots.
+// 4096 probes.
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   uint32_t spins = 0;
   long long t0 = 0;
@@ -63,9 +63,8 @@ __device__ __forceinline__ void mbar_wait_fast(uint32_t bar, uint32_t parity) {
       : "=r"(done) : "r"(bar), "r"(parity) : "memory");
   if (!done) mbar_wait(bar, parity);
 }
-// One lane of a converged warp (PTX elect.sync): the canonical guard for TMA / tcgen05 issue.  With warp-uniform
-// control flow around it the compiler keeps descriptors and barrier addresses in uniform registers; guarding with
-// `lane == 0` instead makes them thread-varying and wraps every UTMALDG / UTCHMMA in a waterfall loop.
+// One lane of a converged warp (PTX elect.sync): the canonical guard for TMA issue.  With warp-uniform control flow
+// around it the compiler keeps descriptors and barrier addresses in uniform registers.
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile("{\n\t.reg .pred P1;\n\telect.sync _|P1, 0xffffffff;\n\tselp.u32 %0, 1, 0, P1;\n\t}" : "=r"(pred));
@@ -89,126 +88,10 @@ __device__ __forceinline__ float4 lds128(uint32_t addr) {
   asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr) : "memory");
   return v;
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tc_mma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// UMMA smem descriptors (cute::UMMA::SmemDescriptor, version 1 = sm_100): K-major, 128-byte swizzle, 8-row groups
-// 1024 B apart; built in the MMA loop as desc_hi | (addr >> 4).
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-// Split form for software pipelining: issue the load of the next chunk, work on the current one, then wait.  The wait
-// takes the destination registers as in/out operands so that no use of them can be scheduled ahead of it.
-__device__ __forceinline__ void tmem_ld32_issue(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld32_wait(uint32_t (&r)[32]) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]),
-                 "+r"(r[8]), "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15]),
-                 "+r"(r[16]), "+r"(r[17]), "+r"(r[18]), "+r"(r[19]), "+r"(r[20]), "+r"(r[21]), "+r"(r[22]), "+r"(r[23]),
-                 "+r"(r[24]), "+r"(r[25]), "+r"(r[26]), "+r"(r[27]), "+r"(r[28]), "+r"(r[29]), "+r"(r[30]), "+r"(r[31])
-               :: "memory");
-}
-__device__ __forceinline__ void tmem_ld16_issue(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld16_wait(uint32_t (&r)[16]) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]),
-                 "+r"(r[8]), "+r"(r[9]), "+r"(r[10]), "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15])
-               :: "memory");
-}
-__device__ __forceinline__ void tmem_ld(uint32_t taddr, uint32_t (&r)[32]) { tmem_ld32(taddr, r); }
-__device__ __forceinline__ void tmem_ld(uint32_t taddr, uint32_t (&r)[16]) { tmem_ld16(taddr, r); }
-// ---- CTA pair (cta_group::2): two CTAs of a 2-CTA cluster on one 256-row tile ------------------------------------
-// A shared::cluster address with bit 24 cleared names the same offset in the EVEN CTA of the pair: TMA loads issued by
-// either CTA complete their bytes on the leader's mbarrier (cute: Sm100MmaPeerBitMask).
-constexpr uint32_t PEER_BIT_MASK = 0xFEFFFFFFu;
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tma_load_4d_cg2(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-      ::"r"(dst), "l"(map), "r"(bar & PEER_BIT_MASK), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
-}
-__device__ __forceinline__ void tma_load_3d_cg2(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1, int c2) {
-  asm volatile(
-      "cp.async.bulk.tensor.3d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-      ::"r"(dst), "l"(map), "r"(bar & PEER_BIT_MASK), "r"(c0), "r"(c1), "r"(c2) : "memory");
-}
-// arrive (no bytes) on the barrier at the same offset in CTA `rank` of the cluster
-__device__ __forceinline__ void mbar_arrive_remote(uint32_t bar, uint32_t rank) {
-  asm volatile(
-      "{\n\t.reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}"
-      ::"r"(bar), "r"(rank) : "memory");
-}
-__device__ __forceinline__ void tc_mma_cg2(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, {%5, %5, %5, %5, %5, %5, %5, %5}, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate), "r"(0u) : "memory");
-}
-// commit of the leader's MMAs: one arrival on the barrier at this offset in BOTH CTAs of the pair
-__device__ __forceinline__ void tc_commit_cg2(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(bar), "h"((uint16_t)3) : "memory");
-}
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
-// generic-proxy smem writes -> visible to the async proxy (TMA engine, tcgen05.mma operand reads)
+// generic-proxy smem writes -> visible to the async proxy (TMA engine, wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 // streaming 16-byte global load: read-only path, no L1 allocation (data is touched once)
 __device__ __forceinline__ float4 ldg_stream4(const float4* p) {
@@ -217,9 +100,69 @@ __device__ __forceinline__ float4 ldg_stream4(const float4* p) {
                : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(p));
   return v;
 }
-// UMMA shared-memory descriptor, K-major operand in the canonical 128-byte-swizzle layout (8-row groups 1024 B
-// apart, version 1 = sm_100): OR in (smem byte address >> 4) & 0x3FFF.
-constexpr uint64_t UMMA_DESC_K_SW128 = (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) | (2ull << 61);
+// named barrier over a subset of the CTA's warps (id 0 is __syncthreads)
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+
+// ---- wgmma (warpgroup MMA, sm_90a): D(64 x N, fp32 registers) += A(64 x 16, smem) * B(16 x N, smem) ----------------
+// The accumulator fragment of thread t of the warpgroup: warp w = t / 32 owns rows 16 w + (t % 32) / 4 and that + 8;
+// register 4 i + {0, 1} holds columns 8 i + 2 (t % 4) + {0, 1} of the first row, 4 i + {2, 3} the same columns of the
+// second.  Accumulators are zeroed by the caller and always accumulated into (scale-d = 1).
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// Keeps the compiler from moving accesses of an accumulator across wgmma issue / wait.
+template <int R>
+__device__ __forceinline__ void wgmma_fence_regs(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+// Shared-memory matrix descriptor, 128-byte swizzle (layout type 1 in bits 62-63), start address >> 4 OR-ed in.
+//   K-major operand: 8-row groups 1024 B apart (stride byte offset), leading byte offset unused (1).
+//   MN-major operand: 64-element MN blocks LBO bytes apart, 8-row K groups 1024 B apart.
+constexpr uint64_t GMMA_DESC_K_SW128 = (1ull << 62) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 16);
+constexpr uint64_t gmma_desc_mn_sw128(uint32_t lbo_bytes) {
+  return (1ull << 62) | ((uint64_t)(1024 >> 4) << 32) | ((uint64_t)(lbo_bytes >> 4) << 16);
+}
+__device__ __forceinline__ uint64_t gmma_desc(uint64_t hi, uint32_t smem_addr) { return hi | (uint64_t)((smem_addr >> 4) & 0x3FFFu); }
+
+#define PM_D8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
+#define PM_WGMMA_N64(TY)                                                                                   \
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"                                           \
+               "wgmma.mma_async.sync.aligned.m64n64k16.f32." TY "." TY " {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, %35;\n\t}" \
+               : PM_D8(0), PM_D8(8), PM_D8(16), PM_D8(24) \
+               : "l"(da), "l"(db), "r"(1), "n"(TRANS_B))
+template <bool BF16, int TRANS_B = 0>
+__device__ __forceinline__ void wgmma_m64n64k16(float (&d)[32], uint64_t da, uint64_t db) {
+  if constexpr (BF16) PM_WGMMA_N64("bf16");
+  else PM_WGMMA_N64("f16");
+}
+#undef PM_WGMMA_N64
+#define PM_WGMMA_N192(TY)                                                                                   \
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %98, 0;\n\t"                                           \
+               "wgmma.mma_async.sync.aligned.m64n192k16.f32." TY "." TY " {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95}, %96, %97, p, 1, 1, 0, %99;\n\t}" \
+               : PM_D8(0), PM_D8(8), PM_D8(16), PM_D8(24), PM_D8(32), PM_D8(40), PM_D8(48), PM_D8(56), PM_D8(64), PM_D8(72), PM_D8(80), PM_D8(88) \
+               : "l"(da), "l"(db), "r"(1), "n"(TRANS_B))
+template <bool BF16, int TRANS_B = 0>
+__device__ __forceinline__ void wgmma_m64n192k16(float (&d)[96], uint64_t da, uint64_t db) {
+  if constexpr (BF16) PM_WGMMA_N192("bf16");
+  else PM_WGMMA_N192("f16");
+}
+#undef PM_WGMMA_N192
+#define PM_WGMMA_N256(TY)                                                                                   \
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"                                           \
+               "wgmma.mma_async.sync.aligned.m64n256k16.f32." TY "." TY " {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1, 0, %131;\n\t}" \
+               : PM_D8(0), PM_D8(8), PM_D8(16), PM_D8(24), PM_D8(32), PM_D8(40), PM_D8(48), PM_D8(56), PM_D8(64), PM_D8(72), PM_D8(80), PM_D8(88), PM_D8(96), PM_D8(104), PM_D8(112), PM_D8(120) \
+               : "l"(da), "l"(db), "r"(1), "n"(TRANS_B))
+template <bool BF16, int TRANS_B = 0>
+__device__ __forceinline__ void wgmma_m64n256k16(float (&d)[128], uint64_t da, uint64_t db) {
+  if constexpr (BF16) PM_WGMMA_N256("bf16");
+  else PM_WGMMA_N256("f16");
+}
+#undef PM_WGMMA_N256
+#undef PM_D8
 
 // ---- host side: cuTensorMapEncodeTiled through the runtime's driver entry point (no -lcuda link dependency) ----
 // 2-byte elements (bf16 / fp16), 128-byte swizzle, zero fill out of bounds.

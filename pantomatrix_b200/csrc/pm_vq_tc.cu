@@ -1,21 +1,22 @@
-// VQ codebook lookup on the tcgen05 tensor cores: exact fp32 argmin at HBM speed.
+// VQ codebook lookup on the Hopper tensor cores (wgmma): exact fp32 argmin at HBM speed.
 //
 //   index[r] = argmin_k ( |z_r|^2 + |e_k|^2 - 2 z_r.e_k ),  first minimum wins   (M.py:60-65, P.py:158-164)
 //
 // 131 072 FLOP per 1 032-byte row is ~40x above the fp32-FMA ridge, so an exact SIMT kernel sits at a few per cent
-// of HBM bandwidth (pm_vq.cu).  Here the 256 x 256 score matrix of a 128-row tile is one fp16 UMMA chain
-// (screen), and only the rows whose two best screened distances are closer than a RIGOROUS bound on the screen's
+// of HBM bandwidth (pm_vq.cu).  Here the 128 x 256 score matrix of a 128-row tile is one fp16 MMA chain per 64-row
+// half (screen), and only the rows whose two best screened distances are closer than a RIGOROUS bound on the screen's
 // error are re-scored in exact fp32 (same expression and tie rule as the SIMT kernel).  The emitted index is
 // therefore the fp32 argmin for every row, while each row's 1 KB is read from HBM once.
 //
-// Persistent kernel, one CTA per SM, 416 threads:
-//   warps 0-7   loaders    - coalesced float4 loads of 8 full rows per warp and batch (16 x 16 B in flight per thread),
-//                            per-row max / sum of squares by warp shuffle, power-of-two row scaling into the fp16
-//                            range, fp16 conversion into the 128B-swizzled K-major UMMA layout
-//   warp  8     MMA issuer - 16 x tcgen05.mma (M=128, N=256, K=16) per tile into one of two TMEM accumulators
-//   warps 9-12  epilogue   - tcgen05.ld, screened distances d~ = e2[k] - 2 z.e (row scale folded into the FMA),
-//                            pass 1: minimum, pass 2: every k within tau of it; rows with more than one candidate
-//                            are re-scored in fp32 by the whole warp (8 lanes per candidate, shuffle reduction)
+// Persistent kernel, one CTA per SM, 384 threads:
+//   warps 0-7   two consumer warpgroups - 16 x wgmma.m64n256k16 per tile (64 rows each) into 128 fp32 registers per
+//                                         thread; screened distances d~ = e2[k] - 2 z.e (row scale folded into the FMA),
+//                                         pass 1: minimum, pass 2: every k within tau of it; rows with more than one
+//                                         candidate are re-scored in fp32 by the whole warp (8 lanes per candidate,
+//                                         shuffle reduction)
+//   warps 8-11  loaders - coalesced float4 loads of 8 full rows per warp and batch, per-row sum of squares by warp
+//                         shuffle, power-of-two row scaling into the fp16 range, fp16 conversion into the 128B-swizzled
+//                         K-major layout; they stage the next tile while the consumers run their epilogue
 // The fp16 codebook (128 KB, scaled by a power of two) stays resident in shared memory for the CTA's lifetime.
 //
 // Screen error bound (DESIGN.md section 4): both operands are rounded to fp16 (relative 2^-11 each, values scaled
@@ -30,19 +31,12 @@ namespace {
 
 constexpr int ED = 256;                 // e_dim
 constexpr int NC = 256;                 // codes
-constexpr int TM = 128;                 // rows per tile (UMMA M)
-#ifndef PM_VQ_EPI_GROUPS
-#define PM_VQ_EPI_GROUPS 2
-#endif
-constexpr int EPI_GROUPS = PM_VQ_EPI_GROUPS;           // epilogue warp groups of four taking alternate tiles.  Measured (profiles/r2/vq_*):
-                                        // with the lean passes one group is far from the bottleneck, and a second one
-                                        // (17 warps) caps the kernel at 96 registers per thread, which slows the loaders
-constexpr int LOAD_WARPS = 8, MMA_WARP = 8, EPI_WARPS = 4 * EPI_GROUPS;      // epilogue = warps 9..
-constexpr int NTHREADS = 32 * (LOAD_WARPS + 1 + EPI_WARPS);     // 416
+constexpr int TM = 128;                 // rows per tile (two 64-row warpgroups)
+constexpr int CONSUMER_WARPS = 8, LOAD_WARPS = 4;
+constexpr int NTHREADS = 32 * (CONSUMER_WARPS + LOAD_WARPS);     // 384
 constexpr int KB_A = TM * 128;          // bytes of one 64-channel k-block of the z tile (16 KB)
 constexpr int KB_B = NC * 128;          // ... of the codebook (32 KB)
 constexpr int MAXC = 8;                 // candidates kept per row (the screen's minimum included); more = "re-score every code"
-constexpr int SLOTS = 4;                // ring of per-tile row info (loaders run at most 2 tiles ahead of the epilogue)
 
 // Instrumented build only (-DPM_VQ_TIMING, tools/vq_timeline.py): clock64 cycles CTA 0 spends per phase.
 #ifdef PM_VQ_TIMING
@@ -66,11 +60,11 @@ struct Smem {
   static constexpr int B = 0;                               // fp16 codebook, 4 k-blocks
   static constexpr int A = B + 4 * KB_B;                    // fp16 z tile, 4 k-blocks
   static constexpr int E2 = A + 4 * KB_A;                   // float[256]
-  static constexpr int INFO = E2 + NC * 4;                  // float2[SLOTS][TM]: (fma multiplier, tau)
-  static constexpr int CAND = INFO + SLOTS * TM * 8;        // uint8[2 groups][TM][MAXC]
-  static constexpr int BARS = CAND + 2 * TM * MAXC;         // mbarriers
-  static constexpr int N_BARS = 2 + 2 + 2 + SLOTS + 1;      // a_full, a_empty (k-blocks 0-1), acc_full[2], acc_empty[2], info_full[SLOTS], a_empty_hi (k-blocks 2-3)
-  static constexpr int MISC = BARS + N_BARS * 8;            // tmem slot, emax
+  static constexpr int INFO = E2 + NC * 4;                  // float2[2 slots][TM]: (fma multiplier, tau)
+  static constexpr int CAND = INFO + 2 * TM * 8;            // uint8[TM][MAXC]
+  static constexpr int CNT = CAND + TM * MAXC;              // int[TM]: codes within tau per row
+  static constexpr int BARS = CNT + TM * 4;                 // a_full, a_empty
+  static constexpr int MISC = BARS + 2 * 8;                 // max |e_k|^2
   static constexpr int TOTAL = MISC + 16;
 };
 
@@ -102,10 +96,6 @@ __device__ __forceinline__ uint32_t pack_h2(float a, float b) {
   const __half2 h = __floats2half2_rn(a, b);
   return *reinterpret_cast<const uint32_t*>(&h);
 }
-__device__ __forceinline__ void prefetch_row(const float* p) {           // one 1 KB row = 8 cache lines
-#pragma unroll
-  for (int i = 0; i < 8; ++i) asm volatile("prefetch.global.L1 [%0];" ::"l"(p + 32 * i));
-}
 // exact power of two 2^s as a float, s in [-126, 127]
 __device__ __forceinline__ float pow2i(int s) { return __uint_as_float((uint32_t)(s + 127) << 23); }
 // s such that m * 2^s lies in [2^13, 2^14) for a finite normal m > 0; 0 for zero / subnormal / non-finite m
@@ -131,30 +121,21 @@ __global__ void __launch_bounds__(NTHREADS, 1) l2_argmin_tc_kernel(
   uint8_t* sm = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const uint32_t sm_u = smem_u32(sm);
   float* e2s = reinterpret_cast<float*>(sm + Smem::E2);
-  const uint32_t e2s_u = sm_u + Smem::E2, info_u = sm_u + Smem::INFO, cands_u = sm_u + Smem::CAND;   // shared-space addresses:
-  // every hot access below is an explicit ld/st.shared (generic pointers cost a 64-bit address computation each)
+  const uint32_t e2s_u = sm_u + Smem::E2, info_u = sm_u + Smem::INFO, cands_u = sm_u + Smem::CAND;
+  int* cnt = reinterpret_cast<int*>(sm + Smem::CNT);
   const uint32_t bars = sm_u + Smem::BARS;
-  const uint32_t a_full = bars, a_empty = bars + 8, acc_full = bars + 16, acc_empty = bars + 32, info_full = bars + 48;
-  const uint32_t a_empty_hi = info_full + 8 * SLOTS;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(sm + Smem::MISC);
-  float* misc_f = reinterpret_cast<float*>(sm + Smem::MISC + 4);       // [0] = max |e_k|^2
+  const uint32_t a_full = bars, a_empty = bars + 8;
+  float* misc_f = reinterpret_cast<float*>(sm + Smem::MISC);       // [0] = max |e_k|^2
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const long long n_tiles = (rows + TM - 1) / TM;
   VQ_T(t_kernel);
 
-  // ---- prologue: barriers, TMEM, resident codebook ----
+  // ---- prologue: barriers, resident codebook ----
   if (tid == 0) {
     mbar_init(a_full, LOAD_WARPS);
-    mbar_init(a_empty, 1);
-    mbar_init(a_empty_hi, 1);
-    for (int b = 0; b < 2; ++b) { mbar_init(acc_full + 8 * b, 1); mbar_init(acc_empty + 8 * b, 4); }
-    for (int s = 0; s < SLOTS; ++s) mbar_init(info_full + 8 * s, LOAD_WARPS);
+    mbar_init(a_empty, 2);                           // one arrival per consumer warpgroup
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == MMA_WARP) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(512) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
   }
   if (warp == 0) {                       // max |e_k|^2 -> codebook scale and the error bound
     float m = 0.f;
@@ -176,43 +157,37 @@ __global__ void __launch_bounds__(NTHREADS, 1) l2_argmin_tc_kernel(
     }
   }
   fence_proxy_async_smem();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp < LOAD_WARPS) {
-    // ===== loaders =====
+  if (warp >= CONSUMER_WARPS) {
+    // ===== loaders: warp lw stages tile rows 32 lw .. 32 lw + 31, eight rows per batch =====
+    const int lw = warp - CONSUMER_WARPS;
     const float bound_c = 2.0f * 0.0009765625f * 1.02f * emax;        // B = bound_c * |z|  (2 * 2^-10 * 1.02 * |e|max)
     const float inv_cb = pow2i(-s_cb);
-    // Instruction budget matters as much as bytes in flight here (ncu, profiles/r2/ncu_vq_*.md: the first version
-    // issued 37 000 warp-instructions per tile, 23 000 of them in this loop, and the SM was issue-bound at 44 % of HBM):
     //  - one row statistic only, sum of squares: the scale comes from |z| (>= every |z_d|), reduced by a halving
     //    butterfly (9 shuffles for 8 rows instead of 80) that leaves row j's total on lanes 4j..4j+3;
     //  - the owner lanes compute scale / multiplier / tau once, the scale is broadcast back with one shuffle per row;
-    //  - dense full tiles address their rows with immediates off one base pointer;
-    //  - the warp's 16 KB of the NEXT tile are pulled into L2 by one bulk prefetch a whole tile period ahead, so HBM
-    //    stays busy during the convert phases and the demand loads hit L2 (a software-pipelined variant with four
-    //    4-row quads through two register sets was measured slower: 44 % against 55 %, profiles/r2/vq_history.md).
+    //  - the warp's 32 KB of the NEXT tile are pulled into L2 by one bulk prefetch a whole tile period ahead, so HBM
+    //    stays busy during the convert phases and the demand loads hit L2.
     const bool dense = rows_per_batch == 0;
-    auto batch_base = [&](long long tl, int half) { return z + (tl * TM + warp * 16 + half * 8) * ED; };
+    auto batch_base = [&](long long tl, int q) { return z + (tl * TM + lw * 32 + q * 8) * ED; };
     int it = 0;
     for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
       const long long r0 = tile * TM;
-      const int slot = it & (SLOTS - 1);
+      const int slot = it & 1;
       const bool full = dense && r0 + TM <= rows;
+      if (lane == 0) {
+        const long long nt = tile + gridDim.x;
+        if (dense && nt * TM + TM <= rows)
+          asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(batch_base(nt, 0)), "r"(32 * ED * 4) : "memory");
+      }
 #pragma unroll 1
-      for (int half = 0; half < 2; ++half) {
-        const int rb = warp * 16 + half * 8;
+      for (int q = 0; q < 4; ++q) {
+        const int rb = lw * 32 + q * 8;
         VQ_T(t_ld);
-        if (lane == 0 && half == 0) {                      // L2 prefetch one whole tile ahead: this warp's 16 rows (16 KB)
-          const long long nt = tile + gridDim.x;
-          if (dense && nt * TM + TM <= rows)
-            asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(batch_base(nt, 0)), "r"(16 * ED * 4) : "memory");
-        }
         float4 v[8][2];
         if (full) {
-          const float4* p = reinterpret_cast<const float4*>(batch_base(tile, half)) + lane;
+          const float4* p = reinterpret_cast<const float4*>(batch_base(tile, q)) + lane;
 #pragma unroll
           for (int j = 0; j < 8; ++j) {
             v[j][0] = ldg_stream4(p + j * (ED / 4));
@@ -267,13 +242,11 @@ __global__ void __launch_bounds__(NTHREADS, 1) l2_argmin_tc_kernel(
           }
         }
         const float sc_own = pow2i(s_own);
-        if (warp == 0) VQ_ADD(0, t_ld);
+        if (lw == 0) VQ_ADD(0, t_ld);
         VQ_T(t_we);
-        // The previous tile's MMAs must have read the A tile before it is overwritten.  They release it in two halves
-        // (k-blocks 0-1, then 2-3), so the first halves of this batch's rows are stored while the MMAs of k-blocks 2-3
-        // still run.
-        if (half == 0) mbar_wait_relaxed<20>(a_empty, (uint32_t)(it & 1) ^ 1u);
-        if (warp == 0) VQ_ADD(1, t_we);
+        // the previous tile's MMAs must have read the A tile before it is overwritten
+        if (q == 0) mbar_wait_relaxed<20>(a_empty, (uint32_t)(it & 1) ^ 1u);
+        if (lw == 0) VQ_ADD(1, t_we);
         VQ_T(t_cv);
         if ((lane & 3) == 0) {
           // d~ = e2[k] + mult * acc ;  tau = 2 B + fp32 slack (covers the exact path's own rounding and flushes)
@@ -284,238 +257,175 @@ __global__ void __launch_bounds__(NTHREADS, 1) l2_argmin_tc_kernel(
         // lane holds channels 4*lane..+3 (k-block lane/16) and 128 + 4*lane..+3 (k-block 2 + lane/16)
         const uint32_t dst0 = sm_u + Smem::A + (lane >> 4) * KB_A + (uint32_t)((rb >> 3) * 1024);   // rb is a multiple of 8
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {                      // row rb + j: 8-row group rb / 8, row j within it; k-blocks 0 / 1
+        for (int j = 0; j < 8; ++j) {                      // row rb + j: 8-row group rb / 8, row j within it
           const float sc = __shfl_sync(0xffffffffu, sc_own, 4 * j);
           const uint32_t dst = dst0 + (uint32_t)(j * 128 + ((((lane & 15) >> 1) ^ j) << 4) + (lane & 1) * 8);
           sts64(dst, pack_h2(v[j][0].x * sc, v[j][0].y * sc), pack_h2(v[j][0].z * sc, v[j][0].w * sc));
+          sts64(dst + 2 * KB_A, pack_h2(v[j][1].x * sc, v[j][1].y * sc), pack_h2(v[j][1].z * sc, v[j][1].w * sc));
         }
-        if (half == 0) mbar_wait_relaxed<20>(a_empty_hi, (uint32_t)(it & 1) ^ 1u);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {                      // k-blocks 2 / 3
-          const float sc = __shfl_sync(0xffffffffu, sc_own, 4 * j);
-          const uint32_t dst = dst0 + (uint32_t)(j * 128 + ((((lane & 15) >> 1) ^ j) << 4) + (lane & 1) * 8) + 2 * KB_A;
-          sts64(dst, pack_h2(v[j][1].x * sc, v[j][1].y * sc), pack_h2(v[j][1].z * sc, v[j][1].w * sc));
-        }
-        if (warp == 0) VQ_ADD(2, t_cv);
+        if (lw == 0) VQ_ADD(2, t_cv);
       }
       fence_proxy_async_smem();
       __syncwarp();
-      if (lane == 0) { mbar_arrive(a_full); mbar_arrive(info_full + 8 * slot); }
+      if (lane == 0) mbar_arrive(a_full);
     }
-  } else if (warp == MMA_WARP) {
-    // ===== MMA issuer =====
-    // instruction descriptor: D = f32, A = B = f16, K-major, N = 256, M = 128
-    constexpr uint32_t IDESC = (1u << 4) | ((uint32_t)(NC >> 3) << 17) | ((uint32_t)(TM >> 4) << 24);
-    const uint64_t a_desc = UMMA_DESC_K_SW128 | (uint64_t)(((sm_u + Smem::A) >> 4) & 0x3FFFu);
-    const uint64_t b_desc = UMMA_DESC_K_SW128 | (uint64_t)(((sm_u + Smem::B) >> 4) & 0x3FFFu);
-    int it = 0;
-    for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
-      const int buf = it & 1;
-      VQ_T(t_m0);
-      mbar_wait(acc_empty + 8 * buf, (uint32_t)((it >> 1) & 1) ^ 1u);   // epilogue has drained this accumulator (one warp: tight spin)
-      VQ_ADD(3, t_m0);
-      VQ_T(t_m1);
-      mbar_wait(a_full, (uint32_t)(it & 1));
-      VQ_ADD(4, t_m1);
-      VQ_CNT(11, 1);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint32_t d = tmem_base + (uint32_t)buf * NC;
+    return;
+  }
+
+  // ===== consumer warpgroup wg: screen of tile rows 64 wg .. 64 wg + 63 against all 256 codes, then the argmin =====
+  const int wg = warp >> 2, t2 = 2 * (lane & 3);
+  const int rloc = (warp & 3) * 16 + (lane >> 2);          // this thread's first row within the warpgroup (and + 8)
+  const uint64_t b_desc = gmma_desc(GMMA_DESC_K_SW128, sm_u + Smem::B);
+  const uint64_t a_desc = gmma_desc(GMMA_DESC_K_SW128, sm_u + Smem::A + wg * (64 * 128));
+  int it = 0;
+  for (long long tile = blockIdx.x; tile < n_tiles; tile += gridDim.x, ++it) {
+    const int slot = it & 1;
+    float acc[NC / 2];
 #pragma unroll
-        for (int kb = 0; kb < 4; ++kb) {
+    for (int i = 0; i < NC / 2; ++i) acc[i] = 0.f;
+    VQ_T(t_m1);
+    mbar_wait(a_full, (uint32_t)(it & 1));
+    if (warp == 0) { VQ_ADD(4, t_m1); VQ_CNT(11, 1); }
+    VQ_T(t_e1);
+    wgmma_fence();
 #pragma unroll
-          for (int k = 0; k < 4; ++k)
-            tc_mma_bf16(d, a_desc + (uint64_t)(kb * (KB_A >> 4) + k * 2), b_desc + (uint64_t)(kb * (KB_B >> 4) + k * 2), IDESC,
-                        (uint32_t)((kb | k) != 0));
-          if (kb == 1) tc_commit(a_empty);                 // k-blocks 0-1 of the A tile may be overwritten
-        }
-        tc_commit(a_empty_hi);
-        tc_commit(acc_full + 8 * buf);
+    for (int kb = 0; kb < 4; ++kb)
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        wgmma_m64n256k16<false>(acc, a_desc + (uint64_t)(kb * (KB_A >> 4) + k * 2), b_desc + (uint64_t)(kb * (KB_B >> 4) + k * 2));
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(acc);
+    float2 inf[2];
+#pragma unroll
+    for (int hr = 0; hr < 2; ++hr) inf[hr] = lds64f(info_u + (uint32_t)(slot * TM + wg * 64 + rloc + 8 * hr) * 8);
+    // the A tile and this tile's row info have been read: the loaders may stage the next tile
+    named_bar_sync(1 + wg, 128);
+    if ((tid & 127) == 0) mbar_arrive(a_empty);
+
+    // pass 1: minimum of the screened distances d~ = e2[k] + mult * acc (first index wins), per thread over its 64
+    // columns in increasing order, then across the four lanes of the quad that share the row
+    float m1[2] = {INFINITY, INFINITY};
+    int k1[2] = {0, 0};
+#pragma unroll
+    for (int i = 0; i < NC / 8; ++i) {
+      const float2 e = lds64f(e2s_u + (uint32_t)(8 * i + t2) * 4);
+#pragma unroll
+      for (int hr = 0; hr < 2; ++hr) {
+        const float d0 = fmaf(inf[hr].x, acc[4 * i + 2 * hr], e.x), d1 = fmaf(inf[hr].x, acc[4 * i + 2 * hr + 1], e.y);
+        if (d0 < m1[hr]) { m1[hr] = d0; k1[hr] = 8 * i + t2; }
+        if (d1 < m1[hr]) { m1[hr] = d1; k1[hr] = 8 * i + t2 + 1; }
       }
-      __syncwarp();
     }
-  } else {
-    // ===== epilogue: TMEM lane quarter = warp % 4, thread = one row of the tile =====
-    // EPI_GROUPS groups of four warps take alternate tiles (no communication between groups).
-    const int q = warp & 3;
-    const int grp = (warp - (MMA_WARP + 1)) >> 2;            // 0 .. EPI_GROUPS-1
-    const int trow = q * 32 + lane;
-    const uint32_t cands_g = cands_u + (uint32_t)(grp * TM * MAXC);
-    int it = grp;
-    for (long long tile = blockIdx.x + (long long)grp * gridDim.x; tile < n_tiles; tile += (long long)EPI_GROUPS * gridDim.x, it += EPI_GROUPS) {
-      const int buf = it & 1, slot = it & (SLOTS - 1);
-      const long long g = tile * TM + trow;
-      VQ_T(t_e0);
-      mbar_wait_relaxed(info_full + 8 * slot, (uint32_t)((it >> 2) & 1));
-      const float2 inf = lds64f(info_u + (uint32_t)(slot * TM + trow) * 8);
-      mbar_wait_relaxed(acc_full + 8 * buf, (uint32_t)((it >> 1) & 1));
-      tc_fence_after();
-      if (warp == MMA_WARP + 1) VQ_ADD(6, t_e0);
-      VQ_T(t_e1);
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)buf * NC;
-      // pass 1: minimum of the screened distances (first index wins).  Four independent running minima (the chain
-      // of 256 dependent compare-selects was latency bound) and the next TMEM chunk in flight while this one is reduced.
-      float mm[4] = {INFINITY, INFINITY, INFINITY, INFINITY};
-      int kk[4] = {0, 1, 2, 3};
-      uint32_t accA[16], accB[16];             // 16-column chunks: two in flight cost 32 registers (the kernel is capped at 96)
-      auto reduce_chunk = [&](const uint32_t (&acc)[16], int c0) {
 #pragma unroll
-        for (int j4 = 0; j4 < 4; ++j4) {
-          const float4 e = lds128(e2s_u + (uint32_t)(c0 + 4 * j4) * 4);
-          const float d0 = fmaf(inf.x, __uint_as_float(acc[4 * j4]), e.x), d1 = fmaf(inf.x, __uint_as_float(acc[4 * j4 + 1]), e.y);
-          const float d2 = fmaf(inf.x, __uint_as_float(acc[4 * j4 + 2]), e.z), d3 = fmaf(inf.x, __uint_as_float(acc[4 * j4 + 3]), e.w);
-          if (d0 < mm[0]) { mm[0] = d0; kk[0] = c0 + 4 * j4; }
-          if (d1 < mm[1]) { mm[1] = d1; kk[1] = c0 + 4 * j4 + 1; }
-          if (d2 < mm[2]) { mm[2] = d2; kk[2] = c0 + 4 * j4 + 2; }
-          if (d3 < mm[3]) { mm[3] = d3; kk[3] = c0 + 4 * j4 + 3; }
-        }
-      };
-      tmem_ld16_issue(taddr, accA);
-#pragma unroll 1
-      for (int c0 = 0; c0 < NC; c0 += 32) {
-        tmem_ld16_wait(accA);
-        tmem_ld16_issue(taddr + c0 + 16, accB);
-        reduce_chunk(accA, c0);
-        tmem_ld16_wait(accB);
-        tmem_ld16_issue(taddr + ((c0 + 32) & (NC - 1)), accA);       // wraps to chunk 0: the first chunk of pass 2
-        reduce_chunk(accB, c0 + 16);
+    for (int hr = 0; hr < 2; ++hr)
+#pragma unroll
+      for (int o = 1; o <= 2; o <<= 1) {
+        const float om = __shfl_xor_sync(0xffffffffu, m1[hr], o);
+        const int ok = __shfl_xor_sync(0xffffffffu, k1[hr], o);
+        if (om < m1[hr] || (om == m1[hr] && ok < k1[hr])) { m1[hr] = om; k1[hr] = ok; }
       }
-      float m1 = mm[0];
-      int k1 = kk[0];
+    if (warp == 0) VQ_ADD(7, t_e1);
+    VQ_T(t_e2);
+    // pass 2: every code within tau of the minimum (the minimum itself included), listed per row in shared memory
+    const int row_w = (warp & 3) * 16 + (lane >> 2);         // row within this warp's 16 = lane >> 2 (+ 8)
+    const int crow0 = wg * 64 + row_w;                       // candidate-list row of the first of this thread's rows
+    if ((lane & 3) == 0) { cnt[crow0] = 0; cnt[crow0 + 8] = 0; }
+    __syncwarp();
 #pragma unroll
-      for (int u = 1; u < 4; ++u)
-        if (mm[u] < m1 || (mm[u] == m1 && kk[u] < k1)) { m1 = mm[u]; k1 = kk[u]; }
-      if (warp == MMA_WARP + 1) VQ_ADD(7, t_e1);
-      VQ_T(t_e2);
-      // pass 2: every code within tau of the minimum (the minimum itself included: nc >= 1)
-      const float thr = m1 + inf.y;
-      const uint32_t my = cands_g + (uint32_t)(trow * MAXC);
-      // The fully unrolled body stays tiny and branch-free: FFMA + compare + one predicated bit-set per code, one hit
-      // mask per 32 codes.  Anything bigger inline - candidate bookkeeping, even a short extraction loop per
-      // chunk - makes the pass issue / fetch bound (13 000 -> 3 700 -> ~1 500 cycles per tile, profiles/r2/vq_timeline_*).
-      uint32_t hits[8];
-      auto mask_chunk = [&](const uint32_t (&acc)[16], int c0, int bit0) {
-        uint32_t h = 0;
+    for (int i = 0; i < NC / 8; ++i) {
+      const float2 e = lds64f(e2s_u + (uint32_t)(8 * i + t2) * 4);
 #pragma unroll
-        for (int j4 = 0; j4 < 4; ++j4) {
-          const float4 e = lds128(e2s_u + (uint32_t)(c0 + 4 * j4) * 4);
-          if (fmaf(inf.x, __uint_as_float(acc[4 * j4]), e.x) <= thr) h |= 1u << (bit0 + 4 * j4);
-          if (fmaf(inf.x, __uint_as_float(acc[4 * j4 + 1]), e.y) <= thr) h |= 1u << (bit0 + 4 * j4 + 1);
-          if (fmaf(inf.x, __uint_as_float(acc[4 * j4 + 2]), e.z) <= thr) h |= 1u << (bit0 + 4 * j4 + 2);
-          if (fmaf(inf.x, __uint_as_float(acc[4 * j4 + 3]), e.w) <= thr) h |= 1u << (bit0 + 4 * j4 + 3);
-        }
-        return h;
-      };
+      for (int hr = 0; hr < 2; ++hr) {
+        const float thr = m1[hr] + inf[hr].y;
 #pragma unroll
-      for (int c = 0; c < 8; ++c) {
-        tmem_ld16_wait(accA);
-        tmem_ld16_issue(taddr + 32 * c + 16, accB);
-        hits[c] = mask_chunk(accA, 32 * c, 0);
-        tmem_ld16_wait(accB);
-        if (c < 7) tmem_ld16_issue(taddr + 32 * c + 32, accA);
-        hits[c] |= mask_chunk(accB, 32 * c + 16, 16);
-      }
-      int nc = 0;                                          // codes within tau of the minimum (the minimum included)
-#pragma unroll
-      for (int c = 0; c < 8; ++c) nc += __popc(hits[c]);
-      if (warp == MMA_WARP + 1) VQ_ADD(8, t_e2);
-      VQ_T(t_e3);
-      // accumulator drained: hand it back to the MMA warp before the (rare, slow) exact re-scoring
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(acc_empty + 8 * buf);
-      const bool flagged = nc > 1 && g < rows;            // more than one code within the screen's error bound
-      if (flagged && nc <= MAXC) {                        // ~5 % of the rows: list the candidates, pull their operands into L1
-        prefetch_row(row_ptr(g));
-        int n = 0;
-#pragma unroll
-        for (int c = 0; c < 8; ++c) {
-          uint32_t h = hits[c];
-          while (h) {
-            const int k = 32 * c + __ffs(h) - 1;
-            h &= h - 1;
-            sts8(my + (uint32_t)n, (uint32_t)k);
-            ++n;
-            prefetch_row(codebook + (long long)k * ED);
+        for (int u = 0; u < 2; ++u) {
+          if (fmaf(inf[hr].x, acc[4 * i + 2 * hr + u], u ? e.y : e.x) <= thr) {
+            const int n = atomicAdd(&cnt[crow0 + 8 * hr], 1);
+            if (n < MAXC) sts8(cands_u + (uint32_t)((crow0 + 8 * hr) * MAXC + n), (uint32_t)(8 * i + t2 + u));
           }
         }
       }
-      __syncwarp();
+    }
+    __syncwarp();
 
-      // ---- exact fp32 re-scoring of rows with more than one candidate.  Two rows per round (one per half warp: the
-      // loop is a chain of memory round trips, so two independent chains run for the price of one), two candidates at
-      // a time per row (8 lanes each: 32 elements per lane, xor-shuffle reduction - a fixed summation order). ----
-      unsigned need = __ballot_sync(0xffffffffu, flagged);
+    if (warp == 0) VQ_ADD(8, t_e2);
+    VQ_T(t_e3);
+    // ---- exact fp32 re-scoring of rows with more than one candidate: the whole warp per row, four candidates at a
+    // time (8 lanes each: 32 elements per lane, xor-shuffle reduction - a fixed summation order) ----
+    const long long gbase = tile * TM + wg * 64 + (warp & 3) * 16;     // global row of this warp's row 0
+    // bit 4 r of the first ballot = row r of the warp, of the second = row r + 8: fold both into one 16-bit row mask
+    unsigned rmask = 0;
+    {
+      const unsigned b0 = __ballot_sync(0xffffffffu, (lane & 3) == 0 && cnt[crow0] > 1 && gbase + (lane >> 2) < rows);
+      const unsigned b1 = __ballot_sync(0xffffffffu, (lane & 3) == 0 && cnt[crow0 + 8] > 1 && gbase + (lane >> 2) + 8 < rows);
+#pragma unroll
+      for (int r = 0; r < 8; ++r) rmask |= (((b0 >> (4 * r)) & 1u) << r) | (((b1 >> (4 * r)) & 1u) << (r + 8));
+    }
 #ifdef PM_VQ_TIMING
-      {
-        const unsigned over = __ballot_sync(0xffffffffu, nc > MAXC);
-        if (warp == MMA_WARP + 1) { VQ_CNT(12, __popc(need)); VQ_CNT(13, __popc(over)); }
-      }
+    if (warp == 0) { VQ_CNT(12, __popc(rmask)); }
 #endif
-      const int lg = (lane >> 3) & 1, gl = lane & 7;
-      while (need) {
-        const int sa = __ffs(need) - 1;
-        need &= need - 1;
-        int sb = sa;
-        if (need) { sb = __ffs(need) - 1; need &= need - 1; }
-        const int src = (lane & 16) ? sb : sa;                           // the row this half warp re-scores
-        const int nsrc = __shfl_sync(0xffffffffu, nc, src);
-        const bool all = nsrc > MAXC;                                    // list overflowed: every code is a candidate
-        const int ncand = all ? NC : nsrc;
-        const int nmax = max(__shfl_sync(0xffffffffu, ncand, 0), __shfl_sync(0xffffffffu, ncand, 16));
-        const float4* zr = reinterpret_cast<const float4*>(row_ptr(tile * TM + q * 32 + src));
-        float4 zv[8];
+    const int grp = lane >> 3, gl = lane & 7;
+    while (rmask) {
+      const int r = __ffs(rmask) - 1;
+      rmask &= rmask - 1;
+      const int lrow = wg * 64 + (warp & 3) * 16 + r;          // candidate-list row
+      const int nsrc = cnt[lrow];
+      const bool all = nsrc > MAXC;                             // list overflowed: every code is a candidate
+      const int ncand = all ? NC : nsrc;
+      const float4* zr = reinterpret_cast<const float4*>(row_ptr(gbase + r));
+      float4 zv[8];
 #pragma unroll
-        for (int i = 0; i < 8; ++i) zv[i] = __ldg(zr + gl + 8 * i);
-        float z2 = 0.f;
+      for (int i = 0; i < 8; ++i) zv[i] = __ldg(zr + gl + 8 * i);
+      float z2 = 0.f;
 #pragma unroll
-        for (int i = 0; i < 8; ++i) z2 = fmaf(zv[i].x, zv[i].x, fmaf(zv[i].y, zv[i].y, fmaf(zv[i].z, zv[i].z, fmaf(zv[i].w, zv[i].w, z2))));
-        z2 += __shfl_xor_sync(0xffffffffu, z2, 1);
-        z2 += __shfl_xor_sync(0xffffffffu, z2, 2);
-        z2 += __shfl_xor_sync(0xffffffffu, z2, 4);
-        float best = INFINITY;
-        int bk = NC;                                                     // NC = "nothing yet" (loses every tie)
-        const uint32_t list = cands_g + (uint32_t)((q * 32 + src) * MAXC);
+      for (int i = 0; i < 8; ++i) z2 = fmaf(zv[i].x, zv[i].x, fmaf(zv[i].y, zv[i].y, fmaf(zv[i].z, zv[i].z, fmaf(zv[i].w, zv[i].w, z2))));
+      z2 += __shfl_xor_sync(0xffffffffu, z2, 1);
+      z2 += __shfl_xor_sync(0xffffffffu, z2, 2);
+      z2 += __shfl_xor_sync(0xffffffffu, z2, 4);
+      float best = INFINITY;
+      int bk = NC;                                                     // NC = "nothing yet" (loses every tie)
+      const uint32_t list = cands_u + (uint32_t)(lrow * MAXC);
 #pragma unroll 1
-        for (int base = 0; base < nmax; base += 2) {
-          const int ci = base + lg;
-          const bool valid = ci < ncand;
-          const int c = all ? (ci & (NC - 1)) : (int)lds8(list + (valid ? ci : 0));
-          const float4* er = reinterpret_cast<const float4*>(codebook + (long long)c * ED);
-          float dot = 0.f;
+      for (int base = 0; base < ncand; base += 4) {
+        const int ci = base + grp;
+        const bool valid = ci < ncand;
+        const int c = all ? (ci & (NC - 1)) : (int)lds8(list + (valid ? ci : 0));
+        const float4* er = reinterpret_cast<const float4*>(codebook + (long long)c * ED);
+        float dot = 0.f;
 #pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const float4 ev = __ldg(er + gl + 8 * i);
-            dot = fmaf(zv[i].x, ev.x, fmaf(zv[i].y, ev.y, fmaf(zv[i].z, ev.z, fmaf(zv[i].w, ev.w, dot))));
-          }
-          dot += __shfl_xor_sync(0xffffffffu, dot, 1);
-          dot += __shfl_xor_sync(0xffffffffu, dot, 2);
-          dot += __shfl_xor_sync(0xffffffffu, dot, 4);
-          float dd = __fsub_rn(__fadd_rn(z2, lds32f(e2s_u + (uint32_t)c * 4)), __fmul_rn(2.f, dot));   // the expression of M.py:64
-          int cc = c;
-          if (!valid) { dd = INFINITY; cc = NC; }
-          const float od = __shfl_xor_sync(0xffffffffu, dd, 8);            // the other candidate of this row
-          const int oc = __shfl_xor_sync(0xffffffffu, cc, 8);
-          if (od < dd || (od == dd && oc < cc)) { dd = od; cc = oc; }
-          if (dd < best || (dd == best && cc < bk)) { best = dd; bk = cc; }
+        for (int i = 0; i < 8; ++i) {
+          const float4 ev = __ldg(er + gl + 8 * i);
+          dot = fmaf(zv[i].x, ev.x, fmaf(zv[i].y, ev.y, fmaf(zv[i].z, ev.z, fmaf(zv[i].w, ev.w, dot))));
         }
-        const int ra = __shfl_sync(0xffffffffu, bk, 0), rb = __shfl_sync(0xffffffffu, bk, 16);
-        if (lane == sa && ra < NC) k1 = ra;       // all-NaN rows keep the screen's answer (0, like torch.argmin)
-        if (lane == sb && rb < NC) k1 = rb;
+        dot += __shfl_xor_sync(0xffffffffu, dot, 1);
+        dot += __shfl_xor_sync(0xffffffffu, dot, 2);
+        dot += __shfl_xor_sync(0xffffffffu, dot, 4);
+        float dd = __fsub_rn(__fadd_rn(z2, lds32f(e2s_u + (uint32_t)c * 4)), __fmul_rn(2.f, dot));   // the expression of M.py:64
+        int cc = c;
+        if (!valid) { dd = INFINITY; cc = NC; }
+#pragma unroll
+        for (int o = 8; o <= 16; o <<= 1) {                            // the other candidates of this round
+          const float od = __shfl_xor_sync(0xffffffffu, dd, o);
+          const int oc = __shfl_xor_sync(0xffffffffu, cc, o);
+          if (od < dd || (od == dd && oc < cc)) { dd = od; cc = oc; }
+        }
+        if (dd < best || (dd == best && cc < bk)) { best = dd; bk = cc; }
       }
-      if (g < rows) index[g] = (long long)k1;
-      if (warp == MMA_WARP + 1) VQ_ADD(9, t_e3);
+      // all-NaN rows keep the screen's answer (0, like torch.argmin)
+      if (bk < NC && (lane >> 2) == (r & 7)) k1[r >> 3] = bk;
     }
+    if ((lane & 3) == 0) {
+#pragma unroll
+      for (int hr = 0; hr < 2; ++hr) {
+        const long long g = gbase + (lane >> 2) + 8 * hr;
+        if (g < rows) index[g] = (long long)k1[hr];
+      }
+    }
+    if (warp == 0) VQ_ADD(9, t_e3);
+    __syncwarp();                     // candidate lists and counters are rewritten for the next tile
   }
-
-  // teardown
-  tc_fence_before();
-  __syncthreads();
   if (warp == 0) VQ_ADD(10, t_kernel);
-  if (warp == MMA_WARP) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(512) : "memory");
-  }
 }
 
 constexpr size_t kSmem = Smem::TOTAL + 1024;

@@ -47,15 +47,14 @@ def wav_out_len(n: int) -> int:
     return length
 
 
-# Arithmetic engine of every Conv1d / Linear ("tap-GEMM"): 0 = fp32 SIMT kernel, 1/2/3 = tcgen05 tensor cores with
+# Arithmetic engine of every Conv1d / Linear ("tap-GEMM"): 0 = fp32 SIMT kernel, 1/2/3 = wgmma tensor cores with
 # 1 / 2 / 3 operand planes (csrc/pm_tapgemm_tc.cu).
-#   fp16x3 (default)  two IEEE fp16 planes (22 mantissa bits), 3 tensor-core products per fp32 product.  Measured on
-#                     B200 (round 2, profiles/README.md): all 38 400 codes of the BASELINE batch identical to the fp32
-#                     reference, latent error 4.3e-4 (bf16x6: 3.8e-4), 24 ms per step against 31 ms.  Operands must stay
+#   fp16x3 (default)  two IEEE fp16 planes (22 mantissa bits), 3 tensor-core products per fp32 product: the parity
+#                     gates of tests/test_emage_gpu.py hold as for bf16x6, at half the MMA work.  Operands must stay
 #                     below 65504 / 64 (activations are pre-scaled by 64, ops.F16_ACT_SCALE): pipeline.py checks the
 #                     outputs for the NaN an overflow would leave and names bf16x6 as the way out.
-#   bf16x6            three bf16 planes, 6 products: same accuracy, no range limit (fp32 exponent range), 1.3x slower.
-#   bf16x3 / bf16     faster, below the parity gates (measured agreement in profiles/README.md).
+#   bf16x6            three bf16 planes, 6 products: same accuracy, no range limit (fp32 exponent range), slower.
+#   bf16x3 / bf16     faster, below the parity gates.
 #   fp32              exact-order fp32 SIMT engine (reference engine of the tests).
 PRECISIONS = {"fp32": 0, "bf16": 1, "bf16x3": 2, "bf16x6": 3, "fp16x3": 2}
 PLANE_FORMAT = {"fp16x3": "fp16"}
@@ -131,7 +130,7 @@ def _record_stream(obj, stream):
 class _Fork:
     """Run independent branches of the schedule on side CUDA streams and join them on the current stream
     (the face decoder || the body stack, the three refine decoders, the four VQ part decoders).  The M = 2048
-    GEMMs of one branch fill only ~100 of the 148 SMs; overlapping branches fills the rest.  Works inside
+    GEMMs of one branch fill only ~100 of the 132 SMs; overlapping branches fills the rest.  Works inside
     CUDA-graph capture (event waits become graph edges).  Sequential when there is no CUDA device (tests)."""
 
     def __init__(self, n_side):
@@ -409,7 +408,7 @@ class _Layer:
 
 
 def _attn_tc():
-    """The tcgen05 attention kernel consumes two-plane fp16 operands: the fp16x3 engine."""
+    """The tensor-core attention kernel consumes two-plane fp16 operands: the fp16x3 engine."""
     return _STATE["nsplit"] == 2 and ops.plane_format() == "fp16"
 
 
@@ -689,7 +688,7 @@ def run_inference(engine: EmageEngine, vq: VQEngine, audio, speaker_id, masked_m
     # spill past the end: `pad` spare rows take that, and the result is the dense [:out_len] prefix (a copy only then).
     pad = max(0, max(off_t for off_t in [sum(k for _, _, k in plan[:i]) + (e - s) for i, (s, e, _) in enumerate(plan)]) - out_len)
     acc = {k + p: torch.empty(bs, out_len + pad, 256, device=dev) for k in ("rec_", "cls_") for p in PARTS}
-    # Clips are independent, and one window is a chain of ~150 dependent kernels whose GEMMs fill 48-288 of the 148 SMs:
+    # Clips are independent, and one window is a chain of ~150 dependent kernels whose GEMMs fill 48-288 of the 132 SMs:
     # the clip batch is therefore split into `groups` lanes that run their window loops on separate streams, so that
     # one lane's launch gaps, drains and epilogue tails are filled by the other lane's thread blocks (the hoisted audio
     # phase above and the final decode stay batched).  Per-clip results do not depend on the grouping.

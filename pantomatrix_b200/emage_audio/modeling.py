@@ -1,9 +1,9 @@
-"""Drop-in replacements for the reference's `models.emage_audio` modules on B200.
+"""Drop-in replacements for the reference's `models.emage_audio` modules on H100.
 
 Same class names, constructor / forward() / inference() / decode() signatures, `.cfg` attributes,
 Hugging Face checkpoint layout (state_dict keys, config.json + model.safetensors) and error behaviour
 as /root/reference/models/emage_audio/modeling_emage_audio.py (M.py) - but the modules own only the
-parameters; all arithmetic runs in the sm_100a kernels of libpm_emage.so through `engine.py`.
+parameters; all arithmetic runs in the sm_90a kernels of libpm_emage.so through `engine.py`.
 
 There is deliberately NO CPU or PyTorch-eager path: calling forward()/inference()/decode() with the
 module on a non-CUDA device, or without the built library, raises.
@@ -158,7 +158,7 @@ def _plain_state(module):
 def _require_cuda(module, what):
     dev = next(module.parameters()).device
     if dev.type != "cuda":
-        raise _lib.PmError(f"{what}: module is on {dev}; the B200 path has no CPU fallback - call .to('cuda') first")
+        raise _lib.PmError(f"{what}: module is on {dev}; the GPU path has no CPU fallback - call .to('cuda') first")
     _lib.load()
     return dev
 

@@ -1,4 +1,4 @@
-"""CaMN and DisCo audio->motion models on the B200 path (BASELINE configs[2], [3]).
+"""CaMN and DisCo audio->motion models on the H100 path (BASELINE configs[2], [3]).
 
 Same names, forward() signature, outputs, `.cfg` and checkpoint layout as
   C.py = /root/reference/models/camn_audio/modeling_camn_audio.py  (CamnAudioModel, forward 237-281)
@@ -185,7 +185,7 @@ class CamnAudioModel(CamnAudioPreTrainedModel):
         super().__init__(config)
         self.cfg, self.pose_rep, self.joint_mask = config, config.pose_rep, MASK_DICT[config.joint_mask]
         if config.pose_rep != "smplx":
-            raise NotImplementedError("only the shipped pose_rep='smplx' configuration is on the B200 path")
+            raise NotImplementedError("only the shipped pose_rep='smplx' configuration is on the GPU path")
         H, L = config.hidden_size, config.n_layer
         in_body = config.pose_dims + 1 + config.speaker_f + config.audio_f
         spec = _wav_spec("audio_encoder") + [("speaker_embedding.weight", (config.speaker_dims, config.speaker_f), "p")]

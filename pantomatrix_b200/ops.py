@@ -189,7 +189,7 @@ def attention(q, k, v, batch, heads, tq, tk, head_dim, nsplit=0, f32=True):
 
 
 def attention_tc(q, q_col0, k, k_col0, v, v_col0, batch, heads, tq, tk, head_dim, nsplit=2, f32=False):
-    """Attention on the tcgen05 tensor cores (fp16x3 engine).  q / k / v: two-plane fp16 Planes whose columns
+    """Attention on the wgmma tensor cores (fp16x3 engine).  q / k / v: two-plane fp16 Planes whose columns
     [*_col0 + h*head_dim, ...) hold head h (the packed q|k|v or k|v projection output is passed as is)."""
     for pl, rows in ((q, tq), (k, tk), (v, tk)):
         assert pl.t.dtype == torch.float16 and pl.t.shape[0] == 2 and pl.t.shape[1] == batch and pl.rows == rows, \
@@ -258,7 +258,7 @@ def _batched_rows(x, ld):
 
 
 def l2_argmin(z, codebook, e2, engine="auto", max_ctas=0):
-    """fp32 argmin_k |z - e_k|^2, first minimum wins.  engine: "auto" (the product path: tcgen05 screen + exact fp32
+    """fp32 argmin_k |z - e_k|^2, first minimum wins.  engine: "auto" (the product path: tensor-core screen + exact fp32
     re-scoring for 256-code codebooks, fp32 SIMT otherwise), "tc" or "simt" (tests / microbenchmarks)."""
     _chk(z), _chk(codebook), _chk(e2)
     assert codebook.is_contiguous()
@@ -346,7 +346,7 @@ def global_trans(rec, ref_trans, dt, vel_off=54):
 
 
 # ------------------------------------------------------------------------------------------------------
-# tcgen05 tensor-core engine: split-bf16 planes
+# wgmma tensor-core engine: split-bf16 planes
 # ------------------------------------------------------------------------------------------------------
 
 

@@ -48,7 +48,7 @@ class CapturedPipeline:
     """generate() captured once into a CUDA graph for a fixed (batch, n_samples) and replayed per call.
 
     The hot path is ~10^3 small kernel launches per step; replaying them as one graph removes the Python /
-    launch latency between kernels (B200 guide: capture launch-bound inner loops in CUDA graphs).  Inputs
+    launch latency between kernels (launch-bound inner loops belong in CUDA graphs).  Inputs
     are copied into static device buffers, outputs are static tensors owned by this object (valid until
     the next call).  Only the default-input form of the demo (masked_motion=None, mask=None) is captured.
     """
@@ -72,7 +72,7 @@ class CapturedPipeline:
         # The capture stream carries the longest dependency chain (the body stack: 1 + 8 layers per window); the face /
         # refine / part branches fork onto default-priority side streams.  Capturing on a high-priority stream makes the
         # kernel nodes of the critical chain win when both have thread blocks ready (a 96-CTA GEMM leaves 52 SMs free,
-        # which the other branch's blocks share): measured effect in profiles/README.md.
+        # which the other branch's blocks share).
         self.capture_stream = torch.cuda.Stream(device=dev, priority=-1) if body_priority else None
         with torch.cuda.graph(self.graph, stream=self.capture_stream):
             self.latent, self.pred = generate(model, motion_vq, self.audio, self.speaker_id, ref_trans=self.ref_trans)

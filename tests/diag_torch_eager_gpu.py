@@ -1,11 +1,11 @@
-"""Diagnostic (not a test): the "library baseline" on the same B200 - the oracle port of the reference run on cuda:0
+"""Diagnostic (not a test): the "library baseline" on the same GPU - the oracle port of the reference run on cuda:0
 through stock torch eager kernels (cuDNN convolutions, cuBLAS GEMMs, ATen elementwise), i.e. what a user of the
 reference gets by calling `.to("cuda")` (SURVEY §8d "reference-on-GPU" bar).  The unmodified reference cannot travel
 to the GPU box, so this times oracle/emage_oracle.py, which restates it op for op with torch.nn.functional calls;
 `sdpa=1` swaps its hand-written attention core for F.scaled_dot_product_attention (the fused path
 nn.MultiheadAttention takes in eval mode).  Same workload and timed span as bench.py (configs[1]).
 
-    python tests/diag_torch_eager_gpu.py [bs] [runs]   -> JSON lines on stdout (committed under profiles/)."""
+    python tests/diag_torch_eager_gpu.py [bs] [runs]   -> JSON lines on stdout."""
 import json
 import math
 import os

@@ -258,7 +258,7 @@ def test_baseline_config_batch32(product, ckpt, precision):
 @pytest.mark.parametrize("precision,rec_tol,min_agree", [("bf16x6", 1e-3, 0.9995), ("bf16x3", 2e-2, 0.99), ("bf16", 1.0, 0.80),
                                                          ("fp16x3", 1e-3, 0.9995)])
 def test_tensor_core_precision_modes(product, ckpt, precision, rec_tol, min_agree):
-    """The tcgen05 engine end to end (teacher-forced single windows, so a flipped code cannot cascade):
+    """The tensor-core engine end to end (teacher-forced single windows, so a flipped code cannot cascade):
     bf16x6 must meet the fp32 gate; bf16x3 / bf16 report their agreement and must stay above a floor."""
     from pantomatrix_b200.emage_audio import engine
     model, _ = product

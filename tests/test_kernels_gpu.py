@@ -17,7 +17,7 @@ def ops():
         pytest.skip("needs a CUDA device")
     from pantomatrix_b200 import _lib, ops as o
     _lib.load()
-    assert _lib.load().pm_device_cc() >= 100, "sm_100a kernels need a Blackwell device"
+    assert _lib.load().pm_device_cc() == 90, "sm_90a kernels need a Hopper (H100) device"
     return o
 
 
@@ -140,7 +140,7 @@ def test_attention(ops, bs, tq, tk):
 
 @pytest.mark.parametrize("bs,tq,tk", [(5, 64, 64), (3, 60, 60), (2, 11, 12), (2, 64, 60), (2, 1, 1), (32, 64, 64)])
 def test_attention_tc(ops, bs, tq, tk):
-    """tcgen05 attention of the fp16x3 engine: two-plane fp16 operands read in place from the packed q|k|v (self) or
+    """Tensor-core attention of the fp16x3 engine: two-plane fp16 operands read in place from the packed q|k|v (self) or
     q + k|v (cross) projection outputs; fp32 and plane outputs against float64."""
     E, H, hd = 768, 4, 192
     qkv = _rand(bs, tq, 3 * E, seed=20)
@@ -195,7 +195,7 @@ def _fp64_margins(z, cb):
     return top.indices[:, 0], top.values[:, 1] - top.values[:, 0]
 
 
-ENGINES = ["tc", "simt"]          # tcgen05 screen + exact fp32 re-scoring (the product path) | fp32 SIMT kernel
+ENGINES = ["tc", "simt"]          # tensor-core screen + exact fp32 re-scoring (the product path) | fp32 SIMT kernel
 
 
 @pytest.mark.parametrize("engine", ENGINES)

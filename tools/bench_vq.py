@@ -4,7 +4,7 @@
     python tools/bench_vq.py [--rows 2097152] [--reps 20] [--engine tc|simt|auto]
 
 Algorithmic bytes per row: 1 024 B of fp32 latent read + 8 B of int64 index written (the 256 KB codebook is
-amortised).  Inputs (rows x 1 KB) are far larger than the 126 MB L2, so every launch streams from HBM.
+amortised).  Inputs (rows x 1 KB) are far larger than the 50 MB L2, so every launch streams from HBM.
 Prints one JSON object: rows/s, GB/s, fraction of MEASURED_PEAKS.json's HBM copy bandwidth (`frac` from the median
 launch, `frac_best` from the fastest of the 20 - the peak itself is a best-of-10 copy)."""
 import argparse
@@ -39,7 +39,7 @@ def measure(rows, reps, engine="auto", max_ctas=0, scale=1.0, seed=0):
         peak = float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"])
         src = "MEASURED_PEAKS.json hbm_gbs"
     except Exception:
-        peak, src = 6650.0, "fallback (B200_PROFILING.md)"
+        peak, src = 3350.0, "H100 SXM data sheet (not measured)"
     gbs = rows * BYTES_PER_ROW / (med * 1e-3) / 1e9
     return {"kernel": "l2_argmin_tc_kernel" if engine != "simt" else "l2_argmin_kernel", "engine": engine, "rows": rows,
             "ms": med, "ms_min": ms[0], "rows_per_s": rows / (med * 1e-3), "achieved": gbs, "peak": peak, "unit": "GB/s",

@@ -11,9 +11,9 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-NAMES = ["loader: load + reduce (warp 0)", "loader: wait a_empty", "loader: convert + store", "mma: wait acc_empty", "mma: wait a_full",
-         "-", "epi: wait info + acc_full (warp 9)", "epi: pass 1", "epi: pass 2", "epi: release + re-score + store", "kernel total", "tiles",
-         "re-scored rows (warp 9)", "overflowed rows (warp 9)"]
+NAMES = ["loader: load + reduce (warp 8)", "loader: wait a_empty", "loader: convert + store", "-", "consumer: wait a_full (warp 0)",
+         "-", "-", "consumer: MMAs + pass 1", "consumer: pass 2", "consumer: re-score + store", "kernel total (warp 0)", "tiles",
+         "re-scored rows (warp 0)", "-"]
 
 
 def main(rows=1 << 21):
