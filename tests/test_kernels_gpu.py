@@ -7,6 +7,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from helpers import check_attention, check_l2_argmin, fp64_margins
 
 pytestmark = pytest.mark.gpu
 
@@ -138,30 +139,71 @@ def test_attention(ops, bs, tq, tk):
     _close(got, want, 1e-5, 1e-5)
 
 
-@pytest.mark.parametrize("bs,tq,tk", [(5, 64, 64), (3, 60, 60), (2, 11, 12), (2, 64, 60), (2, 1, 1), (32, 64, 64)])
+@pytest.mark.parametrize("bs,tq,tk", [(5, 64, 64), (3, 60, 60), (2, 11, 12), (2, 64, 60), (2, 1, 1), (32, 64, 64),
+                                      (3, 64, 11), (3, 11, 64), (1, 64, 64)])
 def test_attention_tc(ops, bs, tq, tk):
     """Tensor-core attention of the fp16x3 engine: two-plane fp16 operands read in place from the packed q|k|v (self) or
-    q + k|v (cross) projection outputs; fp32 and plane outputs against float64."""
+    q + k|v (cross) projection outputs, here at column offsets inside wider planes with columns to spare after the
+    last head; fp32, two-plane and one-plane outputs against float64, every element within its own bound
+    (helpers.attention_reference)."""
     E, H, hd = 768, 4, 192
-    qkv = _rand(bs, tq, 3 * E, seed=20)
-    kv = _rand(bs, tk, 2 * E, seed=21)
+    q0, k0 = 8, 24                                       # first column of Q inside q|k|v, of K inside k|v
+    qkv = _rand(bs, tq, q0 + 3 * E + 40, seed=20)
+    kv = _rand(bs, tk, k0 + 2 * E + 40, seed=21)
     ops.set_plane_format("fp16")
     try:
         qp, kvp = ops.split_bf16(qkv, 2), ops.split_bf16(kv, 2)
-        cross = ops.attention_tc(qp, 0, kvp, 0, kvp, E, bs, H, tq, tk, hd, nsplit=2, f32=True)
+        cross_args = (qp, q0, kvp, k0, kvp, k0 + E, bs, H, tq, tk, hd)
+        cross = ops.attention_tc(*cross_args, nsplit=2, f32=True)
+        one = ops.attention_tc(*cross_args, nsplit=1, f32=False)
         if tq == tk:
-            self_att = ops.attention_tc(qp, 0, qp, E, qp, 2 * E, bs, H, tq, tq, hd, nsplit=0)
+            self_args = (qp, q0, qp, q0 + E, qp, q0 + 2 * E, bs, H, tq, tq, hd)
+            self_att = ops.attention_tc(*self_args, nsplit=0)
     finally:
         ops.set_plane_format("bf16")
 
     def ref(q, k, v):
         q, k, v = (x.double().reshape(bs, -1, H, hd).transpose(1, 2) for x in (q, k, v))
         return (torch.softmax(q @ k.transpose(-1, -2) / math.sqrt(hd), -1) @ v).transpose(1, 2).reshape(bs * tq, E)
-    want = ref(qkv[..., :E], kv[..., :E], kv[..., E:])
+    want = ref(qkv[..., q0:q0 + E], kv[..., k0:k0 + E], kv[..., k0 + E:k0 + 2 * E])
     _close(cross.f, want, 1e-5, 1e-5)
-    assert (_planes_value(cross.p).reshape(bs * tq, E) - cross.f).abs().max() <= 2.0 ** -21 * cross.f.abs().max()
+    used = [check_attention(cross, cross_args, tag="cross")]
+    assert one.f is None and one.p.nsplit == 1
+    used.append(check_attention(one, cross_args, tag="one plane"))
+    assert torch.equal(one.p.t[0, ..., :E], cross.p.t[0, ..., :E])        # the same head plane
     if tq == tk:
-        _close(self_att, ref(qkv[..., :E], qkv[..., E:2 * E], qkv[..., 2 * E:]), 1e-5, 1e-5)
+        _close(self_att, ref(qkv[..., q0:q0 + E], qkv[..., q0 + E:q0 + 2 * E], qkv[..., q0 + 2 * E:q0 + 3 * E]), 1e-5, 1e-5)
+        used.append(check_attention(self_att, self_args, tag="self"))
+    print(f"[attention_tc {bs}x{tq}x{tk}] largest fraction of the per-element bound used: attention "
+          f"{max(u[0] for u in used):.3f}, plane split {max(u[1] for u in used):.3f}")
+
+
+def test_attention_tc_peaked_rows_and_independence(ops):
+    """Peaked softmax rows (scores up to ~40 after scaling, most probabilities far below 2^-24: ex2.approx.ftz and the
+    fp16 planes of 1024 p), and clips / heads computed alone are bit-identical to the batched call."""
+    E, H, hd, bs, t = 768, 4, 192, 6, 64
+    qkv = _rand(bs, t, 3 * E, seed=75, scale=3.2)       # s = q.k / sqrt(192) ~ N(0, 10^2)
+    ops.set_plane_format("fp16")
+    try:
+        qp = ops.split_bf16(qkv, 2)
+        args = (qp, 0, qp, E, qp, 2 * E, bs, H, t, t, hd)
+        got = ops.attention_tc(*args, nsplit=2, f32=True)
+        clips = [ops.attention_tc(ops.split_bf16(qkv[b:b + 1], 2), 0, ops.split_bf16(qkv[b:b + 1], 2), E,
+                                  ops.split_bf16(qkv[b:b + 1], 2), 2 * E, 1, H, t, t, hd, nsplit=0) for b in (0, 3, 5)]
+        heads = [ops.attention_tc(qp, h * hd, qp, E + h * hd, qp, 2 * E + h * hd, bs, 1, t, t, hd, nsplit=0) for h in range(H)]
+    finally:
+        ops.set_plane_format("bf16")
+    q = qkv[..., :E].double().reshape(bs, t, H, hd).transpose(1, 2)
+    k = qkv[..., E:2 * E].double().reshape(bs, t, H, hd).transpose(1, 2)
+    s = q @ k.transpose(-1, -2) / math.sqrt(hd)
+    assert s.abs().max() > 35 and (torch.softmax(s, -1) < 2.0 ** -24).double().mean() > 0.3     # the case is peaked
+    used = check_attention(got, args, tag="peaked")
+    print(f"[attention_tc peaked] largest fraction of the per-element bound used: attention {used[0]:.3f}, "
+          f"plane split {used[1]:.3f}")
+    for b, c in zip((0, 3, 5), clips):
+        assert torch.equal(c, got.f[b * t:(b + 1) * t]), b
+    for h, o in enumerate(heads):
+        assert torch.equal(o, got.f[:, h * hd:(h + 1) * hd]), h
 
 
 def test_broadcast_adds_are_exact(ops):
@@ -190,9 +232,7 @@ def test_window_input_matches_reference_semantics(ops):
 
 
 def _fp64_margins(z, cb):
-    d = (z.double() ** 2).sum(1, keepdim=True) + (cb.double() ** 2).sum(1) - 2 * z.double() @ cb.double().t()
-    top = d.topk(2, dim=1, largest=False)
-    return top.indices[:, 0], top.values[:, 1] - top.values[:, 0]
+    return fp64_margins(z, cb)[:2]
 
 
 ENGINES = ["tc", "simt"]          # tensor-core screen + exact fp32 re-scoring (the product path) | fp32 SIMT kernel
@@ -290,6 +330,49 @@ def test_l2_argmin_million_rows_optimality(ops):
         d = (zz ** 2).sum(1, keepdim=True) + (cb ** 2).sum(1) - 2 * zz @ cb.t()
         picked = d.gather(1, got[lo:lo + (1 << 18), None])[:, 0]
         assert bool((picked - d.min(1).values < 5e-3).all())
+
+
+@pytest.mark.parametrize("max_ctas", [1, 2, 3, 5])
+def test_l2_argmin_tc_persistent_ctas(ops, max_ctas):
+    """~40 tiles on 1-5 persistent CTAs: every CTA runs many tiles, so the A-tile handshake, the alternating INFO slots
+    and the barrier phases all turn over.  Bit-identical to one tile per CTA, and to the fp32 SIMT kernel wherever fp32
+    decides."""
+    z, cb = _rand(40 * 128 - 3, 256, seed=76), _rand(256, 256, seed=77)
+    e2 = ops.row_sqnorm(cb)
+    got = ops.l2_argmin(z, cb, e2, engine="tc", max_ctas=max_ctas)
+    assert torch.equal(got, ops.l2_argmin(z, cb, e2, engine="tc"))
+    decided, rows = check_l2_argmin(got, z, cb, tag=f"max_ctas={max_ctas}")
+    want, margin, _ = fp64_margins(z, cb)
+    ok = margin > 1e-3
+    assert torch.equal(got[ok], ops.l2_argmin(z, cb, e2, engine="simt")[ok])
+    print(f"[l2_argmin max_ctas={max_ctas}] rows decided by float64 {decided}/{rows}")
+
+
+@pytest.mark.parametrize("clips", [40, 1000])
+def test_l2_argmin_tc_strided_tails(ops, clips):
+    """The last 13 frames of 300-frame clips read in place (clip stride 300 * 256): 520 rows (5 tiles) and 13 000 rows
+    (102 tiles), also with the tiles spread over 3 persistent CTAs."""
+    x, cb = _rand(clips, 300, 256, seed=78), _rand(256, 256, seed=79)
+    e2 = ops.row_sqnorm(cb)
+    tail = x[:, 300 - 13:]
+    dense = ops.l2_argmin(tail.contiguous(), cb, e2, engine="tc")
+    for mc in (0, 3):
+        assert torch.equal(ops.l2_argmin(tail, cb, e2, engine="tc", max_ctas=mc), dense), mc
+    check_l2_argmin(dense, tail, cb, tag=f"{clips} strided tails")
+
+
+@pytest.mark.parametrize("rem", [1, 7, 8, 9, 127])
+def test_l2_argmin_tc_partial_last_tile(ops, rem):
+    """rows % 128 in {1, 7, 8, 9, 127}: the loaders' last batch of 8 rows is partial; on 2 CTAs the partial tile is a
+    CTA's later tile.  A row permutation permutes the indices exactly."""
+    rows = 5 * 128 + rem
+    z, cb = _rand(rows, 256, seed=80 + rem), _rand(256, 256, seed=81)
+    e2 = ops.row_sqnorm(cb)
+    got = ops.l2_argmin(z, cb, e2, engine="tc")
+    assert torch.equal(ops.l2_argmin(z, cb, e2, engine="tc", max_ctas=2), got)
+    check_l2_argmin(got, z, cb, tag=f"rows % 128 = {rem}")
+    perm = torch.randperm(rows, generator=torch.Generator().manual_seed(rem)).cuda()
+    assert torch.equal(ops.l2_argmin(z[perm].contiguous(), cb, e2, engine="tc", max_ctas=3), got[perm])
 
 
 def test_window_input_defaults_and_strided_seed(ops):
