@@ -178,6 +178,20 @@ int pm_pose_compose_f32(const float* face, const float* upper, const float* hand
 int pm_global_trans_f32(const float* rec, int ld, int vel_off, const float* ref_trans, int ref_bs, float dt,
                         float* trans, int batch, int t, void* stream);
 
+/* ---- audio front-end: decode output -> 16 kHz mono fp32, the resampling inside librosa.load(path, sr=16000) at
+ * test_emage_audio.py:17 (T.py:17), train_emage_audio.py:48 (TR.py:48) and test_camn_audio.py:15.
+ * pcm: interleaved (batch, n_in, channels) samples, int16 (is_int16 = 1, converted as v / 32768) or fp32 (is_int16 = 0);
+ * clip stride in_bs elements.  Channels are summed in fp32 (x.mean(axis=1) order of the host reader) and divided by
+ * `channels` (1..8, else PM_EUNSUPPORTED).  out (batch, n_out) fp32, clip stride out_bs, n_out = ceil(n_in*up/down):
+ *   out[m] = sum_k h[k] * u[(m + n_pre_remove)*down - k],  u = mono signal upsampled by zero insertion, zero outside
+ *   [0, n_in) - scipy.signal.resample_poly(padtype='constant') with h its front-padded filter.
+ * bank: (up, taps) fp32, phase-major: bank[p*taps + j] = h[p + up*j] (zero past the end); up == down == 1 with
+ * bank = {1} is the pure convert-and-mix.  fp32 FMA accumulation, each output in a fixed order (deterministic,
+ * independent of batch position).  n_in == 0 writes nothing. */
+int pm_resample_poly_f32(const void* pcm, int is_int16, long long in_bs, int batch, long long n_in, int channels,
+                         const float* bank, int up, int down, int taps, long long n_pre_remove,
+                         float* out, long long out_bs, void* stream);
+
 /* ---- CaMN / DisCo (BASELINE configs[2],[3]) ------------------------------------------------------- */
 /* One bidirectional nn.LSTM layer, zero initial state (camn:205-217,264-271; disco:212-216,255).  xproj (batch, t,
  * ldx >= 8*hidden) holds W_ih x + b_ih + b_hh for both directions (column dir*4H + gate*H + unit, gates i,f,g,o);

@@ -44,6 +44,7 @@ SIGNATURES = {
     "pm_lstm_bidir_f32": [_p, _ll, _i, _p, _p, _ll, _i, _p, _i, _i, _i, _p],
     "pm_rot6d_to_aa_f32": [_p, _ll, _i, _p, _p, _p],
     "pm_softmax2_mix_f32": [_p, _p, _p, _p, _ll, _i, _i, _p],
+    "pm_resample_poly_f32": [_p, _i, _ll, _i, _ll, _i, _p, _i, _i, _i, _ll, _p, _ll, _p],
 }
 
 _lib = None

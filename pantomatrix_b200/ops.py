@@ -128,6 +128,34 @@ def wav_stem(audio, a_bs, a_ws, batch, windows, n_samples, w1, b1, wd, bd, *, st
     return y1, sc
 
 
+def resample_poly(pcm, bank, up, down, n_pre_remove, out=None):
+    """Recorded audio -> mono fp32 at up/down times its rate (include/pm_emage.h pm_resample_poly_f32).
+
+    pcm: (batch, n_in, channels) int16 or float32, samples and channels dense (any clip stride); bank: (up, taps)
+    float32 polyphase filter (audio_io.Resampler builds it).  Returns out (batch, ceil(n_in*up/down)) float32; a given
+    `out` may be a view with any clip stride (e.g. a column range of a wider buffer)."""
+    if pcm.dtype not in (torch.int16, torch.float32):
+        raise _lib.PmError(f"resample_poly: PCM must be int16 or float32, got {pcm.dtype}")
+    if pcm.dim() != 3:
+        raise _lib.PmError(f"resample_poly: PCM must be (batch, n_in, channels), got shape {tuple(pcm.shape)}")
+    _chk(pcm, pcm.dtype), _chk(bank)
+    batch, n_in, channels = pcm.shape
+    if n_in > 1 and pcm.stride(1) != channels:
+        raise _lib.PmError("resample_poly: the samples of a clip must be dense (interleaved channels)")
+    if not bank.is_contiguous() or bank.dim() != 2 or bank.shape[0] != up:
+        raise _lib.PmError(f"resample_poly: bank must be a contiguous (up={up}, taps) tensor, got {tuple(bank.shape)}")
+    n_out = -(-n_in * up // down)
+    if out is None:
+        out = torch.empty(batch, n_out, device=pcm.device, dtype=torch.float32)
+    elif tuple(out.shape) != (batch, n_out):
+        raise _lib.PmError(f"resample_poly: out must be {(batch, n_out)}, got {tuple(out.shape)}")
+    _chk(out)
+    _call("pm_resample_poly_f32", pcm.data_ptr(), int(pcm.dtype == torch.int16), pcm.stride(0) if batch > 1 else 0,
+          batch, n_in, channels, bank.data_ptr(), int(up), int(down), bank.shape[1], int(n_pre_remove),
+          out.data_ptr(), out.stride(0) if batch > 1 else 0, _stream())
+    return out
+
+
 class Act:
     """One activation as fp32 tensor (`f`) and/or split-bf16 planes (`p`); either may be None."""
     __slots__ = ("f", "p")

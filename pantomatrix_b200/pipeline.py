@@ -53,18 +53,37 @@ class CapturedPipeline:
     the next call).  Only the default-input form of the demo (masked_motion=None, mask=None) is captured.
     """
 
-    def __init__(self, model, motion_vq, batch: int, n_samples: int, warmup: int = 2, body_priority: bool = True):
+    def __init__(self, model, motion_vq, batch: int, n_samples: int, warmup: int = 2, body_priority: bool = True,
+                 input_rate: int = 16000, input_channels: int = 1, input_dtype=torch.float32):
         self.model, self.vq = model, motion_vq
         dev = next(model.parameters()).device
         self.device = dev
-        self.audio = torch.zeros(batch, n_samples, device=dev)
+        # Recorded audio as it comes (any rate, int16 / float32, 1-8 interleaved channels): a (batch, n_samples,
+        # channels) input buffer at input_rate, and the resampling kernel as the first node of the graph, writing the
+        # 16 kHz buffer that generate() reads.  The defaults (16 kHz float32 mono) take the audio as it is.
+        self.pcm = self.resampler = None
+        if (input_rate, input_channels, input_dtype) != (16000, 1, torch.float32):
+            from .audio_io import Resampler
+            if input_dtype not in (torch.int16, torch.float32) or not 1 <= input_channels <= 8:
+                raise ValueError(f"input must be int16 or float32 with 1-8 channels, got {input_dtype} x {input_channels}")
+            self.resampler = Resampler(input_rate, 16000, device=dev)
+            self.pcm = torch.zeros(batch, n_samples, input_channels, device=dev, dtype=input_dtype)
+            self.audio = torch.zeros(batch, self.resampler.n_out(n_samples), device=dev)
+        else:
+            self.audio = torch.zeros(batch, n_samples, device=dev)
         self.speaker_id = torch.zeros(batch, 1, dtype=torch.long, device=dev)
         self.ref_trans = torch.zeros(1, 3, device=dev)
+
+        def step():
+            if self.resampler is not None:
+                self.resampler(self.pcm, out=self.audio)
+            return generate(model, motion_vq, self.audio, self.speaker_id, ref_trans=self.ref_trans)
+
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(torch.cuda.current_stream(dev))
         with torch.cuda.stream(side):                        # warm-up off the capture: lazy packing, attributes
             for _ in range(warmup):
-                generate(model, motion_vq, self.audio, self.speaker_id, ref_trans=self.ref_trans)
+                step()
         torch.cuda.current_stream(dev).wait_stream(side)
         torch.cuda.synchronize(dev)
         self.graph = torch.cuda.CUDAGraph()
@@ -75,14 +94,27 @@ class CapturedPipeline:
         # which the other branch's blocks share).
         self.capture_stream = torch.cuda.Stream(device=dev, priority=-1) if body_priority else None
         with torch.cuda.graph(self.graph, stream=self.capture_stream):
-            self.latent, self.pred = generate(model, motion_vq, self.audio, self.speaker_id, ref_trans=self.ref_trans)
+            self.latent, self.pred = step()
         self.kernels_per_replay = ops.launch_count - before
         self.nonfinite = generate.nonfinite                  # fp16 planes only: in-graph overflow flag (else None)
 
     @torch.no_grad()
     def __call__(self, audio, speaker_id=None):
-        """audio: (batch, n_samples) float32, host (pinned for async copies) or device."""
-        self.audio.copy_(audio, non_blocking=True)
+        """audio: (batch, n_samples) float32, host (pinned for async copies) or device.  With a recorded-audio input
+        (input_rate / input_channels / input_dtype): exactly (batch, n_samples, input_channels) of input_dtype, in
+        pinned host memory or on this pipeline's device."""
+        if self.pcm is None:
+            self.audio.copy_(audio, non_blocking=True)
+        else:
+            want = (tuple(self.pcm.shape), self.pcm.dtype)
+            if not torch.is_tensor(audio) or (tuple(audio.shape), audio.dtype) != want:
+                got = (tuple(audio.shape), audio.dtype) if torch.is_tensor(audio) else type(audio).__name__
+                raise ValueError(f"CapturedPipeline input must be a {want[0]} {want[1]} tensor, got {got}")
+            if audio.is_cuda and audio.device != self.pcm.device:
+                raise ValueError(f"CapturedPipeline input is on {audio.device}, the pipeline on {self.pcm.device}")
+            if not audio.is_cuda and not audio.is_pinned():
+                raise ValueError("CapturedPipeline host input must be in pinned memory (tensor.pin_memory())")
+            self.pcm.copy_(audio, non_blocking=True)
         if speaker_id is not None:
             self.speaker_id.copy_(speaker_id, non_blocking=True)
         self.graph.replay()
