@@ -122,9 +122,15 @@ int pm_attention_tc(const uint16_t* Q, long long q_ps, long long q_bs, int ldq, 
 int pm_add_rows_f32(const float* x, const float* pe, const float* spk, int first, int second,
                     float* out, int batch, int rows, int ch,
                     uint16_t* planes, long long p_ps, int p_ld, int p_nsplit, void* stream);
-/* out = a + b over n elements viewed as rows of `ch` (M.py:312,320-325) */
+/* out = a + b over n elements viewed as rows of `ch` (M.py:312,320-325): the dense case of pm_add2_strided_f32 */
 int pm_add2_f32(const float* a, const float* b, float* out, long long n, int ch,
                 uint16_t* planes, long long p_ps, int p_ld, int p_nsplit, void* stream);
+/* out[r,:] = a[r,:] + b[r,:] for `rows` rows of `ch` columns with row strides lda / ldb / ldo (column ranges of wider
+ * tensors are read and written in place, e.g. the forward and backward halves of a BiLSTM output, camn:265).
+ * Same fp32 `a + b` as pm_add2_f32; planes as there (ch % 4 == 0). */
+int pm_add2_strided_f32(const float* a, long long lda, const float* b, long long ldb, float* out, long long ldo,
+                        long long rows, long long ch,
+                        uint16_t* planes, long long p_ps, int p_ld, int p_nsplit, void* stream);
 
 /* ---- window assembly (M.py:384-391 and 267-268 fused): builds one window's motion-encoder input.
  * motion/mask: (batch, total_len, ch) full-sequence tensors, either may be NULL = inference()'s defaults (identity
@@ -200,6 +206,16 @@ int pm_resample_poly_f32(const void* pcm, int is_int16, long long in_bs, int bat
 int pm_lstm_bidir_f32(const float* xproj, long long x_bs, int ldx, const float* whh,
                       float* y, long long y_bs, int ldy, unsigned int* barrier,
                       int batch, int t, int hidden, void* stream);
+/* Conditioning columns of the layer-0 LSTM input (camn:238-263, disco:229-253): for clip b < batch, row r < t, writes
+ * out + b*o_bs + r*ldo + [0, spk_dim + pose_dims + 1) = [spk[speaker_id[b]] | seed pose | seed flag].
+ * speaker_id: int64[batch], clamped to [0, n_spk) like pm_gather_rows_f32 (range checks belong to the caller).
+ * seed: (batch, >= min(seed_frames, seed_len), pose_dims) rows with clip stride seed_bs and row stride seed_ld, nullable
+ * (= zeros); seed_len is the length of the caller's seed sequence.  Row r shows seed row j = r when r < seed_len, else
+ * j = r - (t - seed_len) (a shorter seed is extended by its own last t - seed_len rows; t <= 2*seed_len).  Seed row j is
+ * (seed[j], 1) when j < min(seed_frames, seed_len), else zeros.  A pure copy: no arithmetic. */
+int pm_lstm_cond_f32(const float* spk, long long n_spk, int spk_dim, const long long* speaker_id,
+                     const float* seed, long long seed_bs, int seed_ld, int seed_len, int seed_frames, int pose_dims,
+                     float* out, long long o_bs, int ldo, int batch, int t, void* stream);
 /* rot6d (rows, n_sel*6) of the selected joints -> axis-angle (rows, 165), zeros at unselected joints: camn:274-277.
  * slot: device int32[55], position of joint j among the selected ones or -1. */
 int pm_rot6d_to_aa_f32(const float* rot6d, long long rows, int n_sel, const int* slot, float* out, void* stream);

@@ -31,6 +31,7 @@ SIGNATURES = {
                         _p, _i, _i, _i, _i, _i, _i, _p, _ll, _i, _i, _p],
     "pm_add_rows_f32": [_p, _p, _p, _i, _i, _p, _i, _i, _i, _p, _ll, _i, _i, _p],
     "pm_add2_f32": [_p, _p, _p, _ll, _i, _p, _ll, _i, _i, _p],
+    "pm_add2_strided_f32": [_p, _ll, _p, _ll, _p, _ll, _ll, _ll, _p, _ll, _i, _i, _p],
     "pm_window_input_f32": [_p, _p, _p, _p, _p, _i, _i, _i, _i, _i, _i, _ll, _p, _ll, _i, _i, _p],
     "pm_l2_argmin_f32": [_p, _ll, _i, _ll, _p, _p, _i, _i, _p, _p],
     "pm_row_argmax_f32": [_p, _ll, _i, _i, _i, _ll, _p, _p, _p],
@@ -42,6 +43,7 @@ SIGNATURES = {
     "pm_pose_compose_f32": [_p, _p, _p, _p, _p, _p, _p, _ll, _p],
     "pm_global_trans_f32": [_p, _i, _i, _p, _i, _f, _p, _i, _i, _p],
     "pm_lstm_bidir_f32": [_p, _ll, _i, _p, _p, _ll, _i, _p, _i, _i, _i, _p],
+    "pm_lstm_cond_f32": [_p, _ll, _i, _p, _p, _ll, _i, _i, _i, _i, _p, _ll, _i, _i, _i, _p],
     "pm_rot6d_to_aa_f32": [_p, _ll, _i, _p, _p, _p],
     "pm_softmax2_mix_f32": [_p, _p, _p, _p, _ll, _i, _i, _p],
     "pm_resample_poly_f32": [_p, _i, _ll, _i, _ll, _i, _p, _i, _i, _i, _ll, _p, _ll, _p],

@@ -198,21 +198,29 @@ __global__ void __launch_bounds__(256) add_rows_kernel(
   }
 }
 
-// rows x ch (ch % 4 == 0 when planes are requested; otherwise the tensor is treated as one flat row)
+// out = a + b over `rows` rows of `ch` columns, each operand with its own row stride.  The first `nv`
+// float4 chunks of a row go through 16-byte accesses (nv = 0 when the rows are not 16-byte aligned), the remaining
+// ch - 4*nv columns element by element.  A dense tensor is one row of n elements (or n / ch rows with planes).
 template <bool F16>
-__global__ void __launch_bounds__(256) add2_kernel(const float* __restrict__ a, const float* __restrict__ b,
-                                                   float* __restrict__ out, long long n4, long long n, int ch4,
-                                                   PmPlanes P) {
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4;
-       i += (long long)gridDim.x * blockDim.x) {
-    const float4 u = reinterpret_cast<const float4*>(a)[i], v = reinterpret_cast<const float4*>(b)[i];
+__global__ void __launch_bounds__(256) add2_kernel(const float* __restrict__ a, long long lda,
+                                                   const float* __restrict__ b, long long ldb,
+                                                   float* __restrict__ out, long long ldo, long long rows,
+                                                   long long ch, long long nv, PmPlanes P) {
+  const long long i0 = (long long)blockIdx.x * blockDim.x + threadIdx.x, step = (long long)gridDim.x * blockDim.x;
+  for (long long i = i0; i < rows * nv; i += step) {
+    const long long r = rows == 1 ? 0 : i / nv, c = (i - r * nv) * 4;
+    const float4 u = *reinterpret_cast<const float4*>(a + r * lda + c);
+    const float4 v = *reinterpret_cast<const float4*>(b + r * ldb + c);
     const float4 o = make_float4(u.x + v.x, u.y + v.y, u.z + v.z, u.w + v.w);
-    if (out) reinterpret_cast<float4*>(out)[i] = o;
-    if (P.ptr) pm_store_planes4_t<F16>(P, i / ch4, (int)(i % ch4) * 4, o);
+    if (out) *reinterpret_cast<float4*>(out + r * ldo + c) = o;
+    if (P.ptr) pm_store_planes4_t<F16>(P, r, (int)c, o);
   }
-  // scalar tail (n not a multiple of 4; never with planes)
-  if (blockIdx.x == 0 && out) {
-    for (long long i = n4 * 4 + threadIdx.x; i < n; i += blockDim.x) out[i] = a[i] + b[i];
+  const long long nt = ch - 4 * nv;
+  for (long long i = i0; i < rows * nt; i += step) {
+    const long long r = i / nt, c = 4 * nv + (i - r * nt);
+    const float o = a[r * lda + c] + b[r * ldb + c];
+    if (out) out[r * ldo + c] = o;
+    if (P.ptr) pm_store_planes_t<F16>(P, r, (int)c, o);
   }
 }
 
@@ -329,17 +337,34 @@ extern "C" int pm_add_rows_f32(const float* x, const float* pe, const float* spk
   PM_LAUNCH_CHECK();
 }
 
+extern "C" int pm_add2_strided_f32(const float* a, long long lda, const float* b, long long ldb, float* out,
+                                   long long ldo, long long rows, long long ch,
+                                   uint16_t* planes, long long p_ps, int p_ld, int p_nsplit, void* stream) {
+  PM_REQUIRE(a && b && (out || planes) && rows >= 0 && ch > 0);
+  PM_REQUIRE(rows <= 1 || (lda >= ch && ldb >= ch && (!out || ldo >= ch)));
+  PM_REQUIRE(!planes || ((ch & 3) == 0 && ch <= 0x7fffffffLL));
+  PM_TAKE_FMT(p_nsplit, f16);
+  PM_REQUIRE(pm_planes_ok(planes, p_ps, p_ld, p_nsplit, (int)(planes ? ch : 1), true));
+  const PmPlanes P{reinterpret_cast<__nv_bfloat16*>(planes), p_ps, p_ld, p_nsplit};
+  if (rows == 0) return PM_OK;
+  const auto a16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
+  const bool vec = a16(a) && a16(b) && (!out || a16(out)) &&
+                   (rows == 1 || ((lda & 3) == 0 && (ldb & 3) == 0 && (!out || (ldo & 3) == 0)));
+  const long long nv = vec ? ch / 4 : 0;
+  const int grid = grid_for(rows * (nv + (ch - 4 * nv)), 256);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (f16) add2_kernel<true><<<grid, 256, 0, st>>>(a, lda, b, ldb, out, ldo, rows, ch, nv, P);
+  else add2_kernel<false><<<grid, 256, 0, st>>>(a, lda, b, ldb, out, ldo, rows, ch, nv, P);
+  PM_LAUNCH_CHECK();
+}
+
 extern "C" int pm_add2_f32(const float* a, const float* b, float* out, long long n, int ch,
                            uint16_t* planes, long long p_ps, int p_ld, int p_nsplit, void* stream) {
   PM_REQUIRE(a && b && (out || planes) && n >= 0);
   PM_REQUIRE(!planes || (ch > 0 && (ch & 3) == 0 && n % ch == 0));
-  PM_TAKE_FMT(p_nsplit, f16);
-  PM_REQUIRE(pm_planes_ok(planes, p_ps, p_ld, p_nsplit, ch, true));
-  const PmPlanes P{reinterpret_cast<__nv_bfloat16*>(planes), p_ps, p_ld, p_nsplit};
   if (n == 0) return PM_OK;
-  if (f16) add2_kernel<true><<<grid_for(n / 4 + 1, 256), 256, 0, (cudaStream_t)stream>>>(a, b, out, n / 4, n, planes ? ch / 4 : 1, P);
-  else add2_kernel<false><<<grid_for(n / 4 + 1, 256), 256, 0, (cudaStream_t)stream>>>(a, b, out, n / 4, n, planes ? ch / 4 : 1, P);
-  PM_LAUNCH_CHECK();
+  const long long rows = planes ? n / ch : 1, cols = planes ? ch : n;        // the dense case of the strided add
+  return pm_add2_strided_f32(a, cols, b, cols, out, cols, rows, cols, planes, p_ps, p_ld, p_nsplit, stream);
 }
 
 extern "C" int pm_window_input_f32(const float* motion, const float* mask, const float* seed,

@@ -155,7 +155,54 @@ __global__ void __launch_bounds__(NT, 1) lstm_bidir_kernel(LstmParams p) {
   }
 }
 
+// Conditioning columns of the layer-0 input, one thread per output element: [speaker row | seed pose | seed flag].
+// Output row r of a clip shows seed row j = r, or r - (t - seed_len) past the end of a shorter seed (the appended
+// copy of its last t - seed_len rows); rows j < seed_frames carry (seed[j], 1), the others zeros.
+__global__ void __launch_bounds__(256) lstm_cond_kernel(
+    const float* __restrict__ spk, long long n_spk, int spk_dim, const long long* __restrict__ speaker_id,
+    const float* __restrict__ seed, long long seed_bs, int seed_ld, int seed_len, int seed_frames, int pose_dims,
+    float* __restrict__ out, long long o_bs, int ldo, int batch, int t) {
+  const int cols = spk_dim + pose_dims + 1;
+  const long long total = (long long)batch * t * cols;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
+       i += (long long)gridDim.x * blockDim.x) {
+    const int c = (int)(i % cols);
+    const long long bt = i / cols;
+    const int r = (int)(bt % t);
+    const long long b = bt / t;
+    float v;
+    if (c < spk_dim) {
+      long long k = speaker_id[b];                 // clamped like pm_gather_rows_f32: never read outside the table
+      k = k < 0 ? 0 : (k >= n_spk ? n_spk - 1 : k);
+      v = spk[k * spk_dim + c];
+    } else {
+      const int j = r < seed_len ? r : r - (t - seed_len);
+      const bool flagged = j < seed_frames;
+      const int k = c - spk_dim;
+      v = k == pose_dims ? (flagged ? 1.f : 0.f)
+                         : (flagged && seed ? seed[b * seed_bs + (long long)j * seed_ld + k] : 0.f);
+    }
+    out[b * o_bs + (long long)r * ldo + c] = v;
+  }
+}
+
 }  // namespace
+
+extern "C" int pm_lstm_cond_f32(const float* spk, long long n_spk, int spk_dim, const long long* speaker_id,
+                                const float* seed, long long seed_bs, int seed_ld, int seed_len, int seed_frames,
+                                int pose_dims, float* out, long long o_bs, int ldo, int batch, int t, void* stream) {
+  PM_REQUIRE(spk && speaker_id && out && n_spk > 0 && spk_dim >= 0 && pose_dims >= 0 && batch >= 0 && t >= 0);
+  PM_REQUIRE(ldo >= spk_dim + pose_dims + 1 && seed_frames >= 0 && seed_len > 0 && t <= 2LL * seed_len);
+  PM_REQUIRE(!seed || seed_ld >= pose_dims);
+  if (seed_frames > seed_len) seed_frames = seed_len;
+  const long long total = (long long)batch * t * (spk_dim + pose_dims + 1);
+  if (total == 0) return PM_OK;
+  long long g = (total + 255) / 256;
+  if (g > 148 * 16) g = 148 * 16;
+  lstm_cond_kernel<<<(unsigned)g, 256, 0, (cudaStream_t)stream>>>(spk, n_spk, spk_dim, speaker_id, seed, seed_bs, seed_ld,
+                                                                 seed_len, seed_frames, pose_dims, out, o_bs, ldo, batch, t);
+  PM_LAUNCH_CHECK();
+}
 
 extern "C" int pm_lstm_bidir_f32(const float* xproj, long long x_bs, int ldx, const float* whh,
                                  float* y, long long y_bs, int ldy, unsigned int* barrier,

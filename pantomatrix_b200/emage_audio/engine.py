@@ -327,8 +327,9 @@ class _WavEncoder:
                 self.blocks.append((_Conv(_taps(w1), b1.contiguous(), stride, pad), _Conv(_taps(w2), b2.contiguous(), 1, 7),
                                     _Conv(_taps(ds[0]), ds[1].contiguous(), stride, pad) if ds else None))
 
-    def __call__(self, audio, offset, a_ws, windows, n_samples):
-        """audio (bs, n) contiguous; returns (windows*bs, frames, out_dim), window-major."""
+    def __call__(self, audio, offset, a_ws, windows, n_samples, out=None):
+        """audio (bs, n) contiguous; returns (windows*bs, frames, out_dim), window-major.  out: optional fp32 view
+        (e.g. a column range of a wider tensor) the last conv writes its result into."""
         bs, n = audio.shape
         w1, b1, wd, bd, stride, pad = self.stem
         y, sc = ops.wav_stem(audio, n, a_ws, bs, windows, n_samples, w1, b1, wd, bd, stride=stride, pad=pad,
@@ -342,7 +343,8 @@ class _WavEncoder:
         for i, (conv1, conv2, ds) in enumerate(self.blocks[1:], 1):
             y = conv1(x, act=ops.ACT_LEAKY, slope=0.01, want="p")
             sc = ds(x) if ds is not None else x
-            x = conv2(y, act=ops.ACT_LEAKY, slope=0.01, residual=sc, want=form(i), out_slack=8)
+            x = conv2(y, act=ops.ACT_LEAKY, slope=0.01, residual=sc, want=form(i), out_slack=8,
+                      out=out if i == last else None)
         return x
 
 

@@ -246,13 +246,59 @@ def add_rows(x, pe, spk, first, second, batch, rows, ch, nsplit=0, f32=True):
 
 
 def add2(a, b, nsplit=0, f32=True):
+    """a + b.  Dense operands, or (fp32 out only) (..., ch) views with evenly spaced rows - e.g. the two column halves of
+    a BiLSTM output, read in place (pm_add2_strided_f32, same fp32 a + b).  Returns a dense tensor / Act."""
     _chk(a), _chk(b)
-    assert a.is_contiguous() and b.is_contiguous() and a.shape == b.shape
+    assert a.shape == b.shape, (a.shape, b.shape)
+    if not (a.is_contiguous() and b.is_contiguous()):
+        assert nsplit == 0, "strided add2 writes fp32 only"
+        out = torch.empty(a.shape, device=a.device, dtype=torch.float32)
+        rows, lda = _rows_ld(a)
+        _call("pm_add2_strided_f32", a.data_ptr(), lda, b.data_ptr(), _rows_ld(b)[1], out.data_ptr(), a.shape[-1],
+              rows, a.shape[-1], None, 0, 0, 0, _stream())
+        return out
     out = torch.empty_like(a) if (f32 or not nsplit) else None
     ch = a.shape[-1]
     pl = _new_planes(nsplit, (a.shape[0], a.numel() // ch // a.shape[0]), ch, a.device) if nsplit else None
     _call("pm_add2_f32", a.data_ptr(), b.data_ptr(), _ptr(out), a.numel(), ch, *_pargs(pl), _stream())
     return _result(out, pl, nsplit)
+
+
+def _rows_ld(t):
+    """(rows, row stride) of a (..., ch) view whose rows all lie one stride apart (e.g. a column range)."""
+    ch = t.shape[-1]
+    rows = t.numel() // ch if ch else 0
+    lead = [(n, s) for n, s in zip(t.shape[:-1], t.stride()[:-1]) if n > 1]
+    ld = lead[-1][1] if lead else ch
+    want = ld
+    for n, s in reversed(lead):
+        if s != want:
+            raise _lib.PmError(f"rows of a {tuple(t.shape)} view with strides {t.stride()} are not evenly spaced")
+        want = s * n
+    return rows, ld
+
+
+def lstm_cond(spk, speaker_id, seed, seed_len, seed_frames, pose_dims, out):
+    """Speaker row + seed columns of the layer-0 LSTM input, written into `out` (batch, t, spk_dim + pose_dims + 1), a
+    column range of that input (include/pm_emage.h pm_lstm_cond_f32).  speaker_id int64 (batch,) or (batch, 1), clamped
+    into the table; seed (batch, rows, pose_dims) with dense rows or None (zeros); seed_len is the length of the
+    sequence the seed stands for (row mapping in the header)."""
+    _chk(spk), _chk(speaker_id, torch.int64), _chk(out)
+    assert spk.is_contiguous() and speaker_id.is_contiguous()
+    batch, t, cols = out.shape
+    assert speaker_id.numel() == batch and cols == spk.shape[1] + pose_dims + 1, (speaker_id.shape, out.shape)
+    o_bs, ldo = _bs_ld(out)
+    s_bs = s_ld = 0
+    if seed is not None:
+        _chk(seed)
+        assert seed.dim() == 3 and seed.shape[0] == batch and seed.shape[2] == pose_dims, (seed.shape, batch, pose_dims)
+        if seed.numel() == 0:
+            seed = None
+        else:
+            s_bs, s_ld = _bs_ld(seed)
+    _call("pm_lstm_cond_f32", spk.data_ptr(), spk.shape[0], spk.shape[1], speaker_id.data_ptr(), _ptr(seed), s_bs, s_ld,
+          int(seed_len), int(seed_frames), int(pose_dims), out.data_ptr(), o_bs, ldo, batch, t, _stream())
+    return out
 
 
 def window_input(motion, mask, seed, mask_embedding, start, win_len, pre, nsplit=0, f32=True, shape=None):

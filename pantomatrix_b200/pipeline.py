@@ -44,6 +44,36 @@ def generate(model, motion_vq, audio, speaker_id=None, masked_motion=None, mask=
 generate.nonfinite = None
 
 
+def _audio_input(batch, n_samples, dev, input_rate, input_channels, input_dtype):
+    """Static audio buffers of a captured pipeline: (pcm, resampler, audio).  Recorded audio as it comes (any rate,
+    int16 / float32, 1-8 interleaved channels) lands in a (batch, n_samples, channels) pcm buffer, and the resampling
+    kernel - the first node of the graph - writes the 16 kHz buffer the model reads.  The defaults (16 kHz float32 mono)
+    take the audio as it is: pcm and resampler are None."""
+    if (input_rate, input_channels, input_dtype) == (16000, 1, torch.float32):
+        return None, None, torch.zeros(batch, n_samples, device=dev)
+    from .audio_io import Resampler
+    if input_dtype not in (torch.int16, torch.float32) or not 1 <= input_channels <= 8:
+        raise ValueError(f"input must be int16 or float32 with 1-8 channels, got {input_dtype} x {input_channels}")
+    resampler = Resampler(input_rate, 16000, device=dev)
+    pcm = torch.zeros(batch, n_samples, input_channels, device=dev, dtype=input_dtype)
+    return pcm, resampler, torch.zeros(batch, resampler.n_out(n_samples), device=dev)
+
+
+def _stage(dst, src, who, exact):
+    """Copy one call's input into its static buffer (asynchronously).  exact: the input must have the buffer's shape
+    and dtype and sit in pinned host memory or on the buffer's device (recorded audio; nothing is converted)."""
+    if exact:
+        want = (tuple(dst.shape), dst.dtype)
+        if not torch.is_tensor(src) or (tuple(src.shape), src.dtype) != want:
+            got = (tuple(src.shape), src.dtype) if torch.is_tensor(src) else type(src).__name__
+            raise ValueError(f"{who} input must be a {want[0]} {want[1]} tensor, got {got}")
+        if src.is_cuda and src.device != dst.device:
+            raise ValueError(f"{who} input is on {src.device}, the pipeline on {dst.device}")
+        if not src.is_cuda and not src.is_pinned():
+            raise ValueError(f"{who} host input must be in pinned memory (tensor.pin_memory())")
+    dst.copy_(src, non_blocking=True)
+
+
 class CapturedPipeline:
     """generate() captured once into a CUDA graph for a fixed (batch, n_samples) and replayed per call.
 
@@ -58,19 +88,7 @@ class CapturedPipeline:
         self.model, self.vq = model, motion_vq
         dev = next(model.parameters()).device
         self.device = dev
-        # Recorded audio as it comes (any rate, int16 / float32, 1-8 interleaved channels): a (batch, n_samples,
-        # channels) input buffer at input_rate, and the resampling kernel as the first node of the graph, writing the
-        # 16 kHz buffer that generate() reads.  The defaults (16 kHz float32 mono) take the audio as it is.
-        self.pcm = self.resampler = None
-        if (input_rate, input_channels, input_dtype) != (16000, 1, torch.float32):
-            from .audio_io import Resampler
-            if input_dtype not in (torch.int16, torch.float32) or not 1 <= input_channels <= 8:
-                raise ValueError(f"input must be int16 or float32 with 1-8 channels, got {input_dtype} x {input_channels}")
-            self.resampler = Resampler(input_rate, 16000, device=dev)
-            self.pcm = torch.zeros(batch, n_samples, input_channels, device=dev, dtype=input_dtype)
-            self.audio = torch.zeros(batch, self.resampler.n_out(n_samples), device=dev)
-        else:
-            self.audio = torch.zeros(batch, n_samples, device=dev)
+        self.pcm, self.resampler, self.audio = _audio_input(batch, n_samples, dev, input_rate, input_channels, input_dtype)
         self.speaker_id = torch.zeros(batch, 1, dtype=torch.long, device=dev)
         self.ref_trans = torch.zeros(1, 3, device=dev)
 
@@ -104,17 +122,9 @@ class CapturedPipeline:
         (input_rate / input_channels / input_dtype): exactly (batch, n_samples, input_channels) of input_dtype, in
         pinned host memory or on this pipeline's device."""
         if self.pcm is None:
-            self.audio.copy_(audio, non_blocking=True)
+            _stage(self.audio, audio, "CapturedPipeline", exact=False)
         else:
-            want = (tuple(self.pcm.shape), self.pcm.dtype)
-            if not torch.is_tensor(audio) or (tuple(audio.shape), audio.dtype) != want:
-                got = (tuple(audio.shape), audio.dtype) if torch.is_tensor(audio) else type(audio).__name__
-                raise ValueError(f"CapturedPipeline input must be a {want[0]} {want[1]} tensor, got {got}")
-            if audio.is_cuda and audio.device != self.pcm.device:
-                raise ValueError(f"CapturedPipeline input is on {audio.device}, the pipeline on {self.pcm.device}")
-            if not audio.is_cuda and not audio.is_pinned():
-                raise ValueError("CapturedPipeline host input must be in pinned memory (tensor.pin_memory())")
-            self.pcm.copy_(audio, non_blocking=True)
+            _stage(self.pcm, audio, "CapturedPipeline", exact=True)
         if speaker_id is not None:
             self.speaker_id.copy_(speaker_id, non_blocking=True)
         self.graph.replay()
@@ -122,3 +132,98 @@ class CapturedPipeline:
         if self.nonfinite is not None and bool(self.nonfinite):     # one 4-byte read back per step (fp16 planes only)
             raise _lib.PmError(_OVERFLOW)
         return self.latent, self.pred
+
+
+def _memset0(t):
+    _lib.call("pm_memset_async", t.data_ptr(), 0, t.numel() * t.element_size(), torch.cuda.current_stream(t.device).cuda_stream)
+
+
+class CapturedLstmPipeline:
+    """CaMN / DisCo forward() captured once into a CUDA graph for a fixed (batch, n_samples) and replayed per call.
+
+    model: a CamnAudioModel or DiscoAudioModel.  The graph holds library kernels and memset nodes only: the optional
+    resampling of recorded audio (input_rate / input_channels / input_dtype, as in CapturedPipeline), the WavEncoder,
+    the in-place assembly of the LSTM inputs, the recurrences and the heads.  Speaker ids and the first seed_frames seed
+    poses are static inputs.  The pipeline owns the LSTM barrier scratch, so an eager forward() of the same model on
+    another stream cannot interfere with a replay.  The precision mode in effect at construction is the one captured;
+    in fp16x3 an in-graph flag turns an operand overflow into PmError after the replay.  Outputs are a static dict with
+    the keys of forward(), valid until the next call."""
+
+    def __init__(self, model, batch: int, n_samples: int, seed_frames: int = 4, warmup: int = 2,
+                 input_rate: int = 16000, input_channels: int = 1, input_dtype=torch.float32):
+        from .lstm_audio.modeling import wav_frames
+        if seed_frames < 0:
+            raise ValueError(f"seed_frames must be >= 0, got {seed_frames}")
+        dev = next(model.parameters()).device
+        self.model, self.device, self.batch, self.seed_frames = model, dev, batch, seed_frames
+        self.pcm, self.resampler, self.audio = _audio_input(batch, n_samples, dev, input_rate, input_channels, input_dtype)
+        eng = model._eng()
+        self.speaker_dims, self.pose_dims = eng.spk.shape[0], eng.pose_dims
+        self.speaker_id = torch.zeros(batch, 1, dtype=torch.long, device=dev)
+        self.seed = torch.zeros(batch, seed_frames, self.pose_dims, device=dev)
+        self.barrier = torch.zeros(4, dtype=torch.int32, device=dev)
+        t = wav_frames(self.audio.shape[1])
+        guard = ops.plane_format() == "fp16"
+
+        @torch.no_grad()
+        def step():
+            if self.resampler is not None:
+                self.resampler(self.pcm, out=self.audio)
+            # seed_len = t: the seed buffer stands for a t-frame seed whose rows past seed_frames are zeros, which is
+            # forward(seed_motion=x) for any x of length t with these first rows (and forward(seed_motion=None) for zeros)
+            out = eng.forward(self.audio, eng.kernel_cond(self.speaker_id, self.seed, t, seed_frames), True,
+                              barrier=self.barrier)
+            flag = None
+            if guard:                      # an fp16 operand overflow leaves NaN in the motion: the argmax kernel flags it
+                flag = ops.zero_flag(dev)
+                ops.row_argmax(out["motion"], nonfinite=flag)
+            return out, flag
+
+        side = torch.cuda.Stream(device=dev)
+        side.wait_stream(torch.cuda.current_stream(dev))
+        with torch.cuda.stream(side):                        # warm-up off the capture: lazy packing, attributes
+            for _ in range(warmup):
+                step()
+        torch.cuda.current_stream(dev).wait_stream(side)
+        torch.cuda.synchronize(dev)
+        self.graph = torch.cuda.CUDAGraph()
+        before = ops.launch_count
+        with torch.cuda.graph(self.graph):
+            self.out, self.nonfinite = step()
+        self.kernels_per_replay = ops.launch_count - before
+
+    def _stage_inputs(self, audio, speaker_id, seed_motion):
+        """Validate one call's inputs and copy them into the static buffers (asynchronously)."""
+        if self.pcm is None:
+            _stage(self.audio, audio, "CapturedLstmPipeline", exact=False)
+        else:
+            _stage(self.pcm, audio, "CapturedLstmPipeline", exact=True)
+        if speaker_id is None:
+            _memset0(self.speaker_id)
+        else:
+            if not torch.is_tensor(speaker_id) or tuple(speaker_id.shape) != (self.batch, 1) or speaker_id.dtype != torch.int64:
+                got = (tuple(speaker_id.shape), speaker_id.dtype) if torch.is_tensor(speaker_id) else type(speaker_id).__name__
+                raise ValueError(f"speaker_id must be a ({self.batch}, 1) int64 tensor, got {got}")
+            lo, hi = int(speaker_id.min()), int(speaker_id.max())
+            if lo < 0 or hi >= self.speaker_dims:
+                raise ValueError(f"speaker_id must lie in [0, {self.speaker_dims}), got values in [{lo}, {hi}]")
+            self.speaker_id.copy_(speaker_id, non_blocking=True)
+        if seed_motion is None:
+            _memset0(self.seed)
+        else:
+            want = (self.batch, self.seed_frames, self.pose_dims)
+            if not torch.is_tensor(seed_motion) or tuple(seed_motion.shape) != want or seed_motion.dtype != torch.float32:
+                got = (tuple(seed_motion.shape), seed_motion.dtype) if torch.is_tensor(seed_motion) else type(seed_motion).__name__
+                raise ValueError(f"seed_motion must be a {want} float32 tensor or None, got {got}")
+            self.seed.copy_(seed_motion, non_blocking=True)
+
+    @torch.no_grad()
+    def __call__(self, audio, speaker_id=None, seed_motion=None):
+        """audio as for CapturedPipeline; speaker_id (batch, 1) int64 in [0, speaker_dims), None = zeros; seed_motion
+        (batch, seed_frames, pose_dims) float32 rot6d of the first frames, None = zeros (= forward(seed_motion=None))."""
+        self._stage_inputs(audio, speaker_id, seed_motion)
+        self.graph.replay()
+        ops.launch_count += self.kernels_per_replay
+        if self.nonfinite is not None and bool(self.nonfinite):     # one 4-byte read back per step (fp16 planes only)
+            raise _lib.PmError(_OVERFLOW)
+        return self.out
