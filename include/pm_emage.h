@@ -30,6 +30,7 @@ extern "C" {
 
 #define PM_ABI_VERSION 5
 #define PM_FMT_F16 0x100
+#define PM_TC_TILE_SHIFT 16   /* pm_tapgemm_tc: N tile override in bits 16-23 of `nsplit` */
 int pm_abi_version(void);
 /* cudaMemsetAsync on `stream` (a memset node under graph capture, not a kernel): zeroed slack rows, flags */
 int pm_memset_async(void* ptr, int value, long long bytes, void* stream);
@@ -55,8 +56,10 @@ int pm_tapgemm_f32(const float* A, long long a_bs, int lda, int batch, int rows_
  * Same contract as pm_tapgemm_f32 with stride == 1 (strided convs are passed as stride-1 problems over the
  * (rows/s, s*cin) view of the input with zero-padded taps).  A and W are `nsplit` bf16 planes (x = p0+p1+p2),
  * plane strides a_ps / w_ps elements: nsplit 1 = plain bf16, 2 = bf16x3 (p0*p0 + p0*p1 + p1*p0), 3 = bf16x6
- * (all products down to 2^-24).  W planes are (taps, w_rows, ldw) with w_rows >= cout a multiple of the N
- * tile (64), zero rows beyond cout.  lda, ldw, a_bs, a_ps, w_ps must be multiples
+ * (all products down to 2^-24).  W planes are (taps, w_rows, ldw) with w_rows >= cout a multiple of 64, zero
+ * rows beyond cout; 128-column N tiles are used only when w_rows is a multiple of 128.  The N tile is chosen from
+ * the shape and the SM count unless (nsplit >> PM_TC_TILE_SHIFT) & 0xff forces it: 1 = 64, 2 = 128 columns (tests,
+ * A/B runs).  Both tiles give bit-identical results.  lda, ldw, a_bs, a_ps, w_ps must be multiples
  * of 8 elements (TMA 16-byte rule).  The activation is applied to columns < act_cols only (<=0: all).
  * The epilogue writes the fp32 result and/or its bf16 split planes (out_f32 / out_bf16 nullable).
  * Operands are staged by TMA (cp.async.bulk.tensor, zero fill for padding rows, tap shift folded into the

@@ -6,14 +6,16 @@
 // (p0*p0 + p0*p1 + p1*p0), 3 = bf16x6 (every product down to 2^-24): all products accumulate in fp32 registers, so
 // the result has fp32-grade accuracy at tensor-core rates.
 //
-// Structure (one 128 x BN output tile per CTA, 288 threads):
-//   warps 0-7  two consumer warpgroups - warpgroup g issues wgmma.m64nBNk16 for tile rows 64 g .. 64 g + 63 out of
-//                                        the shared operand stage, then runs the epilogue: registers -> smem tile ->
-//                                        bias / residual / activation -> coalesced fp32 store and/or split planes
-//   warp 8     TMA producer             - cp.async.bulk.tensor: A box (64 ch x R rows x NB clips) per plane, with the
-//                                        tap shift folded into the row coordinate (im2col-free; padding rows are TMA
-//                                        zero fill), W box (64 ch x 64 rows) per plane; 128B-swizzled K-major smem
-//                                        tiles; mbarrier ring
+// Structure (one 128 x BN output tile per CTA, BN = 64 or 128 chosen per launch on the host, 384 threads):
+//   warpgroup 0      producer, 40 registers per thread (setmaxnreg.dec) -
+//                      warp 0: TMA (one elected lane): A box (64 ch x R rows x NB clips) per plane, with the tap shift
+//                              folded into the row coordinate (im2col-free; padding rows are TMA zero fill), W box
+//                              (64 ch x BN rows) per plane; 128B-swizzled K-major smem tiles; mbarrier ring
+//                      warp 1: L2 prefetch of the next GEMM's weights; warps 2-3 exit at once
+//   warpgroups 1-2   consumers, 232 registers per thread (setmaxnreg.inc) - consumer warpgroup g issues
+//                      wgmma.m64nBNk16 for tile rows 64 g .. 64 g + 63 out of the shared operand stage into three
+//                      BN / 2-register accumulators, then runs the epilogue: registers -> smem tile ->
+//                      bias / residual / activation -> coalesced fp32 store and/or split planes
 // Contract and reference call sites: include/pm_emage.h (pm_tapgemm_tc).
 #include <cuda.h>
 #include <stdio.h>
@@ -30,8 +32,16 @@ constexpr int BM = 128;             // tile rows (two 64-row warpgroups)
 constexpr int BK = 64;              // bf16 channels per k-block = one 128-byte swizzle row
 constexpr int MMA_K = 16;
 constexpr int A_TILE_BYTES = BM * BK * 2;           // 16 KB per plane
+constexpr int PRODUCER_THREADS = 128;
 constexpr int CONSUMER_THREADS = 256;
-constexpr int NUM_THREADS = CONSUMER_THREADS + 32;  // two consumer warpgroups + the TMA warp
+constexpr int NUM_THREADS = PRODUCER_THREADS + CONSUMER_THREADS;   // producer warpgroup + two consumer warpgroups
+// The CTA is launched with 168 registers per thread (the most 384 threads get: 65536 / 384 rounded down to 8).  The
+// producer hands 128 of every thread's registers back, and the consumers take them: three m64n128 accumulators are
+// 192 registers per thread.  setmaxnreg.inc waits until the pool holds what it asks for, so the split must add up.
+constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;
+static_assert(PRODUCER_THREADS * PRODUCER_REGS + CONSUMER_THREADS * CONSUMER_REGS == (65536 / NUM_THREADS & ~7) * NUM_THREADS,
+              "the setmaxnreg split must use exactly the launch's register pool");
+constexpr int STAMP_WARP = PRODUCER_THREADS / 32;   // first consumer warp: writes the PM_TC_TIMING stamps
 constexpr int MAX_STAGES = 8;
 constexpr int RING_KB = 200;        // operand ring per CTA (one CTA per SM; 227 KB is the sm_90 limit)
 
@@ -68,8 +78,9 @@ __device__ unsigned long long pm_tc_stamps[4096 * 8];
 
 template <int BN, bool F16>
 __device__ __forceinline__ void mma_k16(float (&d)[BN / 2], uint64_t a, uint64_t b) {
-  static_assert(BN == 64, "64-column tiles (see pm_tapgemm_tc)");
-  wgmma_m64n64k16<!F16>(d, a, b);
+  static_assert(BN == 64 || BN == 128, "64- or 128-column tiles (see pm_tapgemm_tc)");
+  if constexpr (BN == 64) wgmma_m64n64k16<!F16>(d, a, b);
+  else wgmma_m64n128k16<!F16>(d, a, b);
 }
 
 // Three fp32 accumulators: two "main" ones that take the p0*p0 products of alternate k-iterations and one
@@ -116,13 +127,13 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tapgemm_tc_kernel(const __grid
   uint64_t* empty_bar = bars + MAX_STAGES;         // [MAX_STAGES]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (warp == 0) PM_STAMP(0);                                   // kernel entry
+  if (warp == STAMP_WARP) PM_STAMP(0);                          // kernel entry
   const int l0 = blockIdx.x * p.R;
   const int n0 = blockIdx.y * BN;
   const int b0 = blockIdx.z * p.NB;
   const int n_iter = p.taps * p.kblocks;
 
-  if (threadIdx.x == CONSUMER_THREADS) {
+  if (threadIdx.x == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_w) : "memory");
     for (int s = 0; s < p.stages; ++s) {
@@ -132,11 +143,12 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tapgemm_tc_kernel(const __grid
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
-  if (warp == 0) PM_STAMP(1);                                   // prologue done (barriers, descriptors)
+  if (warp == STAMP_WARP) PM_STAMP(1);                          // prologue done (barriers, descriptors)
 
-  if (warp == CONSUMER_THREADS / 32) {
-    // ===== TMA producer =====
-    if (lane == 1 && p.prefetch) {
+  if (warp < PRODUCER_THREADS / 32) {
+    // ===== producer warpgroup =====
+    setmaxnreg_dec<PRODUCER_REGS>();
+    if (warp == 1 && lane == 0 && p.prefetch) {
       // Weights are read once per window and the per-window set (0.6-0.8 GB) does not fit the 50 MB L2, so every
       // GEMM would stream its W tiles from HBM at DRAM latency.  Each CTA instead prefetches its share of the NEXT
       // GEMM's weights into L2 (cp.async.bulk.prefetch.L2) while this one computes.
@@ -151,7 +163,8 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tapgemm_tc_kernel(const __grid
         asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(p.prefetch + off), "r"(n) : "memory");
       }
     }
-    __syncwarp();
+    if (warp != 0) return;
+    // ----- warp 0: TMA -----
     const uint32_t tx = (uint32_t)stage_bytes;
     int s = 0, tap = 0, kb = 0;
     uint32_t ph = 0;
@@ -170,11 +183,13 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tapgemm_tc_kernel(const __grid
       if (++s == p.stages) { s = 0; ph ^= 1u; }
       if (++kb == p.kblocks) { kb = 0; ++tap; }
     }
-    return;                                        // the consumers' named barriers below do not count this warp
+    return;                                        // the consumers' named barriers below do not count this warpgroup
   }
 
   // ===== consumer warpgroups =====
-  const int wg = threadIdx.x >> 7;                  // 0 / 1: tile rows 64 wg .. 64 wg + 63
+  setmaxnreg_inc<CONSUMER_REGS>();
+  const int ct = threadIdx.x - PRODUCER_THREADS;    // consumer thread 0 .. 255
+  const int wg = ct >> 7;                           // 0 / 1: tile rows 64 wg .. 64 wg + 63
   float acc0[NACC], acc1[NACC], accc[NACC];
 #pragma unroll
   for (int i = 0; i < NACC; ++i) { acc0[i] = 0.f; acc1[i] = 0.f; accc[i] = 0.f; }
@@ -187,7 +202,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tapgemm_tc_kernel(const __grid
     // names its accumulator statically)
     auto kblock = [&](float (&main)[NACC]) {
       mbar_wait_fast(smem_u32(&full_bar[s]), ph);
-      if (prev < 0 && warp == 0) PM_STAMP(2);                     // first operand stage landed
+      if (prev < 0 && warp == STAMP_WARP) PM_STAMP(2);            // first operand stage landed
       const uint32_t a_base = tiles_u32 + (uint32_t)s * (uint32_t)stage_bytes + (uint32_t)wg * (64 * 128);
       const uint32_t w_base = tiles_u32 + (uint32_t)s * (uint32_t)stage_bytes + (uint32_t)(NSPLIT * A_TILE_BYTES);
       wgmma_fence();
@@ -195,7 +210,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tapgemm_tc_kernel(const __grid
       wgmma_commit();
       // at most one k-block in flight: the previous one has finished reading its stage, hand it back to the producer
       wgmma_wait<1>();
-      if (prev >= 0 && threadIdx.x % 128 == 0) mbar_arrive(smem_u32(&empty_bar[prev]));
+      if (prev >= 0 && ct % 128 == 0) mbar_arrive(smem_u32(&empty_bar[prev]));
       prev = s;
       if (++s == p.stages) { s = 0; ph ^= 1u; }
     };
@@ -205,9 +220,9 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tapgemm_tc_kernel(const __grid
       kblock(acc1);
     }
     if (it < n_iter) kblock(acc0);
-    if (warp == 0) PM_STAMP(3);                                 // all MMAs issued
+    if (warp == STAMP_WARP) PM_STAMP(3);                       // all MMAs issued
     wgmma_wait<0>();
-    if (warp == 0) PM_STAMP(4);                                 // accumulators complete
+    if (warp == STAMP_WARP) PM_STAMP(4);                       // accumulators complete
     wgmma_fence_regs(acc0);
     wgmma_fence_regs(acc1);
     wgmma_fence_regs(accc);
@@ -215,7 +230,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tapgemm_tc_kernel(const __grid
   // every MMA of both warpgroups has read its operands: the ring becomes the epilogue's staging tile
   named_bar_sync(1, CONSUMER_THREADS);
   {
-    const int wq = (threadIdx.x >> 5) & 3, t4 = lane & 3;
+    const int wq = warp & 3, t4 = lane & 3;
     const int r0 = wg * 64 + wq * 16 + (lane >> 2);
     float* stg = reinterpret_cast<float*>(tiles);
 #pragma unroll
@@ -245,7 +260,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tapgemm_tc_kernel(const __grid
   constexpr int C4 = BN / 4;                                     // float4 columns per row
   const float* stg = reinterpret_cast<const float*>(tiles);
 #pragma unroll 1
-  for (int item = threadIdx.x; item < BM * C4; item += CONSUMER_THREADS) {
+  for (int item = ct; item < BM * C4; item += CONSUMER_THREADS) {
     const int rt = item / C4, c = (item % C4) * 4;
     const int b = b0 + (rt >> r_shift), l = l0 + (rt & (p.R - 1));
     const int n = n0 + c;
@@ -286,11 +301,11 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tapgemm_tc_kernel(const __grid
       }
     }
   }
-  if (warp == 0) PM_STAMP(5);                                   // this warp's share of the epilogue issued
+  if (warp == STAMP_WARP) PM_STAMP(5);                         // this warp's share of the epilogue issued
 #ifdef PM_TC_TIMING
   named_bar_sync(1, CONSUMER_THREADS);
 #endif
-  if (warp == 0) PM_STAMP(6);                                   // all consumer warps done
+  if (warp == STAMP_WARP) PM_STAMP(6);                         // all consumer warps done
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -342,6 +357,36 @@ int launch(const CUtensorMap& ma, const CUtensorMap& mw, TcParams& p, dim3 grid,
   PM_LAUNCH_CHECK();
 }
 
+template <int BN>
+int launch_fmt(const CUtensorMap& ma, const CUtensorMap& mw, TcParams& p, dim3 grid, cudaStream_t st, bool f16) {
+  if (f16) {
+    if (p.nsplit == 1) return launch<BN, true, 1>(ma, mw, p, grid, st);
+    if (p.nsplit == 2) return launch<BN, true, 2>(ma, mw, p, grid, st);
+    return launch<BN, true, 3>(ma, mw, p, grid, st);
+  }
+  if (p.nsplit == 1) return launch<BN, false, 1>(ma, mw, p, grid, st);
+  if (p.nsplit == 2) return launch<BN, false, 2>(ma, mw, p, grid, st);
+  return launch<BN, false, 3>(ma, mw, p, grid, st);
+}
+
+// N tile of a launch: a pure function of the shape and the SM count, so a captured graph keeps its choice.
+// One CTA per SM, so a launch runs in waves of `sms` tiles.  A 128-column tile halves the shared-memory operand reads
+// per MAC and the per-tile fixed cost (barrier setup, pipeline fill, epilogue) per FLOP; it is chosen when the
+// 64-column grid needs at least 1.4x as many waves.  So it is not chosen where both grids fit one wave (the 32-clip
+// k = 3 convs of the motion encoder and the seed decode: 64 vs 32 CTAs, 10.5 vs 18.3 us at 128) and is everywhere
+// else on the EMAGE step.  Alone, a 128-column tile costs about 1.7 64-column ones; in the step, the forked face /
+// body / part branches fill partly used waves, and 1.4 measured best.  bench.py on one H100 80GB HBM3 at a 700 W
+// power limit, fp16x3: ratio 1.0 (always 128) 299-300 k frames/s, 1.4 306 k, 1.7 293-294 k, 2.0 292 k, 64 only 283 k.
+// tools/bench_gemm.py (fp16x3, fp32 out, us at BN = 64 / 128): 2048 x 768 <- 768 23.0 / 18.7; 2048 x 2304 <- 768
+// 58.1 / 56.3; 2048 x 1536 <- 768 37.0 / 37.3; 2048 x 768 <- 1536 36.8 / 29.0; 8192 x 1536 <- 768 148.9 / 122.6;
+// 32 x 300 conv k3 256 -> 256 36.5 / 36.1; 128 x 205 conv k15 128 -> 128 95.4 / 69.7.
+int pick_bn(long long row_tiles, int cout, int w_rows, int sms) {
+  if (cout <= 64 || w_rows % 128) return 64;
+  const long long waves64 = (row_tiles * pm_cdiv(cout, 64) + sms - 1) / sms;
+  const long long waves128 = (row_tiles * pm_cdiv(cout, 128) + sms - 1) / sms;
+  return waves128 * 14 <= waves64 * 10 ? 128 : 64;
+}
+
 }  // namespace
 
 extern "C" int pm_tapgemm_tc(const uint16_t* A, long long a_ps, long long a_bs, int lda, int batch, int rows_in, int cin,
@@ -353,6 +398,7 @@ extern "C" int pm_tapgemm_tc(const uint16_t* A, long long a_ps, long long a_bs, 
                              uint16_t* out_bf16, long long ob_ps, long long ob_bs, int ldob, int out_nsplit,
                              const void* prefetch, long long prefetch_bytes, void* stream) {
   PM_REQUIRE(A && W && (out_f32 || out_bf16));
+  const int tile = (nsplit >> PM_TC_TILE_SHIFT) & 0xff;   // N tile override: 0 automatic, 1 = 64, 2 = 128 columns
   PM_TAKE_FMT(nsplit, f16);                 // operand planes: bf16 (default) or fp16
   PM_TAKE_FMT(out_nsplit, out_f16);
   PM_REQUIRE(!out_bf16 || out_f16 == f16);  // emitted planes use the operand format
@@ -373,10 +419,15 @@ extern "C" int pm_tapgemm_tc(const uint16_t* A, long long a_ps, long long a_bs, 
   int R = 128;
   if (rows_out <= 64 && batch > 1) { R = 16; while (R < rows_out) R <<= 1; }
   const int NB = 128 / R;
-  // N tile: 64 columns.  Three m64n128 accumulators per thread (192 registers) do not fit the 168 registers a thread
-  // of a 288- or 384-thread CTA gets on sm_90 (ptxas spills them); three m64n64 ones take 96.
-  constexpr int BNsel = 64;
-  PM_REQUIRE(w_rows % BNsel == 0);
+  PM_REQUIRE(tile <= 2 && w_rows % 64 == 0 && (tile != 2 || w_rows % 128 == 0));
+  int BNsel = tile == 1 ? 64 : 128;
+  if (tile == 0) {
+    int dev = 0, sms = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e == cudaSuccess) e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    if (e != cudaSuccess) return (int)e;
+    BNsel = pick_bn((long long)pm_cdiv(rows_out, R) * pm_cdiv(batch, NB), cout, w_rows, sms);
+  }
 
   TcParams p;
   p.taps = taps; p.pad = pad; p.nsplit = nsplit; p.kblocks = (cin + BK - 1) / BK;
@@ -409,14 +460,8 @@ extern "C" int pm_tapgemm_tc(const uint16_t* A, long long a_ps, long long a_bs, 
   dim3 grid(pm_cdiv(rows_out, R), pm_cdiv(cout, BNsel), pm_cdiv(batch, NB));
   PM_REQUIRE(grid.z <= 65535 && grid.y <= 65535);
   const cudaStream_t st = (cudaStream_t)stream;
-  if (f16) {
-    if (nsplit == 1) return launch<BNsel, true, 1>(ma, mw, p, grid, st);
-    if (nsplit == 2) return launch<BNsel, true, 2>(ma, mw, p, grid, st);
-    return launch<BNsel, true, 3>(ma, mw, p, grid, st);
-  }
-  if (nsplit == 1) return launch<BNsel, false, 1>(ma, mw, p, grid, st);
-  if (nsplit == 2) return launch<BNsel, false, 2>(ma, mw, p, grid, st);
-  return launch<BNsel, false, 3>(ma, mw, p, grid, st);
+  if (BNsel == 128) return launch_fmt<128>(ma, mw, p, grid, st, f16);
+  return launch_fmt<64>(ma, mw, p, grid, st, f16);
 }
 
 #ifdef PM_TC_TIMING

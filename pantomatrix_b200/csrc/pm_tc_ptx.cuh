@@ -15,6 +15,9 @@ __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
 __device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
 }
+// The watchdog's trap, out of line: a trap inlined into code after setmaxnreg.inc makes ptxas allocate that code at the
+// launch's register limit instead of the raised one (the tap-GEMM consumers then spill their accumulators).
+static __device__ __noinline__ void pm_watchdog_trap() { __trap(); }
 // Bounded wait: a protocol bug must become a trap (an error the host sees), never a hung GPU.  The spin body is kept to
 // the probe itself (try_wait suspends the thread for a hardware-defined slice): the watchdog clock is read only every
 // 4096 probes.
@@ -32,7 +35,7 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     if ((++spins & 0xFFFu) == 0) {
       const long long t = clock64();
       if (t0 == 0) t0 = t;
-      else if (t - t0 > 4000000000LL) __trap();
+      else if (t - t0 > 4000000000LL) pm_watchdog_trap();
     }
   }
 }
@@ -100,6 +103,12 @@ __device__ __forceinline__ float4 ldg_stream4(const float4* p) {
                : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(p));
   return v;
 }
+// Warp-specialised register split (sm_90a): a whole warpgroup gives registers back to the CTA's pool or takes them
+// from it.  Every warp of the warpgroup executes the same instruction; N is a multiple of 8 in [24, 256].
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 // named barrier over a subset of the CTA's warps (id 0 is __syncthreads)
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t threads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
@@ -140,7 +149,18 @@ __device__ __forceinline__ void wgmma_m64n64k16(float (&d)[32], uint64_t da, uin
   else PM_WGMMA_N64("f16");
 }
 #undef PM_WGMMA_N64
-#define PM_WGMMA_N192(TY)                                                                                   \
+#define PM_WGMMA_N128(TY)                                                                                   \
+  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"                                           \
+               "wgmma.mma_async.sync.aligned.m64n128k16.f32." TY "." TY " {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, %67;\n\t}" \
+               : PM_D8(0), PM_D8(8), PM_D8(16), PM_D8(24), PM_D8(32), PM_D8(40), PM_D8(48), PM_D8(56) \
+               : "l"(da), "l"(db), "r"(1), "n"(TRANS_B))
+template <bool BF16, int TRANS_B = 0>
+__device__ __forceinline__ void wgmma_m64n128k16(float (&d)[64], uint64_t da, uint64_t db) {
+  if constexpr (BF16) PM_WGMMA_N128("bf16");
+  else PM_WGMMA_N128("f16");
+}
+#undef PM_WGMMA_N128
+#define PM_WGMMA_N192(TY)                                                                                 \
   asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %98, 0;\n\t"                                           \
                "wgmma.mma_async.sync.aligned.m64n192k16.f32." TY "." TY " {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95}, %96, %97, p, 1, 1, 0, %99;\n\t}" \
                : PM_D8(0), PM_D8(8), PM_D8(16), PM_D8(24), PM_D8(32), PM_D8(40), PM_D8(48), PM_D8(56), PM_D8(64), PM_D8(72), PM_D8(80), PM_D8(88) \

@@ -3,8 +3,9 @@
     python -m pantomatrix_b200.build --variant timing -DPM_TC_TIMING
     PM_EMAGE_LIB=pantomatrix_b200/csrc/_build/variants/libpm_emage_timing.so python tools/gemm_timeline.py
 
-Stamps (cycles of the CTA's SM clock, relative to kernel entry of that CTA): prologue done, first operand stage
-landed, all MMAs issued, accumulators complete, epilogue of warp 2 issued, all warps done.  The launch-to-launch
+Stamps, one set per CTA (= per output tile), written by the first consumer warp (cycles of the CTA's SM clock, relative
+to kernel entry of that CTA): prologue done, first operand stage landed, all MMAs issued, accumulators complete, this
+warp's epilogue issued, all consumer warps done.  The launch uses the automatically chosen N tile.  The launch-to-launch
 period (CUDA events around a replayed graph of 20 launches) minus the in-kernel span is launch / drain / tail cost."""
 import ctypes
 import math
