@@ -18,6 +18,8 @@ Schedule differences from the reference that do not change results beyond fp32 r
 """
 from __future__ import annotations
 
+import os
+
 import torch
 
 from .. import ops
@@ -51,35 +53,45 @@ def wav_out_len(n: int) -> int:
 # 1 / 2 / 3 operand planes (csrc/pm_tapgemm_tc.cu).
 #   fp16x3 (default)  two IEEE fp16 planes (22 mantissa bits), 3 tensor-core products per fp32 product: the parity
 #                     gates of tests/test_emage_gpu.py hold as for bf16x6, at half the MMA work.  Operands must stay
-#                     below 65504 / 64 (activations are pre-scaled by 64, ops.F16_ACT_SCALE): pipeline.py checks the
-#                     outputs for the NaN an overflow would leave and names bf16x6 as the way out.
+#                     below 65504 / 64 (activations are pre-scaled by 64, ops.F16_ACT_SCALE): overflow_flag() catches
+#                     the NaN an overflow would leave in the outputs, and bf16x6 is the way out.
 #   bf16x6            three bf16 planes, 6 products: same accuracy, no range limit (fp32 exponent range), slower.
 #   bf16x3 / bf16     faster, below the parity gates.
 #   fp32              exact-order fp32 SIMT engine (reference engine of the tests).
-PRECISIONS = {"fp32": 0, "bf16": 1, "bf16x3": 2, "bf16x6": 3, "fp16x3": 2}
-PLANE_FORMAT = {"fp16x3": "fp16"}
-DEFAULT_PRECISION = __import__("os").environ.get("PM_EMAGE_PRECISION", "fp16x3")     # PM_EMAGE_PRECISION overrides
-_STATE = {"nsplit": PRECISIONS[DEFAULT_PRECISION], "fork": True,   # fork: overlap independent branches on side streams
-          "precision": DEFAULT_PRECISION,
-          # clip-group lanes of the window loop (run_inference).  Measured at batch 32: 1 lane 19.91 ms, 2 lanes 19.59,
-          # 4 lanes 19.49 per step - a 2 % gain for 2-4x the kernel launches, so one lane is the default.
-          "groups": int(__import__("os").environ.get("PM_EMAGE_GROUPS", "1"))}
-ops.set_plane_format(PLANE_FORMAT.get(DEFAULT_PRECISION, "bf16"))
+# name -> (split count, plane format).  The engine stores only the split count (_STATE["nsplit"]); the plane format
+# lives in ops (ops.plane_format()), where the kernels and PackedW read it.
+PRECISIONS = {"fp32": (0, "bf16"), "bf16": (1, "bf16"), "bf16x3": (2, "bf16"), "bf16x6": (3, "bf16"), "fp16x3": (2, "fp16")}
+_MODE_OF = {v: k for k, v in PRECISIONS.items()}
+DEFAULT_PRECISION = os.environ.get("PM_EMAGE_PRECISION", "fp16x3")     # PM_EMAGE_PRECISION overrides
+_STATE = {"nsplit": 0, "fork": True}    # fork: overlap independent branches on side streams
 
 
 def set_precision(name: str) -> None:
     if name not in PRECISIONS:
         raise ValueError(f"precision must be one of {sorted(PRECISIONS)}")
-    _STATE["nsplit"] = PRECISIONS[name]
-    _STATE["precision"] = name
-    ops.set_plane_format(PLANE_FORMAT.get(name, "bf16"))
+    _STATE["nsplit"], fmt = PRECISIONS[name]
+    ops.set_plane_format(fmt)
+
+
+set_precision(DEFAULT_PRECISION)
 
 
 def get_precision() -> str:
-    name = _STATE.get("precision")
-    if name in PRECISIONS and PRECISIONS[name] == _STATE["nsplit"]:
-        return name
-    return next(k for k, v in PRECISIONS.items() if v == _STATE["nsplit"])     # _STATE["nsplit"] was set directly (tests)
+    """The mode that runs, derived from the split count and the plane format."""
+    if _STATE["nsplit"] == 0:          # the fp32 engine builds no operand planes: the plane format does not matter
+        return "fp32"
+    key = (_STATE["nsplit"], ops.plane_format())
+    if key not in _MODE_OF:
+        raise RuntimeError(f"no precision mode runs {key[0]} {key[1]} operand planes (ops.set_plane_format() was called "
+                           f"directly): select one of {sorted(PRECISIONS)} with set_precision()")
+    return _MODE_OF[key]
+
+
+def overflow_flag(device):
+    """A cleared int32[1] device flag (ops.zero_flag: a memset node under graph capture) when the running mode uses
+    fp16 operand planes with a split (fp16x3), else None.  An operand past the fp16 range becomes inf - inf = NaN in
+    the consuming GEMM and propagates to every output, so a row_argmax(..., nonfinite=flag) over an output reveals it."""
+    return ops.zero_flag(device) if get_precision() == "fp16x3" else None
 
 
 def _pk(nsplit: int) -> int:
@@ -90,16 +102,15 @@ def _pk(nsplit: int) -> int:
 def guarded(run, checked):
     """Run `run()` in the current precision; in the fp16x3 engine verify afterwards that no GEMM operand left the
     fp16 range and, if one did, recompute in bf16x6 (same accuracy, fp32 exponent range) - still on the GPU, with a
-    warning.  `checked(result)` returns the fp32 tensors whose NaN would reveal the overflow (an out-of-range operand
-    becomes inf - inf = NaN in the consuming GEMM and propagates to every output).  Inside a CUDA-graph capture nothing
-    can be read back: the captured pipeline carries the flag itself (pipeline.CapturedPipeline)."""
+    warning.  `checked(result)` returns the fp32 tensors whose NaN would reveal the overflow (overflow_flag).  Inside a
+    CUDA-graph capture nothing can be read back: the captured pipelines carry the flag themselves (pipeline.py)."""
     out = run()
-    if ops.plane_format() != "fp16":
-        return out
     tensors = [t for t in checked(out) if t is not None]
     if not tensors or not tensors[0].is_cuda or torch.cuda.is_current_stream_capturing():
         return out
-    flag = ops.zero_flag(tensors[0].device)
+    flag = overflow_flag(tensors[0].device)
+    if flag is None:
+        return out
     for t in tensors:
         ops.row_argmax(t, nonfinite=flag)                # the kernel that reads the logits anyway; indices discarded
     if not bool(flag):
@@ -107,12 +118,11 @@ def guarded(run, checked):
     import warnings
     warnings.warn("fp16x3: a GEMM operand exceeded the fp16 range (|x| > 1023 after the x64 pre-scale); "
                   "recomputing this call with engine.set_precision('bf16x6') - select it up front for this checkpoint")
-    prev = get_precision()
     set_precision("bf16x6")
     try:
         return run()
     finally:
-        set_precision(prev)
+        set_precision("fp16x3")
 
 
 def _record_stream(obj, stream):
@@ -388,7 +398,7 @@ class _Layer:
             att = ops.attention_tc(qkv, 0, qkv, E, qkv, 2 * E, bs, NHEAD, t, t, hd, nsplit=ns)
         else:
             qkv = self.sa.qkv(x).view(bs * t, 3 * E)
-            att = ops.attention(qkv[:, :E], qkv[:, E:2 * E], qkv[:, 2 * E:], bs, NHEAD, t, t, hd, nsplit=ns, f32=ns == 0)
+            att = ops.attention(qkv[:, :E], qkv[:, E:2 * E], qkv[:, 2 * E:], bs, NHEAD, t, t, hd, nsplit=ns, f32=False)
         x = ops.add_layernorm(self.sa.out(_view3(att, bs, t, E), residual=xf), None, *self.norms[0], nsplit=ns)
         k = 1
         if self.ca is not None:
@@ -400,7 +410,7 @@ class _Layer:
                 assert mem_kv.is_contiguous()
                 kv = mem_kv.view(bs * tk, 2 * E)
                 q = self.ca.q(x).view(bs * t, E)
-                att = ops.attention(q, kv[:, :E], kv[:, E:], bs, NHEAD, t, tk, hd, nsplit=ns, f32=ns == 0)
+                att = ops.attention(q, kv[:, :E], kv[:, E:], bs, NHEAD, t, tk, hd, nsplit=ns, f32=False)
             x = ops.add_layernorm(self.ca.out(_view3(att, bs, t, E), residual=_f32(x)), None, *self.norms[1], nsplit=ns)
             k = 2
         h = self.l1(x, act=ops.ACT_RELU, want="p")
@@ -411,7 +421,7 @@ class _Layer:
 
 def _attn_tc():
     """The tensor-core attention kernel consumes two-plane fp16 operands: the fp16x3 engine."""
-    return _STATE["nsplit"] == 2 and ops.plane_format() == "fp16"
+    return get_precision() == "fp16x3"
 
 
 def _window_of(x, j, bs):
@@ -460,7 +470,7 @@ class EmageEngine:
         self.cls = {p: _MLP(sd, "motion_cls_" + p) for p in PARTS[1:]}
         self.cls["face"] = _MLP(sd, "face_cls")
         self._fork_audio = _Fork(1)
-        self._lane_forks = {}          # clip-group lane -> (face || body fork, refine-parts fork): side streams are per lane
+        self._fork_branch, self._fork_parts = _Fork(1), _Fork(2)           # face || body, the three refine decoders
 
     # ------------------------------------------------------------------------------------------------
     def audio_phase(self, audio, offset, a_ws, windows, n_samples, t):
@@ -475,35 +485,29 @@ class EmageEngine:
             return self.face_mem_audio(a_face[:, :t])      # M.py:278-281 (the body stream is never truncated)
 
         def body():
-            mem_body = self.body_mem(self.wav_body(audio, offset, a_ws, windows, n_samples), want="p" if _ns() else "f")
+            mem_body = self.body_mem(self.wav_body(audio, offset, a_ws, windows, n_samples), want="p")
             return [layer.project_memory(mem_body) for layer in self.cross]
 
         kv, mem_face = self._fork_audio.run([body, face])
         return mem_face, kv
 
-    def _forks(self, lane):
-        if lane not in self._lane_forks:
-            self._lane_forks[lane] = (_Fork(1), _Fork(2))
-        return self._lane_forks[lane]
-
-    def window(self, win_in, speaker_id_rows, mem_face_audio, kv_body, dest=None, use_audio=True, lane=0):
+    def window(self, win_in, speaker_id_rows, mem_face_audio, kv_body, dest=None, use_audio=True):
         """One window of EmageAudioModel.forward (M.py:265-341) given the hoisted audio tensors.
         win_in (bs,t,337) is already mask-embedded.  speaker_id_rows = (spk_face_rows, spk_body_rows).
         dest: optional dict name -> (bs, t, 256) fp32 view the final GEMM of that output writes into (the window's rows
         of inference()'s accumulated outputs), so nothing is copied afterwards."""
         dest = dest or {}
-        fork_branch, fork_parts = self._forks(lane)
         # use_audio=False (training-time ablation, M.py:310-311): the body's audio cross-attention output is multiplied
         # by zero, i.e. motion_fea + 0 - the 8 cross layers are simply not run; the face branch still sees the audio.
         bs, t = (win_in.p.batch, win_in.p.rows) if isinstance(win_in, ops.Act) and win_in.f is None else _f32(win_in).shape[:2]
         E = self.E
         spk_f, spk_b = speaker_id_rows
         ns = _ns()
-        hint = self.motion_encoder(win_in, want="p" if ns else "f")                    # M.py:271
+        hint = self.motion_encoder(win_in, want="p")                    # M.py:271
 
         def face_branch():                                                              # M.py:288-294
-            hint_face = self.hint_face(hint, want="p" if ns else "f")
-            mem_f = self.face_mem_hint(hint_face, residual=mem_face_audio, want="p" if ns else "f")
+            hint_face = self.hint_face(hint, want="p")
+            mem_f = self.face_mem_hint(hint_face, residual=mem_face_audio, want="p")
             x = ops.add_rows(None, self.pe, spk_f, ops.ROW_SPK, ops.ROW_PE, bs, t, E, nsplit=ns)
             for i, layer in enumerate(self.face_dec):
                 x = layer(x, layer.project_memory(mem_f), want="fp" if i + 1 < len(self.face_dec) else "p")
@@ -511,7 +515,7 @@ class EmageEngine:
             return {"rec_face": _f32(rec), "cls_face": self.cls["face"](rec, out=dest.get("cls_face"))}
 
         def body_branch():                                                              # M.py:297-330
-            hint_body = self.hint_body(hint, want="p" if ns else "f")
+            hint_body = self.hint_body(hint, want="p")
             x = ops.add_rows(self.moton_proj(hint_body), self.pe, spk_b, ops.ROW_PE, ops.ROW_SPK, bs, t, E, nsplit=ns)
             fea = self.self_enc(x)
             fea = ops.add_rows(fea, self.pe, spk_b, ops.ROW_SPK, ops.ROW_PE, bs, t, E, nsplit=ns)
@@ -519,9 +523,9 @@ class EmageEngine:
             if use_audio:
                 for i, (layer, kv) in enumerate(zip(self.cross, kv_body)):
                     x = layer(x, kv, want="fp" if i + 1 < len(self.cross) else "f")
-                fea = ops.add2(_f32(fea), _f32(x), nsplit=ns, f32=ns == 0)
+                fea = ops.add2(_f32(fea), _f32(x), nsplit=ns, f32=False)
             else:
-                fea = ops.add2(_f32(fea), torch.zeros_like(_f32(fea)), nsplit=ns, f32=ns == 0)
+                fea = ops.add2(_f32(fea), torch.zeros_like(_f32(fea)), nsplit=ns, f32=False)
             lat = {p: self.to_latent[p](fea) for p in PARTS[1:]}
             others = {"upper": ("hands", "lower"), "hands": ("upper", "lower"), "lower": ("upper", "hands")}
 
@@ -529,17 +533,17 @@ class EmageEngine:
                 a, b = others[p]
                 layer = self.refine[p]
                 tgt = ops.add_rows(lat[p], self.pe, spk_b, ops.ROW_SPK, ops.ROW_NONE, bs, t, E, nsplit=ns)
-                mem = ops.add2(lat[a], lat[b], nsplit=ns, f32=ns == 0)
+                mem = ops.add2(lat[a], lat[b], nsplit=ns, f32=False)
                 r = layer(tgt, layer.project_memory(mem))
-                rec = self.out_proj[p](ops.add2(lat[p], r, nsplit=ns, f32=ns == 0), want="fp", out=dest.get("rec_" + p))
+                rec = self.out_proj[p](ops.add2(lat[p], r, nsplit=ns, f32=False), want="fp", out=dest.get("rec_" + p))
                 return {"rec_" + p: _f32(rec), "cls_" + p: self.cls[p](rec, out=dest.get("cls_" + p))}
 
             out = {}
-            for d in fork_parts.run([lambda p=p: refine(p) for p in PARTS[1:]]):
+            for d in self._fork_parts.run([lambda p=p: refine(p) for p in PARTS[1:]]):
                 out.update(d)
             return out
 
-        body, face = fork_branch.run([body_branch, face_branch])
+        body, face = self._fork_branch.run([body_branch, face_branch])
         body.update(face)
         return body
 
@@ -570,7 +574,7 @@ class VQEngine:
             self.global_enc = _ConvStack(sds["global"], "encoder", "encoder", n)
             self.global_dec = _ConvStack(sds["global"], "decoder", "decoder", n)
         self.device = self.codebook["face"].device
-        self._forks = {}               # clip-group lane -> fork of the four part decoders
+        self._fork = _Fork(3)          # the four part decoders
 
     def part_decode(self, p, index=None, latent=None):
         """EmageVQVAEConv.decode / decode_from_latent (M.py:56-70) -> (pose features, indices)."""
@@ -578,14 +582,12 @@ class VQEngine:
             index = ops.l2_argmin(latent, self.codebook[p], self.e2[p])
         return self.decoder[p](ops.gather_rows(self.codebook[p], index.contiguous(), nsplit=_ns())), index
 
-    def decode(self, index, latent, get_global_motion=False, ref_trans=None, lane=0):
+    def decode(self, index, latent, get_global_motion=False, ref_trans=None):
         """index/latent: dicts part -> tensor or None.  Returns the reference's 4-key dict (M.py:193)."""
         shape = next(t.shape[:2] for t in list(index.values()) + list(latent.values()) if t is not None)
         bs, t = int(shape[0]), int(shape[1])
         todo = [p for p in PARTS if index.get(p) is not None or latent.get(p) is not None]
-        if lane not in self._forks:
-            self._forks[lane] = _Fork(3)
-        done = self._forks[lane].run([lambda p=p: self.part_decode(p, index.get(p), latent.get(p))[0] for p in todo])
+        done = self._fork.run([lambda p=p: self.part_decode(p, index.get(p), latent.get(p))[0] for p in todo])
         feats = dict(zip(todo, done))
         expression, aa, m4 = ops.pose_compose(feats.get("face"), feats.get("upper"), feats.get("hands"),
                                               feats.get("lower"), bs, t, self.device)
@@ -690,50 +692,23 @@ def run_inference(engine: EmageEngine, vq: VQEngine, audio, speaker_id, masked_m
     # spill past the end: `pad` spare rows take that, and the result is the dense [:out_len] prefix (a copy only then).
     pad = max(0, max(off_t for off_t in [sum(k for _, _, k in plan[:i]) + (e - s) for i, (s, e, _) in enumerate(plan)]) - out_len)
     acc = {k + p: torch.empty(bs, out_len + pad, 256, device=dev) for k in ("rec_", "cls_") for p in PARTS}
-    # Clips are independent, and one window is a chain of ~150 dependent kernels whose GEMMs fill 48-288 of the 132 SMs:
-    # the clip batch is therefore split into `groups` lanes that run their window loops on separate streams, so that
-    # one lane's launch gaps, drains and epilogue tails are filled by the other lane's thread blocks (the hoisted audio
-    # phase above and the final decode stay batched).  Per-clip results do not depend on the grouping.
-    n_groups = max(1, min(int(_STATE.get("groups", 1)), bs // 8)) if torch.cuda.is_available() else 1
-    bounds = [bs * g // n_groups for g in range(n_groups + 1)]
-
-    def sl(x, g0, g1):                # clips g0..g1 of a (clips, ...) tensor, plane Act or None
-        if x is None:
-            return None
-        if isinstance(x, ops.Act):
-            pl = x.p
-            return ops.Act(None if x.f is None else x.f[g0:g1], None if pl is None else ops.Planes(pl.t[:, g0:g1], pl.rows, pl.ch, 0))
-        return x[g0:g1]
-
-    def run_lane(lane):
-        g0, g1 = bounds[lane], bounds[lane + 1]
-        nb = g1 - g0
-        spk_l = (spk[0][g0:g1], spk[1][g0:g1])
-        seed = None                   # first window: the seed is motion[:, :pre] itself (M.py:379) - window_input keeps it
-        off = 0
-        for wi, (s, e, keep) in enumerate(plan):
-            t = e - s
-            win_in = ops.window_input(sl(motion, g0, g1), sl(full_mask, g0, g1), seed, engine.mask_embedding, s, t, pre,
-                                      nsplit=_ns(), f32=_ns() == 0, shape=(nb, length, ch))
-            mem_face, kv = hoisted[wi]
-            out = engine.window(win_in, spk_l, sl(mem_face, g0, g1), [sl(k, g0, g1) for k in kv],
-                                dest={k: v[g0:g1, off:off + t] for k, v in acc.items()}, lane=lane)
-            off += keep
-            if wi + 1 < len(plan):                                                       # seed for the next window
-                nd = min(t, seed_decode_frames(cfg, vq))
-                tail = {k: v[:, t - nd:] for k, v in out.items()}                        # strided views, read in place
-                idx = {p: ops.row_argmax(tail["cls_" + p]) for p in PARTS}               # M.py:398-401
-                index, latent = select_inputs(cfg, tail, idx)
-                dec = vq.decode(index, latent, lane=lane)
-                seed = dec["all_motion4inference"][:, nd - pre:]                         # M.py:418
-        return None
-
-    if n_groups == 1:
-        run_lane(0)
-    else:
-        if getattr(engine, "_fork_lanes", None) is None or engine._fork_lanes.n_side != n_groups - 1:
-            engine._fork_lanes = _Fork(n_groups - 1)
-        engine._fork_lanes.run([lambda lane=lane: run_lane(lane) for lane in range(n_groups)])
+    ns = _ns()
+    seed = None                       # first window: the seed is motion[:, :pre] itself (M.py:379) - window_input keeps it
+    off = 0
+    for wi, (s, e, keep) in enumerate(plan):
+        t = e - s
+        win_in = ops.window_input(motion, full_mask, seed, engine.mask_embedding, s, t, pre, nsplit=ns, f32=False,
+                                  shape=(bs, length, ch))
+        mem_face, kv = hoisted[wi]
+        out = engine.window(win_in, spk, mem_face, kv, dest={k: v[:, off:off + t] for k, v in acc.items()})
+        off += keep
+        if wi + 1 < len(plan):                                                           # seed for the next window
+            nd = min(t, seed_decode_frames(cfg, vq))
+            tail = {k: v[:, t - nd:] for k, v in out.items()}                            # strided views, read in place
+            idx = {p: ops.row_argmax(tail["cls_" + p]) for p in PARTS}                   # M.py:398-401
+            index, latent = select_inputs(cfg, tail, idx)
+            dec = vq.decode(index, latent)
+            seed = dec["all_motion4inference"][:, nd - pre:]                             # M.py:418
     if pad:
         acc = {k: v[:, :out_len].contiguous() for k, v in acc.items()}
     return acc

@@ -394,8 +394,7 @@ class EmageAudioModel(_EngineOwner):
         # no seed splice here: pre = 0 makes window_input the plain `where(mask==1, embedding, motion)`
 
         def run():
-            ns = E._ns()
-            win_in = ops.window_input(motion, mask, None, eng.mask_embedding, 0, t, 0, nsplit=ns, f32=ns == 0)
+            win_in = ops.window_input(motion, mask, None, eng.mask_embedding, 0, t, 0, nsplit=E._ns(), f32=False)
             mem_face, kv = eng.audio_phase(audio, 0, 0, 1, audio.shape[1], t)
             return eng.window(win_in, eng.speaker_rows(speaker_id.to(dev)), mem_face, kv, use_audio=use_audio)
         return E.guarded(run, lambda out: [out["cls_" + p] for p in E.PARTS])

@@ -224,7 +224,6 @@ class _LstmModelBase(_EngineOwner):
 
     def forward(self, audio, speaker_id, seed_frames=4, seed_motion=None, return_axis_angle=True):
         """audio (bs, n) 16 kHz, speaker_id (bs, 1) long, optional seed_motion (bs, t_m, pose_dims) rot6d."""
-        from ..emage_audio import engine as E
         eng = self._eng()
         return E.guarded(lambda: eng.forward(audio, eng.host_cond(speaker_id, seed_frames, seed_motion), return_axis_angle),
                          lambda out: [out["motion"]])

@@ -7,29 +7,34 @@ from __future__ import annotations
 import torch
 
 from . import _lib, ops
-from .emage_audio.engine import PARTS, select_inputs
+from .emage_audio.engine import PARTS, overflow_flag, select_inputs
 
 _OVERFLOW = ("fp16x3: a GEMM operand exceeded the fp16 range (|x| > 1023 after the x64 pre-scale) and the result is NaN - "
              "use engine.set_precision('bf16x6') for this checkpoint (model.inference() outside a captured graph retries "
              "in bf16x6 by itself)")
 
 
-@torch.no_grad()
 def generate(model, motion_vq, audio, speaker_id=None, masked_motion=None, mask=None, ref_trans=None):
     """audio (bs, n) float32 16 kHz.  Returns (latent_dict, pred_dict) like T.py:32 and T.py:44-47."""
+    return _generate(model, motion_vq, audio, speaker_id, masked_motion, mask, ref_trans)[:2]
+
+
+@torch.no_grad()
+def _generate(model, motion_vq, audio, speaker_id=None, masked_motion=None, mask=None, ref_trans=None):
+    """generate() -> (latent_dict, pred_dict, the fp16 overflow flag of engine.overflow_flag or None).  Outside a
+    graph capture an overflow raises PmError; inside one the caller reads the flag after each replay."""
     dev = next(model.parameters()).device
     bs = audio.shape[0]
     if speaker_id is None:
         speaker_id = torch.zeros(bs, 1, dtype=torch.long, device=dev)                  # T.py:19
     lat = model.inference(audio, speaker_id, motion_vq, masked_motion=masked_motion, mask=mask)
-    # fp16 operand planes turn an out-of-range activation into inf - inf = NaN in the consuming GEMM; a NaN anywhere
-    # upstream reaches the logits (cls_* = MLP(rec_*)), which the argmax kernels read anyway: they raise the flag.
-    generate.nonfinite = ops.zero_flag(dev) if ops.plane_format() == "fp16" else None
+    # a NaN anywhere upstream reaches the logits (cls_* = MLP(rec_*)), which the argmax kernels read anyway
+    nonfinite = overflow_flag(dev)
     cfg = model.cfg.to_dict()
-    idx = {p: ops.row_argmax(lat["cls_" + p], nonfinite=generate.nonfinite) for p in PARTS}       # T.py:39-42
-    if generate.nonfinite is not None:
+    idx = {p: ops.row_argmax(lat["cls_" + p], nonfinite=nonfinite) for p in PARTS}            # T.py:39-42
+    if nonfinite is not None:
         capturing = lat["rec_face"].is_cuda and torch.cuda.is_current_stream_capturing()
-        if not capturing and bool(generate.nonfinite):
+        if not capturing and bool(nonfinite):
             raise _lib.PmError(_OVERFLOW)
     index, latent = select_inputs(cfg, lat, idx)
     if ref_trans is None:
@@ -38,10 +43,7 @@ def generate(model, motion_vq, audio, speaker_id=None, masked_motion=None, mask=
         face_latent=latent["face"], upper_latent=latent["upper"], lower_latent=latent["lower"],
         hands_latent=latent["hands"], face_index=index["face"], upper_index=index["upper"],
         lower_index=index["lower"], hands_index=index["hands"], get_global_motion=True, ref_trans=ref_trans)
-    return lat, pred
-
-
-generate.nonfinite = None
+    return lat, pred, nonfinite
 
 
 def _audio_input(batch, n_samples, dev, input_rate, input_channels, input_dtype):
@@ -95,7 +97,7 @@ class CapturedPipeline:
         def step():
             if self.resampler is not None:
                 self.resampler(self.pcm, out=self.audio)
-            return generate(model, motion_vq, self.audio, self.speaker_id, ref_trans=self.ref_trans)
+            return _generate(model, motion_vq, self.audio, self.speaker_id, ref_trans=self.ref_trans)
 
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(torch.cuda.current_stream(dev))
@@ -112,9 +114,8 @@ class CapturedPipeline:
         # which the other branch's blocks share).
         self.capture_stream = torch.cuda.Stream(device=dev, priority=-1) if body_priority else None
         with torch.cuda.graph(self.graph, stream=self.capture_stream):
-            self.latent, self.pred = step()
+            self.latent, self.pred, self.nonfinite = step()   # nonfinite: the in-graph overflow flag (fp16x3 only)
         self.kernels_per_replay = ops.launch_count - before
-        self.nonfinite = generate.nonfinite                  # fp16 planes only: in-graph overflow flag (else None)
 
     @torch.no_grad()
     def __call__(self, audio, speaker_id=None):
@@ -163,7 +164,6 @@ class CapturedLstmPipeline:
         self.seed = torch.zeros(batch, seed_frames, self.pose_dims, device=dev)
         self.barrier = torch.zeros(4, dtype=torch.int32, device=dev)
         t = wav_frames(self.audio.shape[1])
-        guard = ops.plane_format() == "fp16"
 
         @torch.no_grad()
         def step():
@@ -173,9 +173,8 @@ class CapturedLstmPipeline:
             # forward(seed_motion=x) for any x of length t with these first rows (and forward(seed_motion=None) for zeros)
             out = eng.forward(self.audio, eng.kernel_cond(self.speaker_id, self.seed, t, seed_frames), True,
                               barrier=self.barrier)
-            flag = None
-            if guard:                      # an fp16 operand overflow leaves NaN in the motion: the argmax kernel flags it
-                flag = ops.zero_flag(dev)
+            flag = overflow_flag(dev)
+            if flag is not None:           # an fp16 operand overflow leaves NaN in the motion: the argmax kernel flags it
                 ops.row_argmax(out["motion"], nonfinite=flag)
             return out, flag
 

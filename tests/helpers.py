@@ -1,8 +1,10 @@
 """Shared test helpers: product-side model construction with the synthetic checkpoints, and the float64 references
 with per-element error bounds that the tensor-core kernel tests (tests/test_tapgemm_tc_gpu.py, tests/test_kernels_gpu.py,
 tests/test_kernel_shadow_gpu.py) check every output element against."""
+import functools
 import math
 
+import pytest
 import torch
 
 from synthetic_models import build_lstm_product, build_product  # noqa: F401  (construction lives at the repo root)
@@ -12,6 +14,24 @@ F16_MIN_NORMAL = 2.0 ** -14          # nonzero fp16 operands below this are subn
 UNIT = {torch.bfloat16: 2.0 ** -8, torch.float16: 2.0 ** -11}     # relative size of plane p + 1 to plane p
 ULP32 = 2.0 ** -24
 STEP = 2.0 ** -22                    # error of one wgmma instruction relative to its accumulator's magnitude bound
+
+
+@pytest.fixture(autouse=True)
+def bf16_planes_by_default():
+    """For the kernel test modules that import it: each test starts on bf16 operand planes (ops' default) unless it
+    selects fp16 itself, and leaves the plane format - half of the engine's precision mode - as it found it."""
+    from pantomatrix_b200 import ops
+    found = ops.plane_format()
+    ops.set_plane_format("bf16")
+    yield
+    ops.set_plane_format(found)
+
+
+def use_precision(request, name: str) -> None:
+    """engine.set_precision(name) for the requesting test; the mode it found is selected again afterwards."""
+    from pantomatrix_b200.emage_audio import engine
+    request.addfinalizer(functools.partial(engine.set_precision, engine.get_precision()))
+    engine.set_precision(name)
 
 
 def geodesic_deg(aa_a: torch.Tensor, aa_b: torch.Tensor) -> torch.Tensor:

@@ -309,6 +309,26 @@ def test_fp16_overflow_is_detected_and_recomputed_in_bf16x6(product):
         assert torch.equal(got[k], want[k]), k
 
 
+def test_fp16_overflow_raises_in_the_captured_pipeline(product):
+    """A replay cannot recompute: audio 2e4 times louder than the model's range makes the fp16x3 graph raise PmError
+    naming bf16x6.  Every replay clears the in-graph flag, so the next call on normal audio returns finite outputs."""
+    from pantomatrix_b200 import _lib
+    from pantomatrix_b200.emage_audio import engine
+    from pantomatrix_b200.pipeline import CapturedPipeline
+    model, vqm = product
+    audio = torch.from_numpy(synth_audio(2, 40000, 5))
+    engine.set_precision("fp16x3")
+    try:
+        cap = CapturedPipeline(model, vqm, 2, 40000)
+    finally:
+        engine.set_precision("fp32")
+    with pytest.raises(_lib.PmError, match="bf16x6"):
+        cap((audio * 2e4).cuda())
+    lat, pred = cap(audio.cuda())
+    for k, v in list(lat.items()) + list(pred.items()):
+        assert bool(torch.isfinite(v).all()), k
+
+
 def test_tokenisation_matches_reference_golden(product, golden_dir):
     """map2index / map2latent / EmageVQVAEConv.forward on the GPU against the real reference's outputs
     (tests/golden/case_tokenise.npz); the CPU twin is tests/test_host_logic.py."""

@@ -11,23 +11,20 @@ import torch
 from oracle import emage_oracle as O
 from oracle.weights import make_checkpoint, synth_audio
 import fake_ops
-from helpers import build_product
+from helpers import build_product, use_precision
 
 PARTS = ("face", "upper", "hands", "lower")
 
 
 @pytest.fixture()
-def cpu_product(monkeypatch):
+def cpu_product(monkeypatch, request):
     import pantomatrix_b200.ops as real
     from pantomatrix_b200.emage_audio import modeling
     for name in dir(fake_ops):
         if not name.startswith("_") and callable(getattr(fake_ops, name)) and hasattr(real, name):
             monkeypatch.setattr(real, name, getattr(fake_ops, name))
     monkeypatch.setattr(modeling, "_require_cuda", lambda module, what: torch.device("cpu"))
-    from pantomatrix_b200.emage_audio import engine
-    monkeypatch.setitem(engine._STATE, "nsplit", 0)      # exact fp32 engine unless a test selects a tensor-core mode
-    monkeypatch.setitem(engine._STATE, "precision", "fp32")
-    monkeypatch.setattr(real, "_PLANE_DTYPE", real._PLANE_DTYPE)   # set_precision() may switch the plane format: restore
+    use_precision(request, "fp32")                       # exact fp32 engine unless a test selects a tensor-core mode
     return build_product(seed=0, device="cpu")
 
 
@@ -92,11 +89,37 @@ def test_tensor_core_schedule_host_logic(cpu_product, golden_dir, precision, ato
     g = np.load(os.path.join(golden_dir, "case_tail11.npz"))
     audio = torch.from_numpy(synth_audio(int(g["bs"]), int(g["n_samples"]), int(g["audio_seed"])))
     engine.set_precision(precision)
-    lat, pred = generate(model, vqm, audio)          # (the cpu_product fixture restores the engine state)
+    lat, pred = generate(model, vqm, audio)          # (the cpu_product fixture restores the precision mode)
     for p in PARTS:
         np.testing.assert_allclose(lat["rec_" + p].numpy()[:, ::7], g["rec_" + p], atol=atol, rtol=0)
         agree = (lat["cls_" + p].argmax(-1).numpy() == g["idx_cls_" + p]).mean()
         assert agree > (0.97 if precision == "bf16x3" else 0.999), (p, agree)
+
+
+def test_precision_names_the_mode_that_runs(request):
+    """get_precision() names the mode set_precision() selected; after ops.set_plane_format() changes the plane format
+    under a mode it names the mode that now runs, or refuses when no mode runs that pair.  The fp32 engine builds no
+    planes, so it stays fp32 whatever the plane format."""
+    from pantomatrix_b200 import ops
+    from pantomatrix_b200.emage_audio import engine
+    use_precision(request, "fp32")
+    assert sorted(engine.PRECISIONS) == ["bf16", "bf16x3", "bf16x6", "fp16x3", "fp32"]
+    for name, (nsplit, fmt) in engine.PRECISIONS.items():
+        engine.set_precision(name)
+        assert engine.get_precision() == name and (engine._STATE["nsplit"], ops.plane_format()) == (nsplit, fmt)
+    engine.set_precision("fp16x3")
+    ops.set_plane_format("bf16")                     # two bf16 planes now run: bf16x3 arithmetic, fp32 attention kernel
+    assert engine.get_precision() == "bf16x3" and not engine._attn_tc() and engine.overflow_flag("cpu") is None
+    ops.set_plane_format("fp16")
+    assert engine.get_precision() == "fp16x3" and engine._attn_tc()
+    engine.set_precision("fp32")
+    ops.set_plane_format("fp16")
+    assert engine.get_precision() == "fp32" and not engine._attn_tc() and engine.overflow_flag("cpu") is None
+    for name in ("bf16", "bf16x6"):
+        engine.set_precision(name)
+        ops.set_plane_format("fp16")
+        with pytest.raises(RuntimeError, match="set_precision"):
+            engine.get_precision()
 
 
 @pytest.mark.parametrize("kind", ["camn", "disco"])

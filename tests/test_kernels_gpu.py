@@ -7,7 +7,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from helpers import check_attention, check_l2_argmin, fp64_margins
+from helpers import bf16_planes_by_default, check_attention, check_l2_argmin, fp64_margins  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
@@ -151,16 +151,13 @@ def test_attention_tc(ops, bs, tq, tk):
     qkv = _rand(bs, tq, q0 + 3 * E + 40, seed=20)
     kv = _rand(bs, tk, k0 + 2 * E + 40, seed=21)
     ops.set_plane_format("fp16")
-    try:
-        qp, kvp = ops.split_bf16(qkv, 2), ops.split_bf16(kv, 2)
-        cross_args = (qp, q0, kvp, k0, kvp, k0 + E, bs, H, tq, tk, hd)
-        cross = ops.attention_tc(*cross_args, nsplit=2, f32=True)
-        one = ops.attention_tc(*cross_args, nsplit=1, f32=False)
-        if tq == tk:
-            self_args = (qp, q0, qp, q0 + E, qp, q0 + 2 * E, bs, H, tq, tq, hd)
-            self_att = ops.attention_tc(*self_args, nsplit=0)
-    finally:
-        ops.set_plane_format("bf16")
+    qp, kvp = ops.split_bf16(qkv, 2), ops.split_bf16(kv, 2)
+    cross_args = (qp, q0, kvp, k0, kvp, k0 + E, bs, H, tq, tk, hd)
+    cross = ops.attention_tc(*cross_args, nsplit=2, f32=True)
+    one = ops.attention_tc(*cross_args, nsplit=1, f32=False)
+    if tq == tk:
+        self_args = (qp, q0, qp, q0 + E, qp, q0 + 2 * E, bs, H, tq, tq, hd)
+        self_att = ops.attention_tc(*self_args, nsplit=0)
 
     def ref(q, k, v):
         q, k, v = (x.double().reshape(bs, -1, H, hd).transpose(1, 2) for x in (q, k, v))
@@ -184,15 +181,12 @@ def test_attention_tc_peaked_rows_and_independence(ops):
     E, H, hd, bs, t = 768, 4, 192, 6, 64
     qkv = _rand(bs, t, 3 * E, seed=75, scale=3.2)       # s = q.k / sqrt(192) ~ N(0, 10^2)
     ops.set_plane_format("fp16")
-    try:
-        qp = ops.split_bf16(qkv, 2)
-        args = (qp, 0, qp, E, qp, 2 * E, bs, H, t, t, hd)
-        got = ops.attention_tc(*args, nsplit=2, f32=True)
-        clips = [ops.attention_tc(ops.split_bf16(qkv[b:b + 1], 2), 0, ops.split_bf16(qkv[b:b + 1], 2), E,
-                                  ops.split_bf16(qkv[b:b + 1], 2), 2 * E, 1, H, t, t, hd, nsplit=0) for b in (0, 3, 5)]
-        heads = [ops.attention_tc(qp, h * hd, qp, E + h * hd, qp, 2 * E + h * hd, bs, 1, t, t, hd, nsplit=0) for h in range(H)]
-    finally:
-        ops.set_plane_format("bf16")
+    qp = ops.split_bf16(qkv, 2)
+    args = (qp, 0, qp, E, qp, 2 * E, bs, H, t, t, hd)
+    got = ops.attention_tc(*args, nsplit=2, f32=True)
+    clips = [ops.attention_tc(ops.split_bf16(qkv[b:b + 1], 2), 0, ops.split_bf16(qkv[b:b + 1], 2), E,
+                              ops.split_bf16(qkv[b:b + 1], 2), 2 * E, 1, H, t, t, hd, nsplit=0) for b in (0, 3, 5)]
+    heads = [ops.attention_tc(qp, h * hd, qp, E + h * hd, qp, 2 * E + h * hd, bs, 1, t, t, hd, nsplit=0) for h in range(H)]
     q = qkv[..., :E].double().reshape(bs, t, H, hd).transpose(1, 2)
     k = qkv[..., E:2 * E].double().reshape(bs, t, H, hd).transpose(1, 2)
     s = q @ k.transpose(-1, -2) / math.sqrt(hd)
@@ -487,8 +481,7 @@ def _planes_value(pl):
 @pytest.fixture()
 def plane_format(request, ops):
     ops.set_plane_format(request.param)
-    yield request.param
-    ops.set_plane_format("bf16")
+    return request.param
 
 
 @pytest.mark.parametrize("plane_format", ["bf16", "fp16"], indirect=True)

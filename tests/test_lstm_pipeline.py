@@ -135,20 +135,19 @@ def _lstm_cond_restated(spk, speaker_id, seed, seed_len, seed_frames, pose_dims,
 
 
 @pytest.fixture()
-def emulated(monkeypatch):
+def emulated(monkeypatch, request):
     """The product's host schedule on the CPU: every kernel wrapper replaced by tests/fake_ops.py, and lstm_cond by
     the restatement above; exact fp32 engine."""
     import fake_ops
     import pantomatrix_b200.ops as real
-    from pantomatrix_b200.emage_audio import engine, modeling
+    from pantomatrix_b200.emage_audio import modeling
+    from helpers import use_precision
     for name in dir(fake_ops):
         if not name.startswith("_") and callable(getattr(fake_ops, name)) and hasattr(real, name):
             monkeypatch.setattr(real, name, getattr(fake_ops, name))
     monkeypatch.setattr(real, "lstm_cond", _lstm_cond_restated)
     monkeypatch.setattr(modeling, "_require_cuda", lambda module, what: torch.device("cpu"))
-    monkeypatch.setitem(engine._STATE, "nsplit", 0)
-    monkeypatch.setitem(engine._STATE, "precision", "fp32")
-    monkeypatch.setattr(real, "_PLANE_DTYPE", real._PLANE_DTYPE)
+    use_precision(request, "fp32")
 
 
 @pytest.mark.parametrize("kind", ["camn", "disco"])

@@ -123,6 +123,7 @@ def test_dense_add2_unchanged(ops):
         a, b = torch.randn(n, device="cuda", generator=g), torch.randn(n, device="cuda", generator=g)
         assert _same(ops.add2(a, b), a + b)
     a, b = torch.randn(5, 7, 256, device="cuda", generator=g), torch.randn(5, 7, 256, device="cuda", generator=g)
+    found = ops.plane_format()
     for fmt in ("bf16", "fp16"):
         ops.set_plane_format(fmt)
         try:
@@ -131,7 +132,7 @@ def test_dense_add2_unchanged(ops):
             want = ops.split_bf16(a + b, 2)
             assert torch.equal(r.p.t[..., :256].view(torch.int16), want.t[..., :256].view(torch.int16))
         finally:
-            ops.set_plane_format("fp16")
+            ops.set_plane_format(found)
 
 
 # ---- eager forward: no behaviour change ---------------------------------------------------------------------------

@@ -68,7 +68,7 @@ def _worker(rank, world, port, out_path):
 
 
 @pytest.mark.timeout(600)
-def test_two_rank_sharded_generate_matches_single_process(tmp_path, monkeypatch):
+def test_two_rank_sharded_generate_matches_single_process(tmp_path, monkeypatch, request):
     out_path = str(tmp_path / "rank0.pt")
     mp.spawn(_worker, args=(2, _free_port(), out_path), nprocs=2, join=True)
     got = torch.load(out_path)
@@ -78,14 +78,13 @@ def test_two_rank_sharded_generate_matches_single_process(tmp_path, monkeypatch)
     import pantomatrix_b200.ops as real
     from pantomatrix_b200.emage_audio import modeling
     from pantomatrix_b200.pipeline import generate
-    from helpers import build_product
+    from helpers import build_product, use_precision
     from oracle.weights import synth_audio
     for name in dir(fake_ops):
         if not name.startswith("_") and callable(getattr(fake_ops, name)) and hasattr(real, name):
             monkeypatch.setattr(real, name, getattr(fake_ops, name))
     monkeypatch.setattr(modeling, "_require_cuda", lambda module, what: torch.device("cpu"))
-    from pantomatrix_b200.emage_audio import engine
-    monkeypatch.setitem(engine._STATE, "nsplit", 0)
+    use_precision(request, "fp32")
     model, vqm = build_product(seed=0, device="cpu")
     lat, pred = generate(model, vqm, torch.from_numpy(synth_audio(3, 21600, 77)))
     assert got["aa"].shape == pred["motion_axis_angle"].shape

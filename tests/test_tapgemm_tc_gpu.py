@@ -10,7 +10,7 @@ import math
 import pytest
 import torch
 
-from helpers import check_tapgemm, slack_rows
+from helpers import bf16_planes_by_default, check_tapgemm, slack_rows  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
@@ -93,10 +93,7 @@ def test_tapgemm_tc_fp16_planes(ops, case):
     """Two IEEE fp16 planes, 3 products: the accuracy class of bf16x6 (weights packed pre-scaled by a power of two,
     undone by acc_scale in the epilogue)."""
     ops.set_plane_format("fp16")
-    try:
-        _run_case(ops, case, 2)
-    finally:
-        ops.set_plane_format("bf16")
+    _run_case(ops, case, 2)
 
 
 def test_partial_activation_and_column_slices(ops):
@@ -141,17 +138,14 @@ def test_fp16_planes_small_activations(ops, scale, tol):
     and 20x smaller activations keep the fp32-class accuracy; only tensors that are tiny as a whole (1e-3) degrade to
     single-plane fp16 accuracy (2^-11) - no tensor of this model is that small (smallest GEMM input: ~0.05)."""
     ops.set_plane_format("fp16")
-    try:
-        x = _rand(1, 256, 768, seed=11, scale=scale)
-        w = _rand(1, 256, 768, seed=12, scale=1 / math.sqrt(768))
-        want = torch.nn.functional.linear(x.double(), w[0].double())
-        a, pw = ops.split_bf16(x, 2), ops.PackedW(w, 2)
-        got, _ = ops.tapgemm_tc(a, pw, None, rows_out=256)
-        err = (got.double() - want).abs().max().item()
-        assert err <= tol * float(want.abs().max()), err
-        _check(a, pw, None, got, rows_out=256, tag=f"fp16 activations x{scale}")
-    finally:
-        ops.set_plane_format("bf16")
+    x = _rand(1, 256, 768, seed=11, scale=scale)
+    w = _rand(1, 256, 768, seed=12, scale=1 / math.sqrt(768))
+    want = torch.nn.functional.linear(x.double(), w[0].double())
+    a, pw = ops.split_bf16(x, 2), ops.PackedW(w, 2)
+    got, _ = ops.tapgemm_tc(a, pw, None, rows_out=256)
+    err = (got.double() - want).abs().max().item()
+    assert err <= tol * float(want.abs().max()), err
+    _check(a, pw, None, got, rows_out=256, tag=f"fp16 activations x{scale}")
 
 
 @pytest.mark.parametrize("fmt,nsplit", [("bf16", 1), ("bf16", 2), ("bf16", 3), ("fp16", 2)])
@@ -159,27 +153,24 @@ def test_clips_are_independent(ops, fmt, nsplit):
     """7 clips packed 8 per 128-row tile (R = 16) give bit-identical rows to each clip alone (R = 128) and to the batch
     in reverse order; a Linear over the clips as one tall matrix (Planes.flat) equals the per-clip call."""
     ops.set_plane_format(fmt)
-    try:
-        x = _rand(7, 16, 256, seed=13)
-        pw = ops.PackedW(_rand(3, 96, 256, seed=14, scale=1 / 28), nsplit)
-        bias, res = _rand(96, seed=15, scale=0.1), _rand(7, 16, 96, seed=16)
-        kw = dict(rows_out=16, pad=1, act=ops.ACT_LEAKY, slope=0.2)
-        a = ops.split_bf16(x, nsplit)
-        got, pl = ops.tapgemm_tc(a, pw, bias, residual=res, out_nsplit=nsplit, **kw)
-        _check(a, pw, bias, got, pl, residual=res, tag="7 packed clips", **kw)
-        rev, pl_rev = ops.tapgemm_tc(ops.split_bf16(x.flip(0), nsplit), pw, bias, residual=res.flip(0), out_nsplit=nsplit, **kw)
-        assert torch.equal(rev.flip(0), got) and torch.equal(pl_rev.t.flip(1)[..., :96], pl.t[..., :96])
-        for b in range(7):
-            one, _ = ops.tapgemm_tc(ops.split_bf16(x[b:b + 1], nsplit), pw, bias, residual=res[b:b + 1], **kw)
-            assert torch.equal(one, got[b:b + 1]), b
-        # 1x1 Linear: the flat tall matrix against the per-clip (packed) call
-        pl1 = ops.PackedW(_rand(1, 80, 256, seed=17, scale=1 / 16), nsplit)
-        per_clip, _ = ops.tapgemm_tc(a, pl1, bias[:80], rows_out=16)
-        flat, _ = ops.tapgemm_tc(a.flat(), pl1, bias[:80], rows_out=7 * 16)
-        assert torch.equal(flat.view(7, 16, 80), per_clip)
-        _check(a.flat(), pl1, bias[:80], flat, rows_out=7 * 16, tag="flat Linear")
-    finally:
-        ops.set_plane_format("bf16")
+    x = _rand(7, 16, 256, seed=13)
+    pw = ops.PackedW(_rand(3, 96, 256, seed=14, scale=1 / 28), nsplit)
+    bias, res = _rand(96, seed=15, scale=0.1), _rand(7, 16, 96, seed=16)
+    kw = dict(rows_out=16, pad=1, act=ops.ACT_LEAKY, slope=0.2)
+    a = ops.split_bf16(x, nsplit)
+    got, pl = ops.tapgemm_tc(a, pw, bias, residual=res, out_nsplit=nsplit, **kw)
+    _check(a, pw, bias, got, pl, residual=res, tag="7 packed clips", **kw)
+    rev, pl_rev = ops.tapgemm_tc(ops.split_bf16(x.flip(0), nsplit), pw, bias, residual=res.flip(0), out_nsplit=nsplit, **kw)
+    assert torch.equal(rev.flip(0), got) and torch.equal(pl_rev.t.flip(1)[..., :96], pl.t[..., :96])
+    for b in range(7):
+        one, _ = ops.tapgemm_tc(ops.split_bf16(x[b:b + 1], nsplit), pw, bias, residual=res[b:b + 1], **kw)
+        assert torch.equal(one, got[b:b + 1]), b
+    # 1x1 Linear: the flat tall matrix against the per-clip (packed) call
+    pl1 = ops.PackedW(_rand(1, 80, 256, seed=17, scale=1 / 16), nsplit)
+    per_clip, _ = ops.tapgemm_tc(a, pl1, bias[:80], rows_out=16)
+    flat, _ = ops.tapgemm_tc(a.flat(), pl1, bias[:80], rows_out=7 * 16)
+    assert torch.equal(flat.view(7, 16, 80), per_clip)
+    _check(a.flat(), pl1, bias[:80], flat, rows_out=7 * 16, tag="flat Linear")
 
 
 def test_prefetch_does_not_change_results(ops):
@@ -213,28 +204,25 @@ def test_strided_out_and_residual_views(ops, fmt, nsplit):
     """out= and residual= as column views of wider tensors with odd row strides (ldo 101, ldr 77: the per-element
     epilogue), clip stride != rows * ld: the result lands in the view only, every other element is untouched."""
     ops.set_plane_format(fmt)
-    try:
-        for batch, rows, taps, pad in ((3, 40, 3, 1), (2, 150, 1, 0)):
-            cout = 70
-            x = _rand(batch, rows, 128, seed=21)
-            pw = ops.PackedW(_rand(taps, cout, 128, seed=22, scale=0.05), nsplit)
-            bias = _rand(cout, seed=23, scale=0.1)
-            big_out = _rand(batch, rows + 5, 101, seed=24)
-            big_res = _rand(batch, rows + 2, 77, seed=25)
-            out, res = big_out[:, 2:2 + rows, 13:13 + cout], big_res[:, 1:1 + rows, 3:3 + cout]
-            base, mask = _outside(out)
-            keep = base[mask].clone()
-            res_before = big_res.clone()
-            a = ops.split_bf16(x, nsplit)
-            kw = dict(rows_out=rows, pad=pad, act=ops.ACT_RELU, residual=res)
-            got, pl = ops.tapgemm_tc(a, pw, bias, out=out, out_nsplit=nsplit, out_slack=8, **kw)
-            assert got.data_ptr() == out.data_ptr()
-            assert torch.equal(base[mask], keep), "epilogue wrote outside the out= view"
-            assert torch.equal(big_res, res_before)
-            assert int(torch.count_nonzero(slack_rows(pl))) == 0
-            _check(a, pw, bias, out, pl, tag=f"strided out/residual {(batch, rows, taps)} {fmt}", **kw)
-    finally:
-        ops.set_plane_format("bf16")
+    for batch, rows, taps, pad in ((3, 40, 3, 1), (2, 150, 1, 0)):
+        cout = 70
+        x = _rand(batch, rows, 128, seed=21)
+        pw = ops.PackedW(_rand(taps, cout, 128, seed=22, scale=0.05), nsplit)
+        bias = _rand(cout, seed=23, scale=0.1)
+        big_out = _rand(batch, rows + 5, 101, seed=24)
+        big_res = _rand(batch, rows + 2, 77, seed=25)
+        out, res = big_out[:, 2:2 + rows, 13:13 + cout], big_res[:, 1:1 + rows, 3:3 + cout]
+        base, mask = _outside(out)
+        keep = base[mask].clone()
+        res_before = big_res.clone()
+        a = ops.split_bf16(x, nsplit)
+        kw = dict(rows_out=rows, pad=pad, act=ops.ACT_RELU, residual=res)
+        got, pl = ops.tapgemm_tc(a, pw, bias, out=out, out_nsplit=nsplit, out_slack=8, **kw)
+        assert got.data_ptr() == out.data_ptr()
+        assert torch.equal(base[mask], keep), "epilogue wrote outside the out= view"
+        assert torch.equal(big_res, res_before)
+        assert int(torch.count_nonzero(slack_rows(pl))) == 0
+        _check(a, pw, bias, out, pl, tag=f"strided out/residual {(batch, rows, taps)} {fmt}", **kw)
 
 
 @pytest.mark.parametrize("fmt,nsplit", [("bf16", 1), ("bf16", 2), ("bf16", 3), ("fp16", 2)])
@@ -242,16 +230,13 @@ def test_plane_only_output_with_slack(ops, fmt, nsplit):
     """want_f32=False: the planes are the only result (checked against float64 directly), with out_nsplit below the
     operand split and out_slack zeroed rows after the last clip."""
     ops.set_plane_format(fmt)
-    try:
-        for batch, rows, taps, pad, out_ns in ((5, 33, 3, 1, nsplit), (2, 300, 15, 7, max(1, nsplit - 1))):
-            x = _rand(batch, rows, 64, seed=26)
-            pw = ops.PackedW(_rand(taps, 64, 64, seed=27, scale=1 / math.sqrt(64 * taps)), nsplit)
-            bias, res = _rand(64, seed=28, scale=0.1), _rand(batch, rows, 64, seed=29)
-            a = ops.split_bf16(x, nsplit)
-            kw = dict(rows_out=rows, pad=pad, act=ops.ACT_LEAKY, slope=0.01, residual=res)
-            f, pl = ops.tapgemm_tc(a, pw, bias, want_f32=False, out_nsplit=out_ns, out_slack=8, **kw)
-            assert f is None and pl.nsplit == out_ns and pl.slack == 8
-            assert int(torch.count_nonzero(slack_rows(pl))) == 0
-            _check(a, pw, bias, None, pl, tag=f"planes only {(batch, rows, taps)} out_nsplit={out_ns} {fmt}", **kw)
-    finally:
-        ops.set_plane_format("bf16")
+    for batch, rows, taps, pad, out_ns in ((5, 33, 3, 1, nsplit), (2, 300, 15, 7, max(1, nsplit - 1))):
+        x = _rand(batch, rows, 64, seed=26)
+        pw = ops.PackedW(_rand(taps, 64, 64, seed=27, scale=1 / math.sqrt(64 * taps)), nsplit)
+        bias, res = _rand(64, seed=28, scale=0.1), _rand(batch, rows, 64, seed=29)
+        a = ops.split_bf16(x, nsplit)
+        kw = dict(rows_out=rows, pad=pad, act=ops.ACT_LEAKY, slope=0.01, residual=res)
+        f, pl = ops.tapgemm_tc(a, pw, bias, want_f32=False, out_nsplit=out_ns, out_slack=8, **kw)
+        assert f is None and pl.nsplit == out_ns and pl.slack == 8
+        assert int(torch.count_nonzero(slack_rows(pl))) == 0
+        _check(a, pw, bias, None, pl, tag=f"planes only {(batch, rows, taps)} out_nsplit={out_ns} {fmt}", **kw)

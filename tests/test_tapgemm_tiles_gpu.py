@@ -5,7 +5,7 @@ forced both ways, and each result is also held to helpers.check_tapgemm's per-el
 import pytest
 import torch
 
-from helpers import check_tapgemm, slack_rows
+from helpers import bf16_planes_by_default, check_tapgemm, slack_rows  # noqa: F401
 from test_tapgemm_tc_gpu import CASES, _inputs, _outside, _rand
 
 pytestmark = pytest.mark.gpu
@@ -25,8 +25,7 @@ def ops():
 @pytest.fixture
 def fmt_ops(ops, request):
     ops.set_plane_format(request.param)
-    yield ops
-    ops.set_plane_format("bf16")
+    return ops
 
 
 @pytest.mark.parametrize("fmt_ops,nsplit", FORMATS, indirect=["fmt_ops"])
