@@ -4,9 +4,9 @@
     python examples/camn_disco_demo.py --model camn --checkpoint /path/to/camn_audio --audio_folder ./wavs
     python examples/camn_disco_demo.py --model disco --synthetic --audio_folder ./wavs
 
-These models emit the upper body + hands only and no translation; like the reference demos this needs the SMPL-X body
-model to place the pelvis when writing the npz, which is not available offline - so here the pelvis translation is
-written as zeros (pass --trans-zero explicitly to acknowledge)."""
+These models emit the upper body + hands only and no translation; like the reference demos the npz writer places the
+pelvis with the SMPL-X body model: pass the model file with --smplx SMPLX_NEUTRAL_2020.npz (the translation the
+reference writer derives), or --trans-zero to write zeros instead."""
 import argparse
 import os
 import sys
@@ -32,10 +32,15 @@ def main():
     ap.add_argument("--checkpoint", default=None)
     ap.add_argument("--synthetic", action="store_true")
     ap.add_argument("--trans-zero", action="store_true")
+    ap.add_argument("--smplx", default=None, metavar="PATH", help="SMPL-X model file (SMPLX_NEUTRAL_2020.npz)")
     args = ap.parse_args()
-    if not args.trans_zero:
-        ap.error("the npz needs a pelvis translation; without the SMPL-X model files pass --trans-zero to write zeros")
+    if not args.trans_zero and args.smplx is None:
+        ap.error("the npz needs a pelvis translation: pass --smplx SMPLX_NEUTRAL_2020.npz, or --trans-zero to write zeros")
     device = torch.device("cuda")
+    body_model = None
+    if args.smplx is not None and not args.trans_zero:
+        from pantomatrix_b200.body_model import SmplxBodyModel
+        body_model = SmplxBodyModel.from_npz(args.smplx, device)
     if args.synthetic:
         sys.path.insert(0, os.path.join(ROOT, "tests"))
         from synthetic_models import build_lstm_product
@@ -50,8 +55,9 @@ def main():
         audio = torch.from_numpy(load_audio(os.path.join(args.audio_folder, name), sr=sr)).unsqueeze(0).to(device)
         aa = model(audio, torch.zeros(1, 1, dtype=torch.long, device=device), seed_frames=seed_frames)["motion_axis_angle"]
         t = aa.shape[1]
+        trans = None if body_model is not None else np.zeros((t, 3), dtype=np.float32)
         beat_format_save(os.path.join(args.save_folder, os.path.splitext(name)[0] + "_output.npz"),
-                         aa.cpu().numpy().reshape(t, -1), upsample=30 // fps, trans=np.zeros((t, 3), dtype=np.float32))
+                         aa.cpu().numpy().reshape(t, -1), upsample=30 // fps, trans=trans, body_model=body_model)
         frames += t
     print(f"generate total {frames / fps:.2f} seconds motion in {time.time() - t0:.2f} seconds, saved in {args.save_folder}")
 

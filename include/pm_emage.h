@@ -226,6 +226,46 @@ int pm_rot6d_to_aa_f32(const float* rot6d, long long rows, int n_sel, const int*
 int pm_softmax2_mix_f32(const float* sel, const float* c1, const float* c2, float* out, long long rows, int ch, int ldo,
                         void* stream);
 
+/* ---- SMPL-X body model (pantomatrix_b200/body_model.py): the smplx forward pass that every consumer of generated poses
+ * runs next (emage_utils/motion_rep_transfer.py:38-50, emage_utils/motion_io.py:117-140, datasets/foot_contact.py:46-58).
+ * Frames are rows r = b*t + i of `batch` clips of `t` frames; every per-frame input has a clip stride *_bs and a frame
+ * stride *_ts in elements and a dense last dimension (views are read in place).
+ *
+ * pm_smplx_fk_f32: rest joints, Rodrigues and forward kinematics of every frame in one launch.
+ *   poses (batch, t, 165) axis-angle, joint-major; joint j is used when bit j of joint_mask is set, else it reads as zero;
+ *   pose_mean[165] (the hand means) is added afterwards.  betas (batch, 300) per clip and expr (batch, t, 100) per frame,
+ *   both nullable (= zeros); transl (batch, t, 3) nullable.
+ *   J = j_template (55*3) + j_dirs^T [betas | expr] with j_dirs (400, 55*3) = J_regressor . shapedirs.
+ *   R_j = I + sin K + (1 - cos) K K, angle = |r + 1e-8| (smplx batch_rodrigues).  G_j = G_parent [R_j | J_j - J_parent],
+ *   evaluated one tree level at a time: level_order[55] lists the joints by depth, level l is
+ *   level_order[level_start[l] .. level_start[l+1]), n_levels <= 55; parents[55] with -1 at the root.
+ *   Writes joints (rows, 55, 3) dense = G_j[:, 3] + transl, and (each nullable):
+ *     rel_transforms (rows, 55, 12): A_j = G_j - [0 | G_j (J_j, 0)], the 3x4 rows of smplx's relative transforms;
+ *     the vertex GEMM's A operand row [betas | expr | (R_1 - I) .. (R_54 - I)] (886 values, R row-major) as fp32 `feat`
+ *     (row stride ld_feat >= 886) and / or as operand planes (p_nsplit | PM_FMT_F16 as for pm_add_layernorm_f32). */
+int pm_smplx_fk_f32(const float* poses, long long pose_bs, long long pose_ts,
+                    const float* betas, long long b_bs,
+                    const float* expr, long long e_bs, long long e_ts,
+                    const float* transl, long long t_bs, long long t_ts,
+                    long long joint_mask, int batch, int t,
+                    const float* j_template, const float* j_dirs, const float* pose_mean,
+                    const int* parents, const int* level_order, const int* level_start, int n_levels,
+                    float* joints, float* rel_transforms, float* feat, int ld_feat,
+                    uint16_t* planes, long long p_ps, int p_ld, int p_nsplit, void* stream);
+/* pm_smplx_skin_f32: linear blend skinning in place.  verts (rows, ld >= 3*n_verts) holds v_posed (the vertex GEMM's
+ * output, vertex-major xyz) and receives (sum_j w_vj A_j) (v_posed, 1) + transl.  Weights in CSR form: row_ptr
+ * (n_verts + 1), col / val (row_ptr[n_verts]).  rel_transforms (rows, 55, 12) from pm_smplx_fk_f32; transl as there
+ * (nullable; t = frames per clip). */
+int pm_smplx_skin_f32(float* verts, long long ld, long long rows, int n_verts,
+                      const int* row_ptr, const int* col, const float* val, const float* rel_transforms,
+                      const float* transl, long long t_bs, long long t_ts, int t, void* stream);
+/* pm_motion_rep_f32: get_motion_rep_tensor (emage_utils/motion_rep_transfer.py:31-72).  poses (batch, t, 165) as above,
+ * joints (batch, t, 55, 3) dense -> rep15d (batch, t, 55*15) dense, per joint [position | velocity | rot6d (quaternion
+ * route, P.py:63-104) | angular velocity].  Velocities: (x[i+1] - x[i-1]) / two_dt inside a clip, one-sided over dt at
+ * both ends (t >= 2). */
+int pm_motion_rep_f32(const float* poses, long long pose_bs, long long pose_ts, const float* joints,
+                      int batch, int t, float dt, float two_dt, float* rep15d, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

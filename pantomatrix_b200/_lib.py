@@ -47,6 +47,10 @@ SIGNATURES = {
     "pm_rot6d_to_aa_f32": [_p, _ll, _i, _p, _p, _p],
     "pm_softmax2_mix_f32": [_p, _p, _p, _p, _ll, _i, _i, _p],
     "pm_resample_poly_f32": [_p, _i, _ll, _i, _ll, _i, _p, _i, _i, _i, _ll, _p, _ll, _p],
+    "pm_smplx_fk_f32": [_p, _ll, _ll, _p, _ll, _p, _ll, _ll, _p, _ll, _ll, _ll, _i, _i, _p, _p, _p, _p, _p, _p, _i,
+                        _p, _p, _p, _i, _p, _ll, _i, _i, _p],
+    "pm_smplx_skin_f32": [_p, _ll, _ll, _i, _p, _p, _p, _p, _p, _ll, _ll, _i, _p],
+    "pm_motion_rep_f32": [_p, _ll, _ll, _p, _i, _i, _f, _f, _p, _p],
 }
 
 _lib = None

@@ -1,4 +1,5 @@
-// Pose composition (EmageVQModel.decode, M.py:135-188) and global translation (M.py:195-205).
+// Pose composition (EmageVQModel.decode, M.py:135-188), global translation (M.py:195-205) and the motion
+// representation of the body model (pm_motion_rep_f32).
 // Compiled with -fmad=false: the rotation formulas follow the reference's operation order
 // (P.py:6-104) with one rounding per operation, like the eager torch kernels they replace.
 // Contracts: include/pm_emage.h.
@@ -160,7 +161,54 @@ __global__ void __launch_bounds__(256) softmax2_mix_kernel(const float* __restri
   }
 }
 
+// get_motion_rep_tensor (emage_utils/motion_rep_transfer.py:31-72): per (frame, joint) the 15 values
+// [position | velocity | rot6d | angular velocity].  Differences are one-sided at both ends of a clip and central inside,
+// subtracted and then divided by dt or 2 dt (float32 roundings of the reference's Python scalars), one rounding per op.
+__global__ void __launch_bounds__(256) motion_rep_kernel(const float* __restrict__ poses, long long pose_bs,
+                                                         long long pose_ts, const float* __restrict__ joints,
+                                                         long long rows, int t, float dt, float two_dt,
+                                                         float* __restrict__ rep) {
+  const long long total = rows * 55;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+    const long long r = i / 55;
+    const int j = (int)(i % 55);
+    const long long b = r / t;
+    const int tt = (int)(r % t);
+    const int hi = tt + 1 < t ? tt + 1 : tt, lo = tt > 0 ? tt - 1 : tt;
+    const float den = (tt == 0 || tt == t - 1) ? dt : two_dt;
+    const float* jh = joints + ((b * t + hi) * 55 + j) * 3;
+    const float* jl = joints + ((b * t + lo) * 55 + j) * 3;
+    const float* p = poses + b * pose_bs + (long long)tt * pose_ts + 3 * j;
+    const float* ph = poses + b * pose_bs + (long long)hi * pose_ts + 3 * j;
+    const float* pl = poses + b * pose_bs + (long long)lo * pose_ts + 3 * j;
+    float* o = rep + r * 825 + j * 15;
+    const float aa[3] = {p[0], p[1], p[2]};
+    float r6[6];
+    aa_to_rot6d(aa, r6);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      o[c] = joints[(r * 55 + j) * 3 + c];
+      o[3 + c] = (jh[c] - jl[c]) / den;
+      o[12 + c] = (ph[c] - pl[c]) / den;
+    }
+#pragma unroll
+    for (int c = 0; c < 6; ++c) o[6 + c] = r6[c];
+  }
+}
+
 }  // namespace
+
+extern "C" int pm_motion_rep_f32(const float* poses, long long pose_bs, long long pose_ts, const float* joints,
+                                 int batch, int t, float dt, float two_dt, float* rep15d, void* stream) {
+  PM_REQUIRE(poses && joints && rep15d && batch >= 0 && t >= 2 && dt > 0.f && two_dt > 0.f);
+  const long long rows = (long long)batch * t;
+  if (rows == 0) return PM_OK;
+  long long g = (rows * 55 + 255) / 256;
+  if (g > 148 * 16) g = 148 * 16;
+  motion_rep_kernel<<<(unsigned)g, 256, 0, (cudaStream_t)stream>>>(poses, pose_bs, pose_ts, joints, rows, t, dt, two_dt,
+                                                                  rep15d);
+  PM_LAUNCH_CHECK();
+}
 
 extern "C" int pm_rot6d_to_aa_f32(const float* rot6d, long long rows, int n_sel, const int* slot, float* out, void* stream) {
   PM_REQUIRE(rot6d && slot && out && rows >= 0 && n_sel > 0 && n_sel <= 55);

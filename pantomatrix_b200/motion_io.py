@@ -2,10 +2,10 @@
 
 Behavioural mirror of the parts of /root/reference/emage_utils/motion_io.py the demo needs
 (`beat_format_save` :103-163, `beat_format_load` :165-179, `time_upsample_numpy` :69-101, joint-mask
-select / recover :22-67), written against numpy only.  The reference module imports `smplx` at import time
-and, when `trans` is None, builds a licensed SMPL-X body model to derive a default translation; neither is
-available offline, so here `trans=None` raises with an explanation instead (the EMAGE demo always passes the
-translation it generated, test_emage_audio.py:53-55).
+select / recover :22-67), written against numpy only.  When `trans` is None the reference builds the SMPL-X body
+model to derive a default translation; here the caller passes the model (`body_model=`, pantomatrix_b200.body_model),
+and without one `trans=None` raises with an explanation (the EMAGE demo always passes the translation it generated,
+test_emage_audio.py:53-55).
 """
 from __future__ import annotations
 
@@ -45,9 +45,22 @@ def select_with_mask(motion: np.ndarray, mask) -> np.ndarray:
     return picked.reshape(motion.shape[:-1] + (int(mask.sum()) * c,))
 
 
-def beat_format_save(save_path, motion_data, mask=None, betas=None, expressions=None, trans=None, upsample=None):
+def pelvis_translation(body_model, betas0) -> np.ndarray:
+    """(3,) float32 translation the reference writer derives when none is given (motion_io.py:116-143): minus the
+    midpoint of joints 10 and 11 (the feet) of the rest pose for betas0 (300,).  body_model: a
+    body_model.SmplxBodyModel (or anything with its forward() and device)."""
+    import torch
+    dev = body_model.device
+    b = torch.from_numpy(np.asarray(betas0)[None]).float().to(dev)
+    joints = body_model.forward(torch.zeros(1, 1, 165, device=dev), betas=b)["joints"].reshape(-1, 55, 3)[:1].cpu()
+    return (-((joints[:, 10, :] + joints[:, 11, :]) / 2)).numpy()[0]
+
+
+def beat_format_save(save_path, motion_data, mask=None, betas=None, expressions=None, trans=None, upsample=None,
+                     body_model=None):
     """Write a BEAT-format npz: betas (300,), poses (T,165), expressions (T,100), trans (T,3), model, gender,
-    mocap_frame_rate - same keys, shapes and constants as the reference writer."""
+    mocap_frame_rate - same keys, shapes and constants as the reference writer.  trans=None places the pelvis as the
+    reference does (pelvis_translation of betas[0], repeated over the frames), which needs the SMPL-X `body_model`."""
     motion_data = np.asarray(motion_data)
     n = motion_data.shape[0]
     if betas is None:
@@ -55,9 +68,12 @@ def beat_format_save(save_path, motion_data, mask=None, betas=None, expressions=
     if expressions is None:
         expressions = np.zeros((n, 100), dtype=motion_data.dtype)
     if trans is None:
-        raise NotImplementedError(
-            "beat_format_save(trans=None) needs the SMPL-X body model (licensed files + the smplx package) to place "
-            "the pelvis; pass the translation produced by EmageVQModel.decode(get_global_motion=True)")
+        if body_model is None:
+            raise NotImplementedError(
+                "beat_format_save(trans=None) needs the SMPL-X body model to place the pelvis: pass "
+                "body_model=body_model.SmplxBodyModel.from_npz('SMPLX_NEUTRAL_2020.npz'), or the translation produced "
+                "by EmageVQModel.decode(get_global_motion=True)")
+        trans = np.repeat(pelvis_translation(body_model, betas[0])[None], n, axis=0)
     if mask is not None:
         motion_data = recover_from_mask(motion_data, mask)
     if upsample is not None and upsample > 1:

@@ -566,6 +566,60 @@ def rot6d_to_aa(rot6d, slot, n_sel):
     return out
 
 
+# ------------------------------------------------------------------------------------------------------
+# SMPL-X body model
+# ------------------------------------------------------------------------------------------------------
+
+
+def _clip_frame_strides(x):
+    """(clip stride, frame stride) of a (batch, t, ch) view."""
+    return (x.stride(0), x.stride(1)) if x is not None else (0, 0)
+
+
+def smplx_fk(poses, betas, expression, transl, joint_mask, tables, joints, rel=None, feat=None, planes=None):
+    """Rest joints + Rodrigues + forward kinematics (include/pm_emage.h pm_smplx_fk_f32).  poses (batch, t, 165),
+    betas (batch, 300), expression (batch, t, 100), transl (batch, t, 3): views with a dense last dim, the last three
+    nullable.  tables = (j_template, j_dirs, pose_mean, parents, level_order, level_start) device tensors.  Writes
+    joints (batch*t, 55, 3), rel (batch*t, 55, 12) and the GEMM operand row as fp32 `feat` (rows, ld) and / or Planes."""
+    for x in (poses, betas, expression, transl, joints, rel, feat):
+        if x is not None:
+            _chk(x)
+    jt, jd, pm, par, order, lstart = tables
+    batch, t, _ = poses.shape
+    pb, pt = _clip_frame_strides(poses)
+    eb, et = _clip_frame_strides(expression)
+    tb, tt = _clip_frame_strides(transl)
+    _call("pm_smplx_fk_f32", poses.data_ptr(), pb, pt, _ptr(betas), 0 if betas is None else betas.stride(0),
+          _ptr(expression), eb, et, _ptr(transl), tb, tt, int(joint_mask), batch, t,
+          jt.data_ptr(), jd.data_ptr(), pm.data_ptr(), par.data_ptr(), order.data_ptr(), lstart.data_ptr(),
+          lstart.numel() - 1, joints.data_ptr(), _ptr(rel), _ptr(feat), 0 if feat is None else feat.stride(0),
+          *_pargs(planes), _stream())
+    return joints
+
+
+def smplx_skin(verts, n_verts, csr, rel, transl, t):
+    """Linear blend skinning in place over verts (rows, ld) = v_posed (pm_smplx_skin_f32); csr = (row_ptr, col, val)."""
+    _chk(verts), _chk(rel)
+    row_ptr, col, val = csr
+    tb, tt = _clip_frame_strides(transl)
+    if transl is not None:
+        _chk(transl)
+    _call("pm_smplx_skin_f32", verts.data_ptr(), verts.stride(0), verts.shape[0], int(n_verts), row_ptr.data_ptr(),
+          col.data_ptr(), val.data_ptr(), rel.data_ptr(), _ptr(transl), tb, tt, int(t), _stream())
+    return verts
+
+
+def motion_rep(poses, joints, dt, two_dt, out):
+    """rep15d (batch, t, 825) of get_motion_rep_tensor from poses (batch, t, 165) and joints (batch, t, 55, 3)."""
+    _chk(poses), _chk(joints), _chk(out)
+    assert joints.is_contiguous() and out.is_contiguous()
+    batch, t, _ = poses.shape
+    pb, pt = _clip_frame_strides(poses)
+    _call("pm_motion_rep_f32", poses.data_ptr(), pb, pt, joints.data_ptr(), batch, t, float(dt), float(two_dt),
+          out.data_ptr(), _stream())
+    return out
+
+
 def softmax2_mix(sel, c1, c2, out=None):
     """out[..., :] = softmax(sel[..., 0:2])[0] * c1 + [1] * c2 (out may be a column slice of a wider tensor)."""
     _chk(sel), _chk(c1), _chk(c2)
