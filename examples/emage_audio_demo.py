@@ -3,7 +3,11 @@
 
     python examples/emage_audio_demo.py --checkpoint /path/to/emage_audio --audio_folder ./wavs --save_folder ./out
     python examples/emage_audio_demo.py --synthetic --audio_folder ./wavs            # seeded random weights (no network)
+    python examples/emage_audio_demo.py ... --smplx SMPLX_NEUTRAL_2020.npz --render   # + <name>_frames/frame_%05d.png
 
+`--render` draws the reference demo's two-view SMPL-X frames (fast_render.py render_one_sequence_with_face: face
+close-up left, body right, whole seconds at 30 fps) on the GPU and writes them as PNG files with Pillow next to each
+npz; video encoding is left to the user (e.g. ffmpeg -framerate 30 -i frame_%05d.png).
 `--checkpoint` is a local copy of the Hugging Face repo layout the reference downloads (config.json +
 model.safetensors at the top level, VQ models under emage_vq/{face,upper,lower,hands,global}).
 """
@@ -36,18 +40,35 @@ def load_models(args, device):
     return EmageAudioModel.from_pretrained(ck).to(device).eval(), motion_vq
 
 
+def write_frames(frames, folder):
+    """(N, 720, 960, 3) uint8 frames -> folder/frame_%05d.png."""
+    from PIL import Image
+    os.makedirs(folder, exist_ok=True)
+    for i, img in enumerate(frames.cpu().numpy()):
+        Image.fromarray(img).save(os.path.join(folder, f"frame_{i:05d}.png"))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--audio_folder", default="./examples/audio")
     ap.add_argument("--save_folder", default="./examples/motion")
     ap.add_argument("--checkpoint", default=None)
     ap.add_argument("--synthetic", action="store_true")
+    ap.add_argument("--smplx", default=None, help="SMPLX_NEUTRAL_2020.npz (needed by --render)")
+    ap.add_argument("--render", action="store_true")
     args = ap.parse_args()
     if not args.synthetic and not args.checkpoint:
         ap.error("give --checkpoint DIR or --synthetic")
+    if args.render and not args.smplx:
+        ap.error("--render needs --smplx SMPLX_NEUTRAL_2020.npz")
     os.makedirs(args.save_folder, exist_ok=True)
     device = torch.device("cuda")                      # no CPU fallback by design
     model, motion_vq = load_models(args, device)
+    renderer = None
+    if args.render:
+        from pantomatrix_b200.body_model import SmplxBodyModel
+        from pantomatrix_b200.render import MeshRenderer
+        renderer = MeshRenderer(SmplxBodyModel.from_npz(args.smplx, device))
     sr, fps = model.cfg.audio_sr, model.cfg.pose_fps
     files = sorted(f for f in os.listdir(args.audio_folder) if f.endswith(".wav"))
     frames, t0 = 0, time.time()
@@ -55,10 +76,13 @@ def main():
         audio = torch.from_numpy(load_audio(os.path.join(args.audio_folder, name), sr=sr)).unsqueeze(0)
         _, pred = generate(model, motion_vq, audio.to(device))
         t = pred["motion_axis_angle"].shape[1]
-        beat_format_save(os.path.join(args.save_folder, os.path.splitext(name)[0] + "_output.npz"),
-                         pred["motion_axis_angle"].cpu().numpy().reshape(t, -1), upsample=30 // fps,
+        npz = os.path.join(args.save_folder, os.path.splitext(name)[0] + "_output.npz")
+        beat_format_save(npz, pred["motion_axis_angle"].cpu().numpy().reshape(t, -1), upsample=30 // fps,
                          expressions=pred["expression"].cpu().numpy().reshape(t, -1),
                          trans=pred["trans"].cpu().numpy().reshape(t, -1))
+        if renderer is not None:
+            write_frames(renderer.render_sequence(pred["motion_axis_angle"], pred["expression"], pred["trans"])[0],
+                         os.path.splitext(npz)[0] + "_frames")
         frames += t
     print(f"generate total {frames / fps:.2f} seconds motion in {time.time() - t0:.2f} seconds")
 

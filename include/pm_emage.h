@@ -266,6 +266,41 @@ int pm_smplx_skin_f32(float* verts, long long ld, long long rows, int n_verts,
 int pm_motion_rep_f32(const float* poses, long long pose_bs, long long pose_ts, const float* joints,
                       int batch, int t, float dt, float two_dt, float* rep15d, void* stream);
 
+/* ---- SMPL-X mesh render (pantomatrix_b200/render.py): emage_utils/fast_render.py:286-321
+ * render_one_sequence_with_face, whose frames (fast_render.py:56-68 do_render_one_frame, 80-92 np.hstack) are two
+ * 480 x 720 views side by side, 960 x 720 RGB uint8, row 0 at the top, black background.  Fixed scene (fast_render.py:
+ * 30-57): OrthographicCamera(xmag=1, ymag=1, znear 0.05, zfar 100) at create_pose_camera(-2), so pixel x =
+ * (x_view / xmag + 1) * 240 and y = (1 - y_view / ymag) * 360 (the aspect ratio is ignored: a 1.5x vertical stretch);
+ * DirectionalLight at create_pose_light(-30), direction toward the light l = (0, 0.5, 0.866); colour 220.
+ * A chunk holds `frames` frames of 2 views; view 0 is the left half.  Three launches per chunk:
+ *
+ * pm_mesh_vertex_f32: one thread per (frame, view, vertex).  View k reads verts_k + frame * vk_fs (V rows of xyz, the
+ *   body model's vertex buffer in place), applies p * scale_k + offset_k in fp32 (multiply, then add), then the view
+ *   transform and the projection in fp32, each operation rounded on its own.  Writes xy (frames, 2, V, 2) int32 = the
+ *   pixel coordinates * 256 rounded to nearest even (8 sub-pixel bits), or INT_MIN where a coordinate is not finite or
+ *   beyond the +-2^20-pixel guard band; depth (frames, 2, V) = -z_view fp32; normal (frames, 2, V, 3) fp32 = the
+ *   normalised sum (0 when it is 0) of cross(b - a, c - a) of the transformed corners over the incident faces, in
+ *   ascending face index: vf_ptr (V + 1) / vf_face, a CSR of the faces of each vertex.  faces (F, 3) int32.
+ * pm_mesh_raster: one thread per (frame, view, triangle).  A triangle with an INT_MIN corner or zero area is skipped;
+ *   one with negative area has corners 1 and 2 swapped (both sides are drawn).  Corner k's weight is the int64 edge
+ *   function of the edge from corner k+1 to k+2, w_k = dx (cy - y) - dy (cx - x), at pixel centres (p * 256 + 128);
+ *   a centre is covered when every w_k > 0, or w_k = 0 on a top-left edge (dy < 0, or dy = 0 and dx > 0).  The
+ *   bounding box is clamped to the viewport.  Depth = fp32(((w0 d0 + w1 d1) + w2 d2) / area2), fp64 and each operation
+ *   rounded; pixels outside [znear, zfar] are clipped.  atomicMin of (depth bits << 32 | triangle id) into vis
+ *   (frames, 2, 720, 480) uint64, which the caller clears to all ones (pm_memset_async 0xff): the nearest triangle wins,
+ *   ties to the lower id, whatever the execution order.
+ * pm_mesh_shade_u8: one thread per pixel of vis.  Background (all ones) is 0; otherwise the triangle's weights at the
+ *   pixel centre over area2 interpolate its corner normals, and value = rint(220 max(0, n.l / |n|)) is written to R, G
+ *   and B of out + frame * out_fs + (y * 960 + view * 480 + x) * 3 (out_fs >= 720 * 960 * 3 bytes). */
+int pm_mesh_vertex_f32(const float* verts0, long long v0_fs, const float* verts1, long long v1_fs,
+                       int n_verts, int frames, float scale0, float ox0, float oy0, float oz0,
+                       float scale1, float ox1, float oy1, float oz1, const int* faces,
+                       const int* vf_ptr, const int* vf_face, int* xy, float* depth, float* normal, void* stream);
+int pm_mesh_raster(const int* xy, const float* depth, int n_verts, const int* faces, int n_faces,
+                   int frames, unsigned long long* vis, void* stream);
+int pm_mesh_shade_u8(const unsigned long long* vis, const int* xy, const float* normal, int n_verts,
+                     const int* faces, int frames, unsigned char* out, long long out_fs, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -51,6 +51,9 @@ SIGNATURES = {
                         _p, _p, _p, _i, _p, _ll, _i, _i, _p],
     "pm_smplx_skin_f32": [_p, _ll, _ll, _i, _p, _p, _p, _p, _p, _ll, _ll, _i, _p],
     "pm_motion_rep_f32": [_p, _ll, _ll, _p, _i, _i, _f, _f, _p, _p],
+    "pm_mesh_vertex_f32": [_p, _ll, _p, _ll, _i, _i, _f, _f, _f, _f, _f, _f, _f, _f, _p, _p, _p, _p, _p, _p, _p],
+    "pm_mesh_raster": [_p, _p, _i, _p, _i, _i, _p, _p],
+    "pm_mesh_shade_u8": [_p, _p, _p, _i, _p, _i, _p, _ll, _p],
 }
 
 _lib = None

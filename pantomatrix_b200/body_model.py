@@ -177,13 +177,20 @@ class SmplxBodyModel:
             self._check(expression, "expression", (batch, t, N_EXPR))
         if transl is not None:
             self._check(transl, "transl", (batch, t, 3))
-        joints, rel, operand = self._fk(poses, betas, expression, transl, ALL_JOINTS, vertices)
-        out = {"joints": joints.view(batch, t, N_JOINTS, 3)}
-        if vertices:
-            buf = self._blend(operand, batch * t)
-            ops.smplx_skin(buf, self.n_verts, self.skin_csr, rel, transl, t)
-            out["vertices"] = buf[:, :3 * self.n_verts].view(batch, t, self.n_verts, 3)
-        return out
+        if not vertices:
+            joints, _, _ = self._fk(poses, betas, expression, transl, ALL_JOINTS, False)
+            return {"joints": joints.view(batch, t, N_JOINTS, 3)}
+        joints, verts = self._vertices(poses, betas, expression, transl, ALL_JOINTS)
+        return {"joints": joints.view(batch, t, N_JOINTS, 3), "vertices": verts}
+
+    def _vertices(self, poses, betas, expression, transl, mask):
+        """FK, vertex blend GEMM and skinning of validated inputs with the joints of `mask` posed: (joints (rows, 55,
+        3), vertices (B, T, V, 3) a view with rows 3V rounded up to 4 apart)."""
+        batch, t = poses.shape[:2]
+        joints, rel, operand = self._fk(poses, betas, expression, transl, mask, True)
+        buf = self._blend(operand, batch * t)
+        ops.smplx_skin(buf, self.n_verts, self.skin_csr, rel, transl, t)
+        return joints, buf[:, :3 * self.n_verts].view(batch, t, self.n_verts, 3)
 
     __call__ = forward
 

@@ -18,7 +18,7 @@ LIB = os.path.join(HERE, "libpm_emage.so")
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 # per-file extra flags
-EXTRA = {"pm_pose.cu": ["-fmad=false"]}
+EXTRA = {"pm_pose.cu": ["-fmad=false"], "pm_render.cu": ["-fmad=false"]}
 
 
 def _nvcc():

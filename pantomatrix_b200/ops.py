@@ -620,6 +620,44 @@ def motion_rep(poses, joints, dt, two_dt, out):
     return out
 
 
+# ------------------------------------------------------------------------------------------------------
+# SMPL-X mesh render
+# ------------------------------------------------------------------------------------------------------
+
+
+def mesh_vertex(verts, views, faces, vf_csr, xy, depth, normal):
+    """View transform, projection, snapping and vertex normals of a chunk (pm_mesh_vertex_f32).  verts: one (frames, V,
+    3) view per image view, frames any stride apart; views: ((scale, (ox, oy, oz)), ...) per image view.  Writes xy
+    (frames, 2, V, 2) int32, depth (frames, 2, V) and normal (frames, 2, V, 3)."""
+    for v in verts:
+        _chk(v)
+    _chk(xy, torch.int32), _chk(depth), _chk(normal), _chk(faces, torch.int32)
+    (v0, v1), ((s0, o0), (s1, o1)) = verts, views
+    vf_ptr, vf_face = vf_csr
+    _call("pm_mesh_vertex_f32", v0.data_ptr(), v0.stride(0), v1.data_ptr(), v1.stride(0), v0.shape[1], v0.shape[0],
+          float(s0), float(o0[0]), float(o0[1]), float(o0[2]), float(s1), float(o1[0]), float(o1[1]), float(o1[2]),
+          faces.data_ptr(), vf_ptr.data_ptr(),
+          vf_face.data_ptr(), xy.data_ptr(), depth.data_ptr(), normal.data_ptr(), _stream())
+
+
+def mesh_raster(xy, depth, faces, vis):
+    """Visibility keys of a chunk (pm_mesh_raster) into vis (frames, 2, 720, 480) int64, cleared here to all ones by a
+    memset (a memset node under graph capture)."""
+    _chk(xy, torch.int32), _chk(depth), _chk(faces, torch.int32), _chk(vis, torch.int64)
+    assert xy.is_contiguous() and depth.is_contiguous() and vis.is_contiguous()
+    _lib.call("pm_memset_async", vis.data_ptr(), 0xFF, vis.numel() * 8, _stream())
+    _call("pm_mesh_raster", xy.data_ptr(), depth.data_ptr(), xy.shape[2], faces.data_ptr(), faces.shape[0],
+          xy.shape[0], vis.data_ptr(), _stream())
+
+
+def mesh_shade(vis, xy, normal, faces, out):
+    """Shaded RGB of a chunk (pm_mesh_shade_u8) into out (frames, 720, 960, 3) uint8, frames any stride apart."""
+    _chk(vis, torch.int64), _chk(xy, torch.int32), _chk(normal), _chk(faces, torch.int32), _chk(out, torch.uint8)
+    assert out[0].is_contiguous() and normal.is_contiguous()
+    _call("pm_mesh_shade_u8", vis.data_ptr(), xy.data_ptr(), normal.data_ptr(), xy.shape[2], faces.data_ptr(),
+          vis.shape[0], out.data_ptr(), out.stride(0), _stream())
+
+
 def softmax2_mix(sel, c1, c2, out=None):
     """out[..., :] = softmax(sel[..., 0:2])[0] * c1 + [1] * c2 (out may be a column slice of a wider tensor)."""
     _chk(sel), _chk(c1), _chk(c2)

@@ -1,0 +1,121 @@
+"""SMPL-X mesh frames on the GPU: the reference demo's face and body views of generated poses.
+
+emage_utils/fast_render.py:286-321 render_one_sequence_with_face renders every frame of the SMPL-X mesh twice with
+pyrender and puts the views side by side: on the left a face close-up (only the jaw posed, the mesh scaled x7 and moved
+down by 10), on the right the full body.  This module draws the same scene with three kernels per chunk of frames
+(include/pm_emage.h pm_mesh_vertex_f32 / pm_mesh_raster / pm_mesh_shade_u8, DESIGN.md section 10):
+
+    renderer = MeshRenderer(SmplxBodyModel.from_npz("SMPLX_NEUTRAL_2020.npz"))
+    frames = renderer.render_sequence(pred["motion_axis_angle"], pred["expression"], pred["trans"])  # (B, T', 720, 960, 3)
+
+Geometry, framing, layout and frame count follow the reference; the shading is Lambert with its directional light (not
+pyrender's PBR shader, so pixel parity with pyrender is not claimed).  No host synchronisation: a call can be captured
+in a CUDA graph after one eager call.
+"""
+from __future__ import annotations
+
+import numpy as np
+import torch
+
+from . import ops
+from .body_model import ALL_JOINTS
+
+W, H, VIEWS = 480, 720, 2              # one view (fast_render.py args); output frames are VIEWS views side by side
+FPS = 30                               # render_video_fps: render_sequence draws whole seconds, T // 30 * 30 frames
+CHUNK = 8                              # frames per launch group: 8 x 2 visibility buffers of 2.8 MB stay in the 50 MB L2
+JAW_ONLY = 1 << 22                     # the face view poses the jaw alone (zeroed joints keep the hand means)
+FACE_VIEW = (7.0, (0.0, -10.0, 0.0))   # (scale, offset): v * 7 - (0, 10, 0), fast_render.py:312-315
+BODY_VIEW = (1.0, (0.0, 0.0, 0.0))
+
+
+class MeshRenderer:
+    """Renders the triangle list of an SmplxBodyModel (its model file's `f`).  Raises ValueError on malformed faces."""
+
+    def __init__(self, body_model):
+        nv, faces = body_model.n_verts, body_model.faces
+        if faces is None:
+            raise ValueError("SMPL-X model: no faces (key 'f') in the model file: nothing to render")
+        faces = np.asarray(faces)
+        if faces.ndim != 2 or faces.shape[1] != 3 or faces.shape[0] < 1:
+            raise ValueError(f"SMPL-X model: faces must be (F, 3), got {faces.shape}")
+        if faces.dtype.kind not in "iu":
+            raise ValueError(f"SMPL-X model: faces must be integer vertex indices, got {faces.dtype}")
+        if faces.min() < 0 or faces.max() >= nv:
+            raise ValueError(f"SMPL-X model: face indices must lie in [0, {nv}), got [{faces.min()}, {faces.max()}]")
+        faces = faces.astype(np.int64)
+        n_faces = faces.shape[0]
+        # vertex -> incident faces in ascending face index (each face once): the normal sum's fixed order
+        pairs = np.unique(faces * n_faces + np.arange(n_faces)[:, None])
+        vf_ptr = np.searchsorted(pairs // n_faces, np.arange(nv + 1))
+        dev = body_model.device
+        i32 = lambda x: torch.as_tensor(np.ascontiguousarray(x), dtype=torch.int32, device=dev)
+        self.body_model, self.n_verts, self.n_faces, self.device = body_model, nv, n_faces, dev
+        self.faces = i32(faces)
+        self.vf_csr = (i32(vf_ptr), i32(pairs % n_faces))
+
+    def _frames(self, v, name):
+        if not torch.is_tensor(v):
+            raise ValueError(f"{name} must be a tensor, got {type(v).__name__}")
+        if v.dim() == 4:
+            v = v.view(-1, *v.shape[2:])
+        if v.dim() != 3 or tuple(v.shape[1:]) != (self.n_verts, 3) or v.dtype != torch.float32:
+            raise ValueError(f"{name} must be (N, {self.n_verts}, 3) or (B, T, {self.n_verts}, 3) float32, got "
+                             f"{tuple(v.shape)} {v.dtype}")
+        if v.stride(2) != 1 or v.stride(1) != 3:
+            raise ValueError(f"{name}: each frame's vertices must be dense")
+        return v
+
+    @torch.no_grad()
+    def render(self, vertices, views=(FACE_VIEW, BODY_VIEW), out=None):
+        """Draw N frames of two views: vertices = (left, right), each (N, V, 3) or (B, T, V, 3) float32 CUDA with dense
+        frames any stride apart (body model output is read in place); views = ((scale, (ox, oy, oz)), ...) the affine
+        transform p * scale + offset of each view.  Returns out (N, 720, 960, 3) uint8 (each frame dense)."""
+        if len(vertices) != VIEWS or len(views) != VIEWS:
+            raise ValueError(f"render draws {VIEWS} views: give {VIEWS} vertex tensors and {VIEWS} transforms")
+        verts = [self._frames(v, f"vertices[{i}]") for i, v in enumerate(vertices)]
+        n = verts[0].shape[0]
+        if verts[1].shape[0] != n:
+            raise ValueError(f"the views have {n} and {verts[1].shape[0]} frames")
+        if out is None:
+            out = torch.empty(n, H, VIEWS * W, 3, dtype=torch.uint8, device=verts[0].device)
+        elif tuple(out.shape) != (n, H, VIEWS * W, 3) or out.dtype != torch.uint8 or (n and not out[0].is_contiguous()):
+            raise ValueError(f"out must be ({n}, {H}, {VIEWS * W}, 3) uint8 with dense frames")
+        c = min(n, CHUNK)
+        if c == 0:
+            return out
+        dev = verts[0].device
+        xy = torch.empty(c, VIEWS, self.n_verts, 2, dtype=torch.int32, device=dev)
+        depth = torch.empty(c, VIEWS, self.n_verts, device=dev)
+        normal = torch.empty(c, VIEWS, self.n_verts, 3, device=dev)
+        vis = torch.empty(c, VIEWS, H, W, dtype=torch.int64, device=dev)
+        for s in range(0, n, CHUNK):
+            k = min(CHUNK, n - s)
+            ops.mesh_vertex([v[s:s + k] for v in verts], views, self.faces, self.vf_csr, xy[:k], depth[:k], normal[:k])
+            ops.mesh_raster(xy[:k], depth[:k], self.faces, vis[:k])
+            ops.mesh_shade(vis[:k], xy[:k], normal[:k], self.faces, out[s:s + k])
+        return out
+
+    @torch.no_grad()
+    def render_sequence(self, poses, expression, trans, betas=None, out=None):
+        """render_one_sequence_with_face (fast_render.py:286-321) for clips of generated poses: poses (B, T, 165),
+        expression (B, T, 100), trans (B, T, 3), betas (B, 300) or None, float32 CUDA tensors as generate() /
+        CapturedPipeline return them (read in place).  Every frame uses frame 0's trans (remove_transl=True); the face
+        view poses only the jaw.  Returns out (B, T // 30 * 30, 720, 960, 3) uint8: face view left, body view right."""
+        bm = self.body_model
+        batch, t = bm._poses(poses)
+        bm._check(expression, "expression", (batch, t, 100))
+        bm._check(trans, "trans", (batch, t, 3))
+        if betas is not None:
+            bm._check(betas, "betas", (batch, 300))
+        n = t // FPS * FPS
+        if out is None:
+            out = torch.empty(batch, n, H, VIEWS * W, 3, dtype=torch.uint8, device=poses.device)
+        elif tuple(out.shape) != (batch, n, H, VIEWS * W, 3) or out.dtype != torch.uint8 or not out.is_contiguous():
+            raise ValueError(f"out must be a contiguous ({batch}, {n}, {H}, {VIEWS * W}, 3) uint8 tensor")
+        if n == 0:
+            return out
+        p, e, tr = poses[:, :n], expression[:, :n], trans[:, :1].expand(batch, n, 3)     # frame stride 0: frame 0's trans
+        _, body = bm._vertices(p, betas, e, tr, ALL_JOINTS)
+        _, face = bm._vertices(p, betas, e, tr, JAW_ONLY)
+        self.render((face, body), (FACE_VIEW, BODY_VIEW), out.view(batch * n, H, VIEWS * W, 3))
+        return out

@@ -54,6 +54,111 @@ def smplx_arrays(n_verts=SMPLX_FULL_VERTS, seed=0, parents=SMPLX_PARENTS):
     }
 
 
+# Rest offsets (metres, y up) of the 22 body joints from their parents, a rough standing figure: the surface model's
+# skeleton, so that its mesh is framed like a body by the render's camera.  Hand joints are laid out procedurally.
+_BODY_OFFSETS = {1: (0.06, -0.09, 0.0), 2: (-0.06, -0.09, 0.0), 3: (0.0, 0.11, -0.02), 4: (0.04, -0.38, 0.0),
+                 5: (-0.04, -0.38, 0.0), 6: (0.0, 0.13, 0.02), 7: (-0.01, -0.40, -0.04), 8: (0.01, -0.40, -0.04),
+                 9: (0.0, 0.05, 0.0), 10: (0.02, -0.06, 0.12), 11: (-0.02, -0.06, 0.12), 12: (0.0, 0.21, -0.02),
+                 13: (0.08, 0.12, -0.01), 14: (-0.08, 0.12, -0.01), 15: (0.0, 0.09, 0.05), 16: (0.11, 0.04, -0.01),
+                 17: (-0.11, 0.04, -0.01), 18: (0.26, -0.01, -0.02), 19: (-0.26, -0.01, -0.02), 20: (0.25, 0.01, 0.0),
+                 21: (-0.25, 0.01, 0.0), 22: (0.0, -0.01, 0.03), 23: (0.03, 0.06, 0.07), 24: (-0.03, 0.06, 0.07)}
+
+
+def _surface_joints(parents):
+    off = np.zeros((len(parents), 3))
+    for j, o in _BODY_OFFSETS.items():
+        off[j] = o
+    for j in range(25, len(parents)):                 # 5 fingers x 3 joints per hand, fanned out from the wrist
+        side = 1.0 if j < 40 else -1.0
+        finger, knuckle = divmod((j - 25) % 15, 3)
+        off[j] = (side * 0.03, 0.0, 0.035 - 0.02 * finger) if knuckle == 0 else (side * 0.025, 0.0, 0.0)
+    joints = np.zeros_like(off)
+    for j in range(1, len(parents)):
+        joints[j] = joints[parents[j]] + off[j]
+    return joints
+
+
+def _capsule(a, b, radius, n):
+    """A closed capsule around segment a -> b with at most n vertices (two poles and rings x segments) and its outward
+    triangles.  Returns (vertices, faces, which end each vertex belongs to (0 at a, 1 at b), the equator ring at a)."""
+    segs = max(range(6, 25), key=lambda s: (s * ((n - 2) // s), -abs(s - 12)))
+    rings = (n - 2) // segs
+    half = rings // 2                                  # rings [0, half) on the hemisphere at a, the rest at b
+    z = b - a
+    z = z / np.linalg.norm(z)
+    x = np.cross(z, [1.0, 0.0, 0.0] if abs(z[0]) < 0.9 else [0.0, 1.0, 0.0])
+    x /= np.linalg.norm(x)
+    y = np.cross(z, x)
+    phi = np.arange(segs) * 2 * np.pi / segs
+    circle = np.cos(phi)[:, None] * x + np.sin(phi)[:, None] * y
+    verts, end = [a - z * radius], [0.0]
+    for r in range(rings):
+        at_b = r >= half
+        polar = np.pi / 2 * ((r + 1) / half if not at_b else 1 + (r - half) / (rings - half))
+        verts += list((b if at_b else a) - z * radius * np.cos(polar) + radius * np.sin(polar) * circle)
+        end += [float(at_b)] * segs
+    verts.append(b + z * radius)
+    end.append(1.0)
+    top = len(verts) - 1
+    ring = lambda r, s: 1 + r * segs + s % segs
+    faces = []
+    for s in range(segs):
+        faces += [(0, ring(0, s + 1), ring(0, s)), (top, ring(rings - 1, s), ring(rings - 1, s + 1))]
+        for r in range(rings - 1):
+            faces += [(ring(r, s), ring(r + 1, s + 1), ring(r + 1, s)), (ring(r, s), ring(r, s + 1), ring(r + 1, s + 1))]
+    return np.array(verts), np.array(faces), np.array(end), [ring(half - 1, s) for s in range(segs)]
+
+
+def smplx_surface_arrays(n_verts=SMPLX_FULL_VERTS, seed=0, parents=SMPLX_PARENTS):
+    """A synthetic SMPL-X model with a real surface: the keys and shapes of smplx_arrays, but v_template is a closed
+    capsule around each of the 55 bones of a standing figure (joint j's capsule runs from j to its first child, or on
+    past j for a leaf), the vertices split evenly across the capsules (any remainder sits unreferenced at the joint), f
+    their outward-wound triangulation, J_regressor the mean of the capsule's equator ring at its joint, and each vertex
+    skinned to its capsule's joint, blended 30 % with the parent on the half at the joint.  The other arrays are drawn
+    as in smplx_arrays.  Closed meshes with body-like triangle sizes, for the render's tests and benchmark."""
+    rng = np.random.Generator(np.random.PCG64(seed))
+    nj = len(parents)
+    if n_verts < 16 * nj:
+        raise ValueError(f"smplx_surface_arrays needs at least {16 * nj} vertices")
+    joints = _surface_joints(parents)
+    children = {j: [c for c in range(nj) if parents[c] == j] for j in range(nj)}
+    v_template = np.zeros((n_verts, 3))
+    j_reg = np.zeros((nj, n_verts))
+    weights = np.zeros((n_verts, nj))
+    faces, start = [], 0
+    for j in range(nj):
+        n = n_verts // nj + (j < n_verts % nj)
+        a = joints[j]
+        if j == 15:                                    # the head: a ball above the neck rather than a tube to the jaw
+            b, radius = a + (0.0, 0.14, 0.01), 0.09
+        else:
+            if children[j]:
+                b = joints[children[j][0]]
+            else:
+                b = a + 0.5 * (a - joints[parents[j]])
+            radius = 0.12 if j == 0 else float(np.clip(0.3 * np.linalg.norm(b - a), 0.008, 0.09))
+        v, f, end, equator = _capsule(a, b, radius, n)
+        v_template[start:start + n] = a
+        v_template[start:start + len(v)] = v
+        faces.append(f + start)
+        j_reg[j, start + np.array(equator)] = 1.0 / len(equator)
+        weights[start:start + n, j] = 1.0
+        near = start + np.nonzero(end == 0.0)[0]
+        if parents[j] >= 0:
+            weights[near, j], weights[near, parents[j]] = 0.7, 0.3
+        start += n
+    decay = 1.0 / (1.0 + np.arange(400) / 50.0)
+    shapedirs = rng.standard_normal((n_verts, 3, 400)) * 1e-2 * decay
+    posedirs = rng.standard_normal((n_verts, 3, 486)) * 1e-2
+    kintree = np.stack([np.asarray(parents, dtype=np.int64), np.arange(nj, dtype=np.int64)])
+    return {
+        "v_template": v_template, "shapedirs": shapedirs.astype(np.float32), "posedirs": posedirs.astype(np.float32),
+        "J_regressor": j_reg, "weights": weights, "kintree_table": kintree,
+        "hands_meanl": rng.normal(0.0, 0.2, 45), "hands_meanr": rng.normal(0.0, 0.2, 45),
+        "f": np.concatenate(faces).astype(np.int32),
+    }
+
+
 def write_smplx_npz(path, n_verts=SMPLX_FULL_VERTS, seed=0):
     """Write smplx_arrays(...) as an SMPLX_NEUTRAL_2020.npz-format file; returns the arrays."""
     arrays = smplx_arrays(n_verts, seed)
