@@ -20,6 +20,11 @@
  *     planes instead of bf16 (same 2-byte storage).  Two fp16 planes carry 22 mantissa bits, so nsplit = 2
  *     (3 tensor-core products) gives the accuracy of 3 bf16 planes (6 products) - provided magnitudes stay below
  *     65504; an overflow becomes inf - inf = NaN in the consuming GEMM, which the host checks for.
+ *   - the split rule, the same in every producer: fp16 activation planes hold 64 x (exact pre-scale).  Each plane is
+ *     the running remainder rounded to nearest even (bf16: v = x; fp16: v = 64 x; plane p = RNE(v), v -= plane p),
+ *     except two fp16 activation planes: plane 0 = the head of v rounded half away from zero to 11 significant bits on
+ *     the fp32 bit pattern ((bits + 0x1000) & 0xFFFFE000), plane 1 = RNE(v - head).  The head is exact in fp16 for
+ *     |v| >= 2^-14; of the canonical NaN it is -0, and plane 1 carries the NaN.
  */
 #ifndef PM_EMAGE_H
 #define PM_EMAGE_H
@@ -77,7 +82,8 @@ int pm_tapgemm_tc(const uint16_t* A, long long a_ps, long long a_bs, int lda, in
                   uint16_t* out_bf16, long long ob_ps, long long ob_bs, int ldob, int out_nsplit,
                   const void* prefetch, long long prefetch_bytes, void* stream);
 
-/* fp32 (batch, rows, ch) -> nsplit bf16 planes (round-to-nearest hi, then residual planes). */
+/* fp32 (batch, rows, ch) -> nsplit bf16 or fp16 planes by the split rule above: each plane the running remainder
+ * rounded to nearest even; two fp16 planes take the half-away head of 64 x, then RNE(64 x - head). */
 int pm_split_bf16(const float* x, long long x_bs, int ldx, int batch, int rows, int ch,
                   uint16_t* out, long long o_ps, long long o_bs, int ldo, int nsplit, void* stream);
 

@@ -210,10 +210,13 @@ __global__ void __launch_bounds__(NTHREADS, 1) attention_tc_kernel(const __grid_
       if (frow) *reinterpret_cast<float2*>(frow + c) = make_float2(x0, x1);
       if (p.planes.ptr) {
         if (pair_ok) {
+          // the split of pm_store_planes_t: the half-away head only under a second plane, one plane is a0 rounded
+          // to nearest even (a head would round ties away and turn the canonical NaN into -0)
           const float a0 = x0 * PM_F16_ACT_SCALE, a1 = x1 * PM_F16_ACT_SCALE;
-          const float f0 = pm_f16_head(a0), f1 = pm_f16_head(a1);
+          const bool two = p.planes.nsplit > 1;
+          const float f0 = two ? pm_f16_head(a0) : a0, f1 = two ? pm_f16_head(a1) : a1;
           *reinterpret_cast<__half2*>(prow + c) = __floats2half2_rn(f0, f1);
-          if (p.planes.nsplit > 1) *reinterpret_cast<__half2*>(prow + p.planes.ps + c) = __floats2half2_rn(a0 - f0, a1 - f1);
+          if (two) *reinterpret_cast<__half2*>(prow + p.planes.ps + c) = __floats2half2_rn(a0 - f0, a1 - f1);
         } else {
           pm_store_planes_t<true>(p.planes, grow, h * HD + c, x0);
           pm_store_planes_t<true>(p.planes, grow, h * HD + c + 1, x1);

@@ -53,7 +53,8 @@ __device__ __forceinline__ float pm_warp_max(float v) {
   return v;
 }
 
-// ---- split-bf16 planes (operands of the tensor-core engine): x ~ p0 + p1 + p2, round-to-nearest each ----
+// ---- split planes (operands of the tensor-core engine): x ~ p0 + p1 + p2, each the running remainder rounded to
+// nearest even; two fp16 activation planes start from the half-away head of pm_f16_head instead (include/pm_emage.h) ----
 struct PmPlanes {
   __nv_bfloat16* ptr;   // plane 0, element (row 0, channel 0); nullptr = no plane output
   long long ps;         // plane stride (elements)
