@@ -10,12 +10,15 @@
 //   warpgroup 0      producer, 40 registers per thread (setmaxnreg.dec) -
 //                      warp 0: TMA (one elected lane): A box (64 ch x R rows x NB clips) per plane, with the tap shift
 //                              folded into the row coordinate (im2col-free; padding rows are TMA zero fill), W box
-//                              (64 ch x BN rows) per plane; 128B-swizzled K-major smem tiles; mbarrier ring
-//                      warp 1: L2 prefetch of the next GEMM's weights; warps 2-3 exit at once
+//                              (64 ch x BN rows) per plane; 128B-swizzled K-major smem tiles; mbarrier ring.
+//                              After the last k-block: the tile's fp32 residual (BN ch x R rows x NB clips) into
+//                              ring slots the remaining MMAs no longer read
+//                      warp 1: L2 prefetch of the next GEMM's weights; warp 2: the tile's bias into smem; warp 3
+//                              exits at once
 //   warpgroups 1-2   consumers, 232 registers per thread (setmaxnreg.inc) - consumer warpgroup g issues
 //                      wgmma.m64nBNk16 for tile rows 64 g .. 64 g + 63 out of the shared operand stage into three
 //                      BN / 2-register accumulators, then runs the epilogue: registers -> smem tile ->
-//                      bias / residual / activation -> coalesced fp32 store and/or split planes
+//                      bias / residual (both from smem) / activation -> coalesced fp32 store and/or split planes
 // Contract and reference call sites: include/pm_emage.h (pm_tapgemm_tc).
 #include <cuda.h>
 #include <stdio.h>
@@ -52,10 +55,12 @@ struct TcParams {
   int w_rows;                       // rows per tap in the packed weight tensor (>= cout, multiple of BN)
   const float* bias;
   const float* residual; long long r_bs; int ldr;
+  int res_tma;                      // residual tile loaded by TMA (map_r) into the ring; else read per element
   int act, act_cols; float slope;
   float* out_f32; long long o_bs; int ldo;
   __nv_bfloat16* out_bf16; long long ob_ps, ob_bs; int ldob; int out_nsplit;
   int stages;
+  int res_slot0, rot;               // residual tile's first physical ring slot; ring slot rotation (see the kernel)
   const uint8_t* prefetch; long long prefetch_bytes;   // next GEMM's weights: pulled into L2 while this one runs
   float acc_scale;   // fp16 operands: weights are packed scaled by a power of two, undone here (1 for bf16)
 };
@@ -112,19 +117,25 @@ __device__ __forceinline__ void mma_kblock(float (&main)[BN / 2], float (&corr)[
 template <int BN, bool F16, int NSPLIT>
 __global__ void __launch_bounds__(NUM_THREADS, 1) tapgemm_tc_kernel(const __grid_constant__ CUtensorMap map_a,
                                                                   const __grid_constant__ CUtensorMap map_w,
+                                                                  const __grid_constant__ CUtensorMap map_r,
                                                                   const TcParams p) {
   constexpr int W_TILE_BYTES = BN * BK * 2;
   constexpr int NACC = BN / 2;                      // accumulator registers per thread (m64 x BN over 128 threads)
   constexpr int ST = BN + 8;                        // epilogue staging row stride (floats)
+  constexpr int RES_BYTES = BM * BN * 4;            // fp32 residual tile, [NB clips][R rows][BN ch]
 
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  // carve: [stages][nsplit A tiles][nsplit W tiles] (1024-aligned), then barriers.  The epilogue reuses the ring.
+  // carve: [stages][nsplit A tiles][nsplit W tiles] (1024-aligned), then barriers, then the tile's BN bias values.
+  // The epilogue reuses the ring: the staging tile at its start, the residual tile in its last RES_BYTES (launch()
+  // checks that they do not overlap).
   uint8_t* tiles = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const int stage_bytes = p.nsplit * (A_TILE_BYTES + W_TILE_BYTES);
   const int ring_bytes = p.stages * stage_bytes > BM * ST * 4 ? p.stages * stage_bytes : BM * ST * 4;
   uint64_t* bars = reinterpret_cast<uint64_t*>(tiles + ring_bytes);
   uint64_t* full_bar = bars;                       // [MAX_STAGES]
   uint64_t* empty_bar = bars + MAX_STAGES;         // [MAX_STAGES]
+  uint64_t* epi_bar = bars + 2 * MAX_STAGES;       // bias (and residual tile) in smem
+  float* bias_s = reinterpret_cast<float*>(bars + 2 * MAX_STAGES + 2);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (warp == STAMP_WARP) PM_STAMP(0);                          // kernel entry
@@ -132,14 +143,19 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tapgemm_tc_kernel(const __grid
   const int n0 = blockIdx.y * BN;
   const int b0 = blockIdx.z * p.NB;
   const int n_iter = p.taps * p.kblocks;
+  // Ring slot s (barrier index) lives at physical slot (s + p.rot) % stages.  The residual tile takes the physical
+  // slots p.res_slot0 .. stages - 1; the rotation puts the last k-block just below them, so they hold the oldest
+  // k-blocks in flight and are handed back, and refilled with the residual, while the last k-blocks still compute.
 
   if (threadIdx.x == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_w) : "memory");
+    if (p.res_tma) asm volatile("prefetch.tensormap [%0];" ::"l"(&map_r) : "memory");
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(smem_u32(&full_bar[s]), 1);
       mbar_init(smem_u32(&empty_bar[s]), 2);       // one arrival per consumer warpgroup
     }
+    mbar_init(smem_u32(epi_bar), p.res_tma ? 2 : 1);   // warp 2's bias arrival (+ warp 0's residual transaction)
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
@@ -163,16 +179,21 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tapgemm_tc_kernel(const __grid
         asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(p.prefetch + off), "r"(n) : "memory");
       }
     }
+    if (warp == 2) {
+      for (int c = lane; c < BN; c += 32) bias_s[c] = p.bias && n0 + c < p.cout ? __ldg(p.bias + n0 + c) : 0.f;
+      __syncwarp();
+      if (lane == 0) mbar_arrive(smem_u32(epi_bar));
+    }
     if (warp != 0) return;
     // ----- warp 0: TMA -----
     const uint32_t tx = (uint32_t)stage_bytes;
-    int s = 0, tap = 0, kb = 0;
+    int s = 0, q = p.rot, tap = 0, kb = 0;
     uint32_t ph = 0;
     for (int it = 0; it < n_iter; ++it) {
       mbar_wait_fast(smem_u32(&empty_bar[s]), ph ^ 1u);       // whole warp waits (uniform control flow)
       if (elect_one()) {
         const uint32_t bar = smem_u32(&full_bar[s]);
-        uint8_t* st = tiles + (size_t)s * stage_bytes;
+        uint8_t* st = tiles + (size_t)q * stage_bytes;
         mbar_expect_tx(bar, tx);
         for (int pl = 0; pl < p.nsplit; ++pl) {
           tma_load_4d(smem_u32(st + pl * A_TILE_BYTES), &map_a, bar, kb * BK, l0 + tap - p.pad, b0, pl);
@@ -181,7 +202,22 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tapgemm_tc_kernel(const __grid
       }
       __syncwarp();
       if (++s == p.stages) { s = 0; ph ^= 1u; }
+      if (++q == p.stages) q = 0;
       if (++kb == p.kblocks) { kb = 0; ++tap; }
+    }
+    if (p.res_tma) {
+      // the next stages - res_slot0 ring slots are the residual's physical slots: once their k-blocks are consumed
+      // (or were never filled), load the residual tile over them
+      for (int j = p.res_slot0; j < p.stages; ++j) {
+        mbar_wait_fast(smem_u32(&empty_bar[s]), ph ^ 1u);
+        if (++s == p.stages) { s = 0; ph ^= 1u; }
+      }
+      if (elect_one()) {
+        const uint32_t bar = smem_u32(epi_bar);
+        mbar_expect_tx(bar, (uint32_t)RES_BYTES);
+        tma_load_3d(smem_u32(tiles + ring_bytes - RES_BYTES), &map_r, bar, n0, l0, b0);
+      }
+      __syncwarp();
     }
     return;                                        // the consumers' named barriers below do not count this warpgroup
   }
@@ -195,7 +231,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tapgemm_tc_kernel(const __grid
   for (int i = 0; i < NACC; ++i) { acc0[i] = 0.f; acc1[i] = 0.f; accc[i] = 0.f; }
   {
     const uint32_t tiles_u32 = smem_u32(tiles);
-    int s = 0;
+    int s = 0, q = p.rot;
     uint32_t ph = 0;
     int prev = -1;                                  // stage whose MMAs are still in flight
     // one k-block: the even ones accumulate into acc0, the odd ones into acc1 (unrolled by two, so that every wgmma
@@ -203,8 +239,8 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tapgemm_tc_kernel(const __grid
     auto kblock = [&](float (&main)[NACC]) {
       mbar_wait_fast(smem_u32(&full_bar[s]), ph);
       if (prev < 0 && warp == STAMP_WARP) PM_STAMP(2);            // first operand stage landed
-      const uint32_t a_base = tiles_u32 + (uint32_t)s * (uint32_t)stage_bytes + (uint32_t)wg * (64 * 128);
-      const uint32_t w_base = tiles_u32 + (uint32_t)s * (uint32_t)stage_bytes + (uint32_t)(NSPLIT * A_TILE_BYTES);
+      const uint32_t a_base = tiles_u32 + (uint32_t)q * (uint32_t)stage_bytes + (uint32_t)wg * (64 * 128);
+      const uint32_t w_base = tiles_u32 + (uint32_t)q * (uint32_t)stage_bytes + (uint32_t)(NSPLIT * A_TILE_BYTES);
       wgmma_fence();
       mma_kblock<BN, F16, NSPLIT>(main, accc, gmma_desc(GMMA_DESC_K_SW128, a_base), gmma_desc(GMMA_DESC_K_SW128, w_base));
       wgmma_commit();
@@ -213,6 +249,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tapgemm_tc_kernel(const __grid
       if (prev >= 0 && ct % 128 == 0) mbar_arrive(smem_u32(&empty_bar[prev]));
       prev = s;
       if (++s == p.stages) { s = 0; ph ^= 1u; }
+      if (++q == p.stages) q = 0;
     };
     int it = 0;
     for (; it + 1 < n_iter; it += 2) {
@@ -251,14 +288,18 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tapgemm_tc_kernel(const __grid
 
   // ===== epilogue: one float4 of one row per thread and round; consecutive threads cover a row (coalesced) =====
   const bool vec_f = p.out_f32 && ((p.ldo & 3) == 0) && ((reinterpret_cast<uintptr_t>(p.out_f32) & 15) == 0) && ((p.o_bs & 3) == 0);
-  const bool vec_r = p.residual && ((p.ldr & 3) == 0) && ((reinterpret_cast<uintptr_t>(p.residual) & 15) == 0) && ((p.r_bs & 3) == 0);
   const bool vec_b = p.out_bf16 && ((p.ldob & 3) == 0) && ((reinterpret_cast<uintptr_t>(p.out_bf16) & 7) == 0) &&
                      ((p.ob_bs & 3) == 0) && ((p.ob_ps & 3) == 0);
-  const bool all_vec = (!p.out_f32 || vec_f) && (!p.residual || vec_r) && (!p.out_bf16 || vec_b);
+  // the vector path reads the residual from the TMA-loaded tile; a residual TMA cannot describe is read per element
+  const bool all_vec = (!p.out_f32 || vec_f) && (!p.residual || p.res_tma) && (!p.out_bf16 || vec_b);
   const float act_slope = p.act == PM_ACT_NONE ? 1.f : (p.act == PM_ACT_RELU ? 0.f : p.slope);
   const int r_shift = 31 - __clz(p.R);                           // R is a power of two
   constexpr int C4 = BN / 4;                                     // float4 columns per row
   const float* stg = reinterpret_cast<const float*>(tiles);
+  const float* res_s = reinterpret_cast<const float*>(tiles + ring_bytes - RES_BYTES);
+  mbar_wait_fast(smem_u32(epi_bar), 0);                          // bias (and residual tile) landed
+  // Kept rolled: unrolled (all shared-memory reads first, then the stores) the EMAGE step ran at 294 k instead of
+  // 325 k frames/s (bench.py, H100 80GB HBM3 at 700 W): the larger kernel costs more than the overlap gains.
 #pragma unroll 1
   for (int item = ct; item < BM * C4; item += CONSUMER_THREADS) {
     const int rt = item / C4, c = (item % C4) * 4;
@@ -275,9 +316,12 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tapgemm_tc_kernel(const __grid
                      p.ob_ps, p.ldob, p.out_nsplit};
     if (all_vec && n + 4 <= p.cout) {
       float4 x = x4;
-      if (p.bias) { x.x += __ldg(p.bias + n); x.y += __ldg(p.bias + n + 1); x.z += __ldg(p.bias + n + 2); x.w += __ldg(p.bias + n + 3); }
+      if (p.bias) {
+        const float4 t = *reinterpret_cast<const float4*>(bias_s + c);
+        x.x += t.x; x.y += t.y; x.z += t.z; x.w += t.w;
+      }
       if (p.residual) {
-        const float4 t = *reinterpret_cast<const float4*>(p.residual + orr + n);
+        const float4 t = *reinterpret_cast<const float4*>(res_s + rt * BN + c);
         x.x += t.x; x.y += t.y; x.z += t.z; x.w += t.w;
       }
       x.x = x.x < 0.f ? (n < p.act_cols ? act_slope : 1.f) * x.x : x.x;
@@ -293,7 +337,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tapgemm_tc_kernel(const __grid
       for (int k = 0; k < 4; ++k) {
         if (n + k >= p.cout) break;
         float y = xs[k];
-        if (p.bias) y += __ldg(p.bias + n + k);
+        if (p.bias) y += bias_s[c + k];
         if (p.residual) y += p.residual[orr + n + k];
         y = y < 0.f ? (n + k < p.act_cols ? act_slope : 1.f) * y : y;
         if (p.out_f32) p.out_f32[of + n + k] = y;
@@ -339,34 +383,39 @@ __global__ void __launch_bounds__(256) split_bf16_kernel(const float* __restrict
 
 // ---------------------------------------------------------------------------------------------------
 template <int BN, bool F16, int NSPLIT>
-int launch(const CUtensorMap& ma, const CUtensorMap& mw, TcParams& p, dim3 grid, cudaStream_t st) {
-  const int stage_bytes = p.nsplit * (A_TILE_BYTES + BN * BK * 2);
-  int stages = RING_KB * 1024 / stage_bytes;
-  if (stages > MAX_STAGES) stages = MAX_STAGES;
-  if (stages < 2) return PM_EUNSUPPORTED;
+int launch(const CUtensorMap& ma, const CUtensorMap& mw, const CUtensorMap& mr, TcParams& p, dim3 grid, cudaStream_t st) {
+  constexpr int stage_bytes = NSPLIT * (A_TILE_BYTES + BN * BK * 2);
+  constexpr int stages = RING_KB * 1024 / stage_bytes < MAX_STAGES ? RING_KB * 1024 / stage_bytes : MAX_STAGES;
+  static_assert(stages >= 2, "the operand ring needs two stages");
+  // The epilogue's staging tile (ring start) and residual tile (ring end) must not overlap, and the residual must
+  // leave the slot below it to the last k-block.
+  constexpr int staging = BM * (BN + 8) * 4, res_bytes = BM * BN * 4;
+  static_assert(staging + res_bytes <= stages * stage_bytes && res_bytes <= (stages - 1) * stage_bytes,
+                "staging and residual tiles must fit the ring side by side");
   p.stages = stages;
-  const int staging = BM * (BN + 8) * 4;
-  const size_t ring = (size_t)stages * stage_bytes > (size_t)staging ? (size_t)stages * stage_bytes : (size_t)staging;
-  const size_t smem = ring + 1024 /*align slack*/ + 2 * MAX_STAGES * sizeof(uint64_t);
+  p.res_slot0 = (stages * stage_bytes - res_bytes) / stage_bytes;
+  p.rot = (p.res_slot0 - 1 - (p.taps * p.kblocks - 1) % stages + stages) % stages;
+  const size_t smem = (size_t)stages * stage_bytes + 1024 /*align slack*/ + (2 * MAX_STAGES + 2) * sizeof(uint64_t) + BN * sizeof(float);
   static unsigned long long configured = 0;       // per template instantiation, one bit per device
   if (pm_first_use_on_device(configured)) {
     cudaError_t e = cudaFuncSetAttribute(tapgemm_tc_kernel<BN, F16, NSPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     if (e != cudaSuccess) { configured = 0; return (int)e; }
   }
-  tapgemm_tc_kernel<BN, F16, NSPLIT><<<grid, NUM_THREADS, smem, st>>>(ma, mw, p);
+  tapgemm_tc_kernel<BN, F16, NSPLIT><<<grid, NUM_THREADS, smem, st>>>(ma, mw, mr, p);
   PM_LAUNCH_CHECK();
 }
 
 template <int BN>
-int launch_fmt(const CUtensorMap& ma, const CUtensorMap& mw, TcParams& p, dim3 grid, cudaStream_t st, bool f16) {
+int launch_fmt(const CUtensorMap& ma, const CUtensorMap& mw, const CUtensorMap& mr, TcParams& p, dim3 grid, cudaStream_t st,
+               bool f16) {
   if (f16) {
-    if (p.nsplit == 1) return launch<BN, true, 1>(ma, mw, p, grid, st);
-    if (p.nsplit == 2) return launch<BN, true, 2>(ma, mw, p, grid, st);
-    return launch<BN, true, 3>(ma, mw, p, grid, st);
+    if (p.nsplit == 1) return launch<BN, true, 1>(ma, mw, mr, p, grid, st);
+    if (p.nsplit == 2) return launch<BN, true, 2>(ma, mw, mr, p, grid, st);
+    return launch<BN, true, 3>(ma, mw, mr, p, grid, st);
   }
-  if (p.nsplit == 1) return launch<BN, false, 1>(ma, mw, p, grid, st);
-  if (p.nsplit == 2) return launch<BN, false, 2>(ma, mw, p, grid, st);
-  return launch<BN, false, 3>(ma, mw, p, grid, st);
+  if (p.nsplit == 1) return launch<BN, false, 1>(ma, mw, mr, p, grid, st);
+  if (p.nsplit == 2) return launch<BN, false, 2>(ma, mw, mr, p, grid, st);
+  return launch<BN, false, 3>(ma, mw, mr, p, grid, st);
 }
 
 // N tile of a launch: a pure function of the shape and the SM count, so a captured graph keeps its choice.
@@ -457,11 +506,24 @@ extern "C" int pm_tapgemm_tc(const uint16_t* A, long long a_ps, long long a_bs, 
     cuuint32_t box[3] = {(cuuint32_t)BK, (cuuint32_t)BNsel, 1};
     if (!encode_map(&mw, W, 3, dims, strides, box, f16)) return PM_EBADARG;
   }
+  // The residual tile by TMA where it can describe the view (16-byte base and strides); the box is the output tile,
+  // zero-filled past cout / rows_out / batch.  Any other view (or one the driver declines to encode) is read per
+  // element in the epilogue.
+  CUtensorMap mr;
+  std::memset(&mr, 0, sizeof(mr));
+  p.res_tma = residual && (reinterpret_cast<uintptr_t>(residual) & 15) == 0 && (ldr & 3) == 0 && (batch == 1 || (r_bs & 3) == 0);
+  if (p.res_tma) {
+    const long long bs_el = batch > 1 ? r_bs : (long long)rows_out * ldr;
+    cuuint64_t dims[3] = {(cuuint64_t)cout, (cuuint64_t)rows_out, (cuuint64_t)batch};
+    cuuint64_t strides[2] = {(cuuint64_t)ldr * 4, (cuuint64_t)bs_el * 4};
+    cuuint32_t box[3] = {(cuuint32_t)BNsel, (cuuint32_t)R, (cuuint32_t)NB};
+    p.res_tma = encode_tiled(&mr, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, CU_TENSOR_MAP_SWIZZLE_NONE, residual, 3, dims, strides, box);
+  }
   dim3 grid(pm_cdiv(rows_out, R), pm_cdiv(cout, BNsel), pm_cdiv(batch, NB));
   PM_REQUIRE(grid.z <= 65535 && grid.y <= 65535);
   const cudaStream_t st = (cudaStream_t)stream;
-  if (BNsel == 128) return launch_fmt<128>(ma, mw, p, grid, st, f16);
-  return launch_fmt<64>(ma, mw, p, grid, st, f16);
+  if (BNsel == 128) return launch_fmt<128>(ma, mw, mr, p, grid, st, f16);
+  return launch_fmt<64>(ma, mw, mr, p, grid, st, f16);
 }
 
 #ifdef PM_TC_TIMING

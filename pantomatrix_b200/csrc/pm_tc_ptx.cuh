@@ -185,7 +185,7 @@ __device__ __forceinline__ void wgmma_m64n256k16(float (&d)[128], uint64_t da, u
 #undef PM_D8
 
 // ---- host side: cuTensorMapEncodeTiled through the runtime's driver entry point (no -lcuda link dependency) ----
-// 2-byte elements (bf16 / fp16), 128-byte swizzle, zero fill out of bounds.
+// Zero fill out of bounds.  encode_map: 2-byte elements (bf16 / fp16), 128-byte swizzle (wgmma operands).
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -202,14 +202,19 @@ static inline EncodeTiledFn get_encode() {
   return fn;
 }
 
-static inline bool encode_map(CUtensorMap* m, const void* base, int rank, const cuuint64_t* dims, const cuuint64_t* strides_bytes,
-                const cuuint32_t* box, bool f16 = false) {
+static inline bool encode_tiled(CUtensorMap* m, CUtensorMapDataType type, CUtensorMapSwizzle swizzle, const void* base,
+                                int rank, const cuuint64_t* dims, const cuuint64_t* strides_bytes, const cuuint32_t* box) {
   EncodeTiledFn fn = get_encode();
   if (!fn) return false;
   cuuint32_t ones[5] = {1, 1, 1, 1, 1};
-  return fn(m, f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank,
-            const_cast<void*>(base), dims, strides_bytes, box, ones, CU_TENSOR_MAP_INTERLEAVE_NONE,
-            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+  return fn(m, type, (cuuint32_t)rank, const_cast<void*>(base), dims, strides_bytes, box, ones,
+            CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
+
+static inline bool encode_map(CUtensorMap* m, const void* base, int rank, const cuuint64_t* dims, const cuuint64_t* strides_bytes,
+                const cuuint32_t* box, bool f16 = false) {
+  return encode_tiled(m, f16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16,
+                      CU_TENSOR_MAP_SWIZZLE_128B, base, rank, dims, strides_bytes, box);
 }
 

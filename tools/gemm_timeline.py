@@ -19,13 +19,18 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 from pantomatrix_b200 import _lib, ops  # noqa: E402
 
-SHAPES = [  # name, batch, rows, cin, cout, taps, pad
-    ("lin 2048x768x64", 1, 2048, 64, 768, 1, 0),
-    ("lin 2048x768x768", 1, 2048, 768, 768, 1, 0),
-    ("lin 2048x768x3072", 1, 2048, 3072, 768, 1, 0),
-    ("lin 2048x2304x768", 1, 2048, 768, 2304, 1, 0),
-    ("conv k3 32x64 256->256", 32, 64, 256, 256, 3, 1),
-    ("conv k15 128x1241 64->64", 128, 1241, 64, 64, 15, 7),
+SHAPES = [  # name, batch, rows, cin, cout, taps, pad, fp32 residual
+    ("lin 2048x768x64", 1, 2048, 64, 768, 1, 0, False),
+    ("lin 2048x768x768", 1, 2048, 768, 768, 1, 0, False),
+    ("lin 2048x768x3072", 1, 2048, 3072, 768, 1, 0, False),
+    ("lin 2048x2304x768", 1, 2048, 768, 2304, 1, 0, False),
+    ("conv k3 32x64 256->256", 32, 64, 256, 256, 3, 1, False),
+    ("conv k15 128x1241 64->64", 128, 1241, 64, 64, 15, 7, False),
+    # with a residual, as the decoder layers' sa.out / ca.out / l2 and every WavEncoder conv2 run them
+    ("lin 2048x768x768 +res", 1, 2048, 768, 768, 1, 0, True),
+    ("lin 2048x768x1536 +res", 1, 2048, 1536, 768, 1, 0, True),
+    ("lin 2048x2304x768 +res", 1, 2048, 768, 2304, 1, 0, True),
+    ("conv k15 32x32638 64->64 +res", 32, 32638, 64, 64, 15, 7, True),   # WavEncoder block 0 conv2, 10 s clips
 ]
 NAMES = ["prologue", "first stage", "mma issued", "acc ready", "epilogue w2", "all done"]
 
@@ -42,7 +47,7 @@ def main():
     fp16 = len(sys.argv) > 2 and sys.argv[2] == "fp16"          # the default engine: two fp16 planes
     if fp16:
         ops.set_plane_format("fp16")
-    for name, b, rows, cin, cout, taps, pad in SHAPES:
+    for name, b, rows, cin, cout, taps, pad, with_res in SHAPES:
         if only and only not in name:
             continue
         g = torch.Generator().manual_seed(0)
@@ -50,10 +55,12 @@ def main():
         w = (torch.randn(taps, cout, cin, generator=g) / math.sqrt(cin * taps)).cuda()
         bias = torch.zeros(cout, device="cuda")
         rows_out = rows + 2 * pad - taps + 1
+        res = torch.randn(b, rows_out, cout, generator=g).cuda() if with_res else None
         for ns in ((2,) if fp16 else (1, 3)):
             a, pw = ops.split_bf16(x, ns), ops.PackedW(w, ns)
             for out_mode in ("f32", "f+p", "p"):
-                kw = dict(rows_out=rows_out, pad=pad, act=ops.ACT_RELU, out_nsplit=0 if out_mode == "f32" else ns)
+                kw = dict(rows_out=rows_out, pad=pad, act=ops.ACT_RELU, residual=res,
+                          out_nsplit=0 if out_mode == "f32" else ns)
                 if out_mode == "p":
                     kw["want_f32"] = False
                 else:
