@@ -3,10 +3,15 @@
 
     python examples/camn_disco_demo.py --model camn --checkpoint /path/to/camn_audio --audio_folder ./wavs
     python examples/camn_disco_demo.py --model disco --synthetic --audio_folder ./wavs
+    python examples/camn_disco_demo.py ... --smplx SMPLX_NEUTRAL_2020.npz --render   # + <name>_frames/frame_%05d.png
 
 These models emit the upper body + hands only and no translation; like the reference demos the npz writer places the
 pelvis with the SMPL-X body model: pass the model file with --smplx SMPLX_NEUTRAL_2020.npz (the translation the
-reference writer derives), or --trans-zero to write zeros instead."""
+reference writer derives), or --trans-zero to write zeros instead.
+`--render` (needs --smplx) draws the reference demos' SMPL-X body view (fast_render.py render_one_sequence_no_gt: one
+480 x 720 view, whole seconds at 30 fps) of the motion upsampled to 30 fps as the npz stores it, on the GPU, with the
+translation the npz receives, and writes the frames as PNG files with Pillow next to each npz; video encoding is left to
+the user (e.g. ffmpeg -framerate 30 -i frame_%05d.png)."""
 import argparse
 import os
 import sys
@@ -21,7 +26,15 @@ sys.path.insert(0, ROOT)
 from models.camn_audio import CamnAudioModel  # noqa: E402
 from models.disco_audio import DiscoAudioModel  # noqa: E402
 from pantomatrix_b200.audio_io import load_audio  # noqa: E402
-from pantomatrix_b200.motion_io import beat_format_save  # noqa: E402
+from pantomatrix_b200.motion_io import beat_format_save, pelvis_translation  # noqa: E402
+
+
+def write_frames(frames, folder):
+    """(N, 720, 480, 3) uint8 frames -> folder/frame_%05d.png."""
+    from PIL import Image
+    os.makedirs(folder, exist_ok=True)
+    for i, img in enumerate(frames.cpu().numpy()):
+        Image.fromarray(img).save(os.path.join(folder, f"frame_{i:05d}.png"))
 
 
 def main():
@@ -33,14 +46,21 @@ def main():
     ap.add_argument("--synthetic", action="store_true")
     ap.add_argument("--trans-zero", action="store_true")
     ap.add_argument("--smplx", default=None, metavar="PATH", help="SMPL-X model file (SMPLX_NEUTRAL_2020.npz)")
+    ap.add_argument("--render", action="store_true")
     args = ap.parse_args()
     if not args.trans_zero and args.smplx is None:
         ap.error("the npz needs a pelvis translation: pass --smplx SMPLX_NEUTRAL_2020.npz, or --trans-zero to write zeros")
+    if args.render and args.smplx is None:
+        ap.error("--render needs --smplx SMPLX_NEUTRAL_2020.npz")
     device = torch.device("cuda")
-    body_model = None
-    if args.smplx is not None and not args.trans_zero:
+    body_model = renderer = None
+    if args.smplx is not None:
         from pantomatrix_b200.body_model import SmplxBodyModel
-        body_model = SmplxBodyModel.from_npz(args.smplx, device)
+        smplx_model = SmplxBodyModel.from_npz(args.smplx, device)
+        body_model = None if args.trans_zero else smplx_model
+        if args.render:
+            from pantomatrix_b200.render import MeshRenderer
+            renderer = MeshRenderer(smplx_model)
     if args.synthetic:
         sys.path.insert(0, os.path.join(ROOT, "tests"))
         from synthetic_models import build_lstm_product
@@ -56,8 +76,14 @@ def main():
         aa = model(audio, torch.zeros(1, 1, dtype=torch.long, device=device), seed_frames=seed_frames)["motion_axis_angle"]
         t = aa.shape[1]
         trans = None if body_model is not None else np.zeros((t, 3), dtype=np.float32)
-        beat_format_save(os.path.join(args.save_folder, os.path.splitext(name)[0] + "_output.npz"),
-                         aa.cpu().numpy().reshape(t, -1), upsample=30 // fps, trans=trans, body_model=body_model)
+        npz = os.path.join(args.save_folder, os.path.splitext(name)[0] + "_output.npz")
+        beat_format_save(npz, aa.cpu().numpy().reshape(t, -1), upsample=30 // fps, trans=trans, body_model=body_model)
+        if renderer is not None:
+            # the npz's translation: the writer's pelvis placement (betas zero), or zeros under --trans-zero
+            pelvis = np.zeros(3, np.float32) if trans is not None else pelvis_translation(body_model, np.zeros(300, np.float32))
+            tr = torch.as_tensor(pelvis, device=device).expand(1, t, 3)
+            write_frames(renderer.render_body(aa.reshape(1, t, -1), tr, upsample=30 // fps)[0],
+                         os.path.splitext(npz)[0] + "_frames")
         frames += t
     print(f"generate total {frames / fps:.2f} seconds motion in {time.time() - t0:.2f} seconds, saved in {args.save_folder}")
 

@@ -306,6 +306,29 @@ int pm_mesh_raster(const int* xy, const float* depth, int n_verts, const int* fa
                    int frames, unsigned long long* vis, void* stream);
 int pm_mesh_shade_u8(const unsigned long long* vis, const int* xy, const float* normal, int n_verts,
                      const int* faces, int frames, unsigned char* out, long long out_fs, void* stream);
+/* The same three stages with `views` (1 or 2) image views per frame; with 2 they are the entry points above, bit for
+ * bit.  With 1 (render_one_sequence_no_gt: one 480 x 720 body view), verts1 / v1_fs and the second transform are not
+ * read (verts1 may be NULL); xy, depth, normal and vis are (frames, 1, ...) and the output frame is 480 wide:
+ * out + frame * out_fs + (y * 480 + x) * 3, out_fs >= 720 * 480 * 3 bytes.  In general the frame is views * 480 wide
+ * and view k is its k-th 480-column block. */
+int pm_mesh_vertex_views_f32(const float* verts0, long long v0_fs, const float* verts1, long long v1_fs,
+                             int n_verts, int frames, float scale0, float ox0, float oy0, float oz0,
+                             float scale1, float ox1, float oy1, float oz1, const int* faces,
+                             const int* vf_ptr, const int* vf_face, int* xy, float* depth, float* normal,
+                             int views, void* stream);
+int pm_mesh_raster_views(const int* xy, const float* depth, int n_verts, const int* faces, int n_faces,
+                         int frames, unsigned long long* vis, int views, void* stream);
+int pm_mesh_shade_views_u8(const unsigned long long* vis, const int* xy, const float* normal, int n_verts,
+                           const int* faces, int frames, unsigned char* out, long long out_fs, int views,
+                           void* stream);
+/* pm_time_upsample_f32: motion_io.time_upsample_numpy (the npz writer's upsample=30 // pose_fps) as the renderer reads
+ * its output back, float32.  x (batch, t, channels) with clip / frame strides x_bs / x_ts and a dense last dimension ->
+ * out (batch, k t, channels) dense.  k = 1 copies.  Otherwise, with n = k t, output frame j sits at
+ * pos = j * step, step = (t-1) / (n-1) in fp64 (numpy's linspace; pos = t-1 exactly for j = n-1, 0 for every j when
+ * t = 1), lo = clamp(floor(pos), 0, max(t-2, 0)), frac = pos - lo, a = x[lo], b = x[min(lo+1, t-1)], d = fp32(b - a)
+ * and out = fp32(double(a) + double(d) * frac), each operation rounded on its own. */
+int pm_time_upsample_f32(const float* x, long long x_bs, long long x_ts, int batch, int t, int channels, int k,
+                         float* out, void* stream);
 
 #ifdef __cplusplus
 }

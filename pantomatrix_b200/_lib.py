@@ -54,6 +54,11 @@ SIGNATURES = {
     "pm_mesh_vertex_f32": [_p, _ll, _p, _ll, _i, _i, _f, _f, _f, _f, _f, _f, _f, _f, _p, _p, _p, _p, _p, _p, _p],
     "pm_mesh_raster": [_p, _p, _i, _p, _i, _i, _p, _p],
     "pm_mesh_shade_u8": [_p, _p, _p, _i, _p, _i, _p, _ll, _p],
+    "pm_mesh_vertex_views_f32": [_p, _ll, _p, _ll, _i, _i, _f, _f, _f, _f, _f, _f, _f, _f, _p, _p, _p, _p, _p, _p, _i,
+                                 _p],
+    "pm_mesh_raster_views": [_p, _p, _i, _p, _i, _i, _p, _i, _p],
+    "pm_mesh_shade_views_u8": [_p, _p, _p, _i, _p, _i, _p, _ll, _i, _p],
+    "pm_time_upsample_f32": [_p, _ll, _ll, _i, _i, _i, _i, _p, _p],
 }
 
 _lib = None

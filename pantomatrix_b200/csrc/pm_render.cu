@@ -1,9 +1,11 @@
-// SMPL-X mesh render (pantomatrix_b200/render.py): the two-view frame of emage_utils/fast_render.py
-// render_one_sequence_with_face, three launches per chunk of frames: pm_mesh_vertex_f32 (view transform, projection,
-// snapping, vertex normals), pm_mesh_raster (visibility keys by atomicMin) and pm_mesh_shade_u8 (Lambert shading into
-// the side-by-side RGB frame).  Contracts and the exact rules: include/pm_emage.h; CPU restatement:
-// oracle/render_oracle.py.  Built with -fmad=false: every fp32 / fp64 product and sum is rounded on its own, so the
-// restatement reproduces the snapped coordinates and depths operation by operation.
+// SMPL-X mesh render (pantomatrix_b200/render.py): the frames of emage_utils/fast_render.py, one view per frame
+// (render_one_sequence_no_gt) or two side by side (render_one_sequence_with_face, render_one_sequence).  Three launches
+// per chunk of frames: pm_mesh_vertex_f32 (view transform, projection, snapping, vertex normals), pm_mesh_raster
+// (visibility keys by atomicMin) and pm_mesh_shade_u8 (Lambert shading into the RGB frame), each a two-view entry point
+// and a *_views one that takes the view count; plus pm_time_upsample_f32, the piecewise-linear frame-rate upsampling of
+// the npz writer.  Contracts and the exact rules: include/pm_emage.h; CPU restatement: oracle/render_oracle.py.  Built
+// with -fmad=false: every fp32 / fp64 product and sum is rounded on its own, so the restatement reproduces the snapped
+// coordinates and depths operation by operation.
 #include <limits.h>
 #include <math.h>
 
@@ -12,9 +14,7 @@
 
 namespace {
 
-constexpr int VIEWS = 2;                  // face close-up (left), body (right)
 constexpr int W = 480, H = 720;           // one view (fast_render.py args, OffscreenRenderer(480, 720))
-constexpr int OUT_W = VIEWS * W;
 constexpr int SUB = 256;                  // 8 sub-pixel bits
 constexpr float GUARD = 1048576.f;        // 2^20 pixels: |snapped| < 2^28, edge products < 2^59 fit int64
 constexpr int BAD = INT_MIN;              // snapped x of a vertex that no triangle may use
@@ -44,6 +44,8 @@ __device__ __forceinline__ unsigned char shade(float nx, float ny, float nz) {
   return (unsigned char)min(255, __float2int_rn(COLOR * fmaxf(0.f, d)));
 }
 
+// NV views per frame (1 or 2): view k of frame f is image view k, read from verts_k.
+template <int NV>
 __global__ void __launch_bounds__(256) mesh_vertex_kernel(const float* __restrict__ v0, long long v0_fs,
                                                           const float* __restrict__ v1, long long v1_fs, int nv,
                                                           long long total, const ViewXf xf,
@@ -51,11 +53,12 @@ __global__ void __launch_bounds__(256) mesh_vertex_kernel(const float* __restric
                                                           const int* __restrict__ vf_ptr,
                                                           const int* __restrict__ vf_face, int2* __restrict__ xy,
                                                           float* __restrict__ depth, float* __restrict__ normal) {
+  static_assert(NV == 1 || NV == 2, "one or two views per frame");
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= total) return;
   const long long fv = i / nv;
-  const int v = (int)(i % nv), view = (int)(fv & 1);
-  const long long f = fv >> 1;
+  const int v = (int)(i % nv), view = (int)(fv & (NV - 1));
+  const long long f = fv >> (NV - 1);
   const float* base = view ? v1 + f * v1_fs : v0 + f * v0_fs;
   const float s = view ? xf.s1 : xf.s0, ox = view ? xf.ox1 : xf.ox0, oy = view ? xf.oy1 : xf.oy0,
               oz = view ? xf.oz1 : xf.oz0;
@@ -169,16 +172,18 @@ __global__ void __launch_bounds__(256) mesh_raster_kernel(const int2* __restrict
   }
 }
 
+template <int NV>
 __global__ void __launch_bounds__(256) mesh_shade_kernel(const unsigned long long* __restrict__ vis,
                                                          const int2* __restrict__ xy,
                                                          const float* __restrict__ normal, int nv,
                                                          const int* __restrict__ faces, long long total,
                                                          unsigned char* __restrict__ out, long long out_fs) {
+  static_assert(NV == 1 || NV == 2, "one or two views per frame");
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= total) return;
   const long long fv = i / (W * H);
-  const int pix = (int)(i % (W * H)), py = pix / W, px = pix % W, view = (int)(fv & 1);
-  unsigned char* dst = out + (fv >> 1) * out_fs + ((long long)py * OUT_W + view * W + px) * 3;
+  const int pix = (int)(i % (W * H)), py = pix / W, px = pix % W, view = (int)(fv & (NV - 1));
+  unsigned char* dst = out + (fv >> (NV - 1)) * out_fs + ((long long)py * (NV * W) + view * W + px) * 3;
   const unsigned long long key = vis[i];
   unsigned char c = 0;
   if (key != ~0ull) {
@@ -198,7 +203,71 @@ __global__ void __launch_bounds__(256) mesh_shade_kernel(const unsigned long lon
   dst[0] = c; dst[1] = c; dst[2] = c;
 }
 
+// out[b, j, c] = fp32(a + d * frac) of the two source frames around position pos_j = j * ((t-1) / (k t - 1)) (the
+// last one t-1 exactly), as numpy's linspace and motion_io.time_upsample_numpy compute it in fp64; k = 1 copies.
+__global__ void __launch_bounds__(256) time_upsample_kernel(const float* __restrict__ x, long long x_bs, long long x_ts,
+                                                            int t, int ch, int k, long long total,
+                                                            float* __restrict__ out) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= total) return;
+  const int c = (int)(i % ch);
+  const long long row = i / ch;
+  const int n = k * t, j = (int)(row % n);
+  const float* src = x + (row / n) * x_bs + c;
+  if (k == 1) {
+    out[i] = src[(long long)j * x_ts];
+    return;
+  }
+  // linspace(0, t-1, n): i * step with step = (t-1) / (n-1); step = 0 (t = 1) gives 0 everywhere
+  const double step = __ddiv_rn((double)(t - 1), (double)(n - 1));
+  const double pos = j == n - 1 ? (double)(t - 1) : __dmul_rn((double)j, step);
+  const int lo = min(max((int)floor(pos), 0), max(t - 2, 0));
+  const double frac = __dsub_rn(pos, (double)lo);
+  const float a = src[(long long)lo * x_ts], b = src[(long long)min(lo + 1, t - 1) * x_ts];
+  out[i] = __double2float_rn(__dadd_rn((double)a, __dmul_rn((double)__fsub_rn(b, a), frac)));
+}
+
 inline unsigned blocks(long long n) { return (unsigned)((n + 255) / 256); }
+
+int launch_vertex(int views, const float* verts0, long long v0_fs, const float* verts1, long long v1_fs, int n_verts,
+                  int frames, const ViewXf& xf, const int* faces, const int* vf_ptr, const int* vf_face, int* xy,
+                  float* depth, float* normal, void* stream) {
+  PM_REQUIRE(views == 1 || views == 2);
+  PM_REQUIRE(verts0 && (views == 1 || verts1) && faces && vf_ptr && vf_face && xy && depth && normal);
+  PM_REQUIRE(n_verts > 0 && frames >= 0 && v0_fs >= 3LL * n_verts && (views == 1 || v1_fs >= 3LL * n_verts));
+  const long long total = (long long)frames * views * n_verts;
+  if (total == 0) return PM_OK;
+  PM_REQUIRE(total / 256 < 0x7fffffffLL);
+  auto kernel = views == 2 ? mesh_vertex_kernel<2> : mesh_vertex_kernel<1>;
+  kernel<<<blocks(total), 256, 0, (cudaStream_t)stream>>>(verts0, v0_fs, verts1, v1_fs, n_verts, total, xf, faces,
+                                                          vf_ptr, vf_face, reinterpret_cast<int2*>(xy), depth, normal);
+  PM_LAUNCH_CHECK();
+}
+
+int launch_raster(int views, const int* xy, const float* depth, int n_verts, const int* faces, int n_faces, int frames,
+                  unsigned long long* vis, void* stream) {
+  PM_REQUIRE(views == 1 || views == 2);
+  PM_REQUIRE(xy && depth && faces && vis && n_verts > 0 && n_faces >= 0 && frames >= 0);
+  // the raster does not depend on the layout: one image per (frame, view)
+  const long long total = (long long)frames * views * n_faces;
+  if (total == 0) return PM_OK;
+  PM_REQUIRE(total / 256 < 0x7fffffffLL);
+  mesh_raster_kernel<<<blocks(total), 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<const int2*>(xy), depth,
+                                                                       n_verts, faces, n_faces, total, vis);
+  PM_LAUNCH_CHECK();
+}
+
+int launch_shade(int views, const unsigned long long* vis, const int* xy, const float* normal, int n_verts,
+                 const int* faces, int frames, unsigned char* out, long long out_fs, void* stream) {
+  PM_REQUIRE(views == 1 || views == 2);
+  PM_REQUIRE(vis && xy && normal && faces && out && n_verts > 0 && frames >= 0 && out_fs >= 3LL * views * W * H);
+  const long long total = (long long)frames * views * W * H;
+  if (total == 0) return PM_OK;
+  auto kernel = views == 2 ? mesh_shade_kernel<2> : mesh_shade_kernel<1>;
+  kernel<<<blocks(total), 256, 0, (cudaStream_t)stream>>>(vis, reinterpret_cast<const int2*>(xy), normal, n_verts,
+                                                          faces, total, out, out_fs);
+  PM_LAUNCH_CHECK();
+}
 
 }  // namespace
 
@@ -207,34 +276,49 @@ extern "C" int pm_mesh_vertex_f32(const float* verts0, long long v0_fs, const fl
                                   float scale1, float ox1, float oy1, float oz1, const int* faces,
                                   const int* vf_ptr, const int* vf_face, int* xy, float* depth, float* normal,
                                   void* stream) {
-  PM_REQUIRE(verts0 && verts1 && faces && vf_ptr && vf_face && xy && depth && normal);
-  PM_REQUIRE(n_verts > 0 && frames >= 0 && v0_fs >= 3LL * n_verts && v1_fs >= 3LL * n_verts);
-  const long long total = (long long)frames * VIEWS * n_verts;
-  if (total == 0) return PM_OK;
-  PM_REQUIRE(total / 256 < 0x7fffffffLL);
-  mesh_vertex_kernel<<<blocks(total), 256, 0, (cudaStream_t)stream>>>(
-      verts0, v0_fs, verts1, v1_fs, n_verts, total, ViewXf{scale0, ox0, oy0, oz0, scale1, ox1, oy1, oz1}, faces,
-      vf_ptr, vf_face, reinterpret_cast<int2*>(xy), depth, normal);
-  PM_LAUNCH_CHECK();
+  return launch_vertex(2, verts0, v0_fs, verts1, v1_fs, n_verts, frames,
+                       ViewXf{scale0, ox0, oy0, oz0, scale1, ox1, oy1, oz1}, faces, vf_ptr, vf_face, xy, depth, normal,
+                       stream);
 }
 
 extern "C" int pm_mesh_raster(const int* xy, const float* depth, int n_verts, const int* faces, int n_faces,
                               int frames, unsigned long long* vis, void* stream) {
-  PM_REQUIRE(xy && depth && faces && vis && n_verts > 0 && n_faces >= 0 && frames >= 0);
-  const long long total = (long long)frames * VIEWS * n_faces;
-  if (total == 0) return PM_OK;
-  PM_REQUIRE(total / 256 < 0x7fffffffLL);
-  mesh_raster_kernel<<<blocks(total), 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<const int2*>(xy), depth,
-                                                                       n_verts, faces, n_faces, total, vis);
-  PM_LAUNCH_CHECK();
+  return launch_raster(2, xy, depth, n_verts, faces, n_faces, frames, vis, stream);
 }
 
 extern "C" int pm_mesh_shade_u8(const unsigned long long* vis, const int* xy, const float* normal, int n_verts,
                                 const int* faces, int frames, unsigned char* out, long long out_fs, void* stream) {
-  PM_REQUIRE(vis && xy && normal && faces && out && n_verts > 0 && frames >= 0 && out_fs >= 3LL * OUT_W * H);
-  const long long total = (long long)frames * VIEWS * W * H;
+  return launch_shade(2, vis, xy, normal, n_verts, faces, frames, out, out_fs, stream);
+}
+
+extern "C" int pm_mesh_vertex_views_f32(const float* verts0, long long v0_fs, const float* verts1, long long v1_fs,
+                                        int n_verts, int frames, float scale0, float ox0, float oy0, float oz0,
+                                        float scale1, float ox1, float oy1, float oz1, const int* faces,
+                                        const int* vf_ptr, const int* vf_face, int* xy, float* depth, float* normal,
+                                        int views, void* stream) {
+  return launch_vertex(views, verts0, v0_fs, verts1, v1_fs, n_verts, frames,
+                       ViewXf{scale0, ox0, oy0, oz0, scale1, ox1, oy1, oz1}, faces, vf_ptr, vf_face, xy, depth, normal,
+                       stream);
+}
+
+extern "C" int pm_mesh_raster_views(const int* xy, const float* depth, int n_verts, const int* faces, int n_faces,
+                                    int frames, unsigned long long* vis, int views, void* stream) {
+  return launch_raster(views, xy, depth, n_verts, faces, n_faces, frames, vis, stream);
+}
+
+extern "C" int pm_mesh_shade_views_u8(const unsigned long long* vis, const int* xy, const float* normal, int n_verts,
+                                      const int* faces, int frames, unsigned char* out, long long out_fs, int views,
+                                      void* stream) {
+  return launch_shade(views, vis, xy, normal, n_verts, faces, frames, out, out_fs, stream);
+}
+
+extern "C" int pm_time_upsample_f32(const float* x, long long x_bs, long long x_ts, int batch, int t, int channels,
+                                    int k, float* out, void* stream) {
+  PM_REQUIRE(x && out && batch >= 0 && t > 0 && channels > 0 && k >= 1);
+  PM_REQUIRE((long long)k * t <= 0x7fffffffLL);
+  const long long total = (long long)batch * k * t * channels;
   if (total == 0) return PM_OK;
-  mesh_shade_kernel<<<blocks(total), 256, 0, (cudaStream_t)stream>>>(vis, reinterpret_cast<const int2*>(xy), normal,
-                                                                      n_verts, faces, total, out, out_fs);
+  PM_REQUIRE(total / 256 < 0x7fffffffLL);
+  time_upsample_kernel<<<blocks(total), 256, 0, (cudaStream_t)stream>>>(x, x_bs, x_ts, t, channels, k, total, out);
   PM_LAUNCH_CHECK();
 }

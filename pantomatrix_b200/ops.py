@@ -628,7 +628,10 @@ def motion_rep(poses, joints, dt, two_dt, out):
 def mesh_vertex(verts, views, faces, vf_csr, xy, depth, normal):
     """View transform, projection, snapping and vertex normals of a chunk (pm_mesh_vertex_f32).  verts: one (frames, V,
     3) view per image view, frames any stride apart; views: ((scale, (ox, oy, oz)), ...) per image view.  Writes xy
-    (frames, 2, V, 2) int32, depth (frames, 2, V) and normal (frames, 2, V, 3)."""
+    (frames, 2, V, 2) int32, depth (frames, 2, V) and normal (frames, 2, V, 3).  Buffers of one view, (frames, 1, ...),
+    take the single-view path (mesh_vertex_views)."""
+    if xy.shape[1] != 2:
+        return mesh_vertex_views(verts, views, faces, vf_csr, xy, depth, normal)
     for v in verts:
         _chk(v)
     _chk(xy, torch.int32), _chk(depth), _chk(normal), _chk(faces, torch.int32)
@@ -642,7 +645,9 @@ def mesh_vertex(verts, views, faces, vf_csr, xy, depth, normal):
 
 def mesh_raster(xy, depth, faces, vis):
     """Visibility keys of a chunk (pm_mesh_raster) into vis (frames, 2, 720, 480) int64, cleared here to all ones by a
-    memset (a memset node under graph capture)."""
+    memset (a memset node under graph capture).  (frames, 1, ...) buffers take the single-view path."""
+    if xy.shape[1] != 2:
+        return mesh_raster_views(xy, depth, faces, vis)
     _chk(xy, torch.int32), _chk(depth), _chk(faces, torch.int32), _chk(vis, torch.int64)
     assert xy.is_contiguous() and depth.is_contiguous() and vis.is_contiguous()
     _lib.call("pm_memset_async", vis.data_ptr(), 0xFF, vis.numel() * 8, _stream())
@@ -651,11 +656,64 @@ def mesh_raster(xy, depth, faces, vis):
 
 
 def mesh_shade(vis, xy, normal, faces, out):
-    """Shaded RGB of a chunk (pm_mesh_shade_u8) into out (frames, 720, 960, 3) uint8, frames any stride apart."""
+    """Shaded RGB of a chunk (pm_mesh_shade_u8) into out (frames, 720, 960, 3) uint8, frames any stride apart.
+    (frames, 1, ...) buffers take the single-view path into (frames, 720, 480, 3)."""
+    if vis.shape[1] != 2:
+        return mesh_shade_views(vis, xy, normal, faces, out)
     _chk(vis, torch.int64), _chk(xy, torch.int32), _chk(normal), _chk(faces, torch.int32), _chk(out, torch.uint8)
     assert out[0].is_contiguous() and normal.is_contiguous()
     _call("pm_mesh_shade_u8", vis.data_ptr(), xy.data_ptr(), normal.data_ptr(), xy.shape[2], faces.data_ptr(),
           vis.shape[0], out.data_ptr(), out.stride(0), _stream())
+
+
+def mesh_vertex_views(verts, views, faces, vf_csr, xy, depth, normal):
+    """mesh_vertex with xy.shape[1] (1 or 2) views per frame (pm_mesh_vertex_views_f32): verts and views hold one entry
+    per view; xy (frames, views, V, 2), depth (frames, views, V), normal (frames, views, V, 3)."""
+    nviews = xy.shape[1]
+    if len(verts) != nviews or len(views) != nviews:
+        raise _lib.PmError(f"mesh_vertex_views: {nviews} views need {nviews} vertex tensors and transforms")
+    for v in verts:
+        _chk(v)
+    _chk(xy, torch.int32), _chk(depth), _chk(normal), _chk(faces, torch.int32)
+    v0, (s0, o0) = verts[0], views[0]
+    v1, (s1, o1) = (verts[1], views[1]) if nviews == 2 else (None, (0.0, (0.0, 0.0, 0.0)))
+    vf_ptr, vf_face = vf_csr
+    _call("pm_mesh_vertex_views_f32", v0.data_ptr(), v0.stride(0), _ptr(v1), 0 if v1 is None else v1.stride(0),
+          v0.shape[1], v0.shape[0], float(s0), float(o0[0]), float(o0[1]), float(o0[2]), float(s1), float(o1[0]),
+          float(o1[1]), float(o1[2]), faces.data_ptr(), vf_ptr.data_ptr(), vf_face.data_ptr(), xy.data_ptr(),
+          depth.data_ptr(), normal.data_ptr(), nviews, _stream())
+
+
+def mesh_raster_views(xy, depth, faces, vis):
+    """mesh_raster with xy.shape[1] views per frame (pm_mesh_raster_views): vis (frames, views, 720, 480) int64."""
+    _chk(xy, torch.int32), _chk(depth), _chk(faces, torch.int32), _chk(vis, torch.int64)
+    assert xy.is_contiguous() and depth.is_contiguous() and vis.is_contiguous() and vis.shape[1] == xy.shape[1]
+    _lib.call("pm_memset_async", vis.data_ptr(), 0xFF, vis.numel() * 8, _stream())
+    _call("pm_mesh_raster_views", xy.data_ptr(), depth.data_ptr(), xy.shape[2], faces.data_ptr(), faces.shape[0],
+          xy.shape[0], vis.data_ptr(), xy.shape[1], _stream())
+
+
+def mesh_shade_views(vis, xy, normal, faces, out):
+    """mesh_shade with vis.shape[1] views per frame (pm_mesh_shade_views_u8): out (frames, 720, views * 480, 3) uint8,
+    frames any stride apart."""
+    _chk(vis, torch.int64), _chk(xy, torch.int32), _chk(normal), _chk(faces, torch.int32), _chk(out, torch.uint8)
+    assert out[0].is_contiguous() and normal.is_contiguous() and out.shape[2] == vis.shape[1] * vis.shape[3]
+    _call("pm_mesh_shade_views_u8", vis.data_ptr(), xy.data_ptr(), normal.data_ptr(), xy.shape[2], faces.data_ptr(),
+          vis.shape[0], out.data_ptr(), out.stride(0), vis.shape[1], _stream())
+
+
+def time_upsample(x, k, out=None):
+    """motion_io.time_upsample_numpy in float32 (pm_time_upsample_f32): x (batch, t, ch), any clip / frame strides with
+    a dense last dimension -> out (batch, k*t, ch) dense."""
+    _chk(x)
+    batch, t, ch = x.shape
+    if out is None:
+        out = torch.empty(batch, k * t, ch, device=x.device, dtype=torch.float32)
+    _chk(out)
+    assert tuple(out.shape) == (batch, k * t, ch) and out.is_contiguous()
+    xb, xt = _clip_frame_strides(x)
+    _call("pm_time_upsample_f32", x.data_ptr(), xb, xt, batch, t, ch, int(k), out.data_ptr(), _stream())
+    return out
 
 
 def softmax2_mix(sel, c1, c2, out=None):
