@@ -33,7 +33,7 @@
 extern "C" {
 #endif
 
-#define PM_ABI_VERSION 5
+#define PM_ABI_VERSION 6
 #define PM_FMT_F16 0x100
 #define PM_TC_TILE_SHIFT 16   /* pm_tapgemm_tc: N tile override in bits 16-23 of `nsplit` */
 int pm_abi_version(void);
@@ -131,15 +131,12 @@ int pm_attention_tc(const uint16_t* Q, long long q_ps, long long q_bs, int ldq, 
 int pm_add_rows_f32(const float* x, const float* pe, const float* spk, int first, int second,
                     float* out, int batch, int rows, int ch,
                     uint16_t* planes, long long p_ps, int p_ld, int p_nsplit, void* stream);
-/* out = a + b over n elements viewed as rows of `ch` (M.py:312,320-325): the dense case of pm_add2_strided_f32 */
-int pm_add2_f32(const float* a, const float* b, float* out, long long n, int ch,
+/* out[r,:] = a[r,:] + b[r,:] for `rows` rows of `ch` columns with row strides lda / ldb / ldo (M.py:312,320-325; column
+ * ranges of wider tensors are read and written in place, e.g. the forward and backward halves of a BiLSTM output,
+ * camn:265).  A dense tensor of n elements is one row of n, or n / ch rows of ch with planes (ch % 4 == 0). */
+int pm_add2_f32(const float* a, long long lda, const float* b, long long ldb, float* out, long long ldo,
+                long long rows, long long ch,
                 uint16_t* planes, long long p_ps, int p_ld, int p_nsplit, void* stream);
-/* out[r,:] = a[r,:] + b[r,:] for `rows` rows of `ch` columns with row strides lda / ldb / ldo (column ranges of wider
- * tensors are read and written in place, e.g. the forward and backward halves of a BiLSTM output, camn:265).
- * Same fp32 `a + b` as pm_add2_f32; planes as there (ch % 4 == 0). */
-int pm_add2_strided_f32(const float* a, long long lda, const float* b, long long ldb, float* out, long long ldo,
-                        long long rows, long long ch,
-                        uint16_t* planes, long long p_ps, int p_ld, int p_nsplit, void* stream);
 
 /* ---- window assembly (M.py:384-391 and 267-268 fused): builds one window's motion-encoder input.
  * motion/mask: (batch, total_len, ch) full-sequence tensors, either may be NULL = inference()'s defaults (identity
@@ -272,20 +269,22 @@ int pm_smplx_skin_f32(float* verts, long long ld, long long rows, int n_verts,
 int pm_motion_rep_f32(const float* poses, long long pose_bs, long long pose_ts, const float* joints,
                       int batch, int t, float dt, float two_dt, float* rep15d, void* stream);
 
-/* ---- SMPL-X mesh render (pantomatrix_b200/render.py): emage_utils/fast_render.py:286-321
- * render_one_sequence_with_face, whose frames (fast_render.py:56-68 do_render_one_frame, 80-92 np.hstack) are two
- * 480 x 720 views side by side, 960 x 720 RGB uint8, row 0 at the top, black background.  Fixed scene (fast_render.py:
- * 30-57): OrthographicCamera(xmag=1, ymag=1, znear 0.05, zfar 100) at create_pose_camera(-2), so pixel x =
+/* ---- SMPL-X mesh render (pantomatrix_b200/render.py): emage_utils/fast_render.py's frames of `views` (1 or 2)
+ * 480 x 720 image views side by side, views * 480 x 720 RGB uint8, row 0 at the top, black background; view k is the
+ * frame's k-th 480-column block.  Two views: render_one_sequence_with_face (fast_render.py:286-321; 56-68
+ * do_render_one_frame, 80-92 np.hstack) and render_one_sequence (323-361); one: render_one_sequence_no_gt (363-391).
+ * Fixed scene (fast_render.py:30-57): OrthographicCamera(xmag=1, ymag=1, znear 0.05, zfar 100) at create_pose_camera(-2), so pixel x =
  * (x_view / xmag + 1) * 240 and y = (1 - y_view / ymag) * 360 (the aspect ratio is ignored: a 1.5x vertical stretch);
  * DirectionalLight at create_pose_light(-30), direction toward the light l = (0, 0.5, 0.866); colour 220.
- * A chunk holds `frames` frames of 2 views; view 0 is the left half.  Three launches per chunk:
+ * A chunk holds `frames` frames of `views` views.  With one view, verts1 / v1_fs and the second transform are not read
+ * (verts1 may be NULL).  Three launches per chunk:
  *
  * pm_mesh_vertex_f32: one thread per (frame, view, vertex).  View k reads verts_k + frame * vk_fs (V rows of xyz, the
  *   body model's vertex buffer in place), applies p * scale_k + offset_k in fp32 (multiply, then add), then the view
- *   transform and the projection in fp32, each operation rounded on its own.  Writes xy (frames, 2, V, 2) int32 = the
- *   pixel coordinates * 256 rounded to nearest even (8 sub-pixel bits), or INT_MIN where a coordinate is not finite or
- *   beyond the +-2^20-pixel guard band; depth (frames, 2, V) = -z_view fp32; normal (frames, 2, V, 3) fp32 = the
- *   normalised sum (0 when it is 0) of cross(b - a, c - a) of the transformed corners over the incident faces, in
+ *   transform and the projection in fp32, each operation rounded on its own.  Writes xy (frames, views, V, 2) int32 =
+ *   the pixel coordinates * 256 rounded to nearest even (8 sub-pixel bits), or INT_MIN where a coordinate is not finite
+ *   or beyond the +-2^20-pixel guard band; depth (frames, views, V) = -z_view fp32; normal (frames, views, V, 3) fp32 =
+ *   the normalised sum (0 when it is 0) of cross(b - a, c - a) of the transformed corners over the incident faces, in
  *   ascending face index: vf_ptr (V + 1) / vf_face, a CSR of the faces of each vertex.  faces (F, 3) int32.
  * pm_mesh_raster: one thread per (frame, view, triangle).  A triangle with an INT_MIN corner or zero area is skipped;
  *   one with negative area has corners 1 and 2 swapped (both sides are drawn).  Corner k's weight is the int64 edge
@@ -293,34 +292,20 @@ int pm_motion_rep_f32(const float* poses, long long pose_bs, long long pose_ts, 
  *   a centre is covered when every w_k > 0, or w_k = 0 on a top-left edge (dy < 0, or dy = 0 and dx > 0).  The
  *   bounding box is clamped to the viewport.  Depth = fp32(((w0 d0 + w1 d1) + w2 d2) / area2), fp64 and each operation
  *   rounded; pixels outside [znear, zfar] are clipped.  atomicMin of (depth bits << 32 | triangle id) into vis
- *   (frames, 2, 720, 480) uint64, which the caller clears to all ones (pm_memset_async 0xff): the nearest triangle wins,
- *   ties to the lower id, whatever the execution order.
+ *   (frames, views, 720, 480) uint64, which the caller clears to all ones (pm_memset_async 0xff): the nearest triangle
+ *   wins, ties to the lower id, whatever the execution order.
  * pm_mesh_shade_u8: one thread per pixel of vis.  Background (all ones) is 0; otherwise the triangle's weights at the
  *   pixel centre over area2 interpolate its corner normals, and value = rint(220 max(0, n.l / |n|)) is written to R, G
- *   and B of out + frame * out_fs + (y * 960 + view * 480 + x) * 3 (out_fs >= 720 * 960 * 3 bytes). */
+ *   and B of out + frame * out_fs + (y * views * 480 + view * 480 + x) * 3 (out_fs >= 720 * views * 480 * 3 bytes). */
 int pm_mesh_vertex_f32(const float* verts0, long long v0_fs, const float* verts1, long long v1_fs,
                        int n_verts, int frames, float scale0, float ox0, float oy0, float oz0,
                        float scale1, float ox1, float oy1, float oz1, const int* faces,
-                       const int* vf_ptr, const int* vf_face, int* xy, float* depth, float* normal, void* stream);
+                       const int* vf_ptr, const int* vf_face, int* xy, float* depth, float* normal,
+                       int views, void* stream);
 int pm_mesh_raster(const int* xy, const float* depth, int n_verts, const int* faces, int n_faces,
-                   int frames, unsigned long long* vis, void* stream);
+                   int frames, unsigned long long* vis, int views, void* stream);
 int pm_mesh_shade_u8(const unsigned long long* vis, const int* xy, const float* normal, int n_verts,
-                     const int* faces, int frames, unsigned char* out, long long out_fs, void* stream);
-/* The same three stages with `views` (1 or 2) image views per frame; with 2 they are the entry points above, bit for
- * bit.  With 1 (render_one_sequence_no_gt: one 480 x 720 body view), verts1 / v1_fs and the second transform are not
- * read (verts1 may be NULL); xy, depth, normal and vis are (frames, 1, ...) and the output frame is 480 wide:
- * out + frame * out_fs + (y * 480 + x) * 3, out_fs >= 720 * 480 * 3 bytes.  In general the frame is views * 480 wide
- * and view k is its k-th 480-column block. */
-int pm_mesh_vertex_views_f32(const float* verts0, long long v0_fs, const float* verts1, long long v1_fs,
-                             int n_verts, int frames, float scale0, float ox0, float oy0, float oz0,
-                             float scale1, float ox1, float oy1, float oz1, const int* faces,
-                             const int* vf_ptr, const int* vf_face, int* xy, float* depth, float* normal,
-                             int views, void* stream);
-int pm_mesh_raster_views(const int* xy, const float* depth, int n_verts, const int* faces, int n_faces,
-                         int frames, unsigned long long* vis, int views, void* stream);
-int pm_mesh_shade_views_u8(const unsigned long long* vis, const int* xy, const float* normal, int n_verts,
-                           const int* faces, int frames, unsigned char* out, long long out_fs, int views,
-                           void* stream);
+                     const int* faces, int frames, unsigned char* out, long long out_fs, int views, void* stream);
 /* pm_time_upsample_f32: motion_io.time_upsample_numpy (the npz writer's upsample=30 // pose_fps) as the renderer reads
  * its output back, float32.  x (batch, t, channels) with clip / frame strides x_bs / x_ts and a dense last dimension ->
  * out (batch, k t, channels) dense.  k = 1 copies.  Otherwise, with n = k t, output frame j sits at

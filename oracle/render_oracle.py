@@ -1,7 +1,7 @@
 """CPU restatement of the SMPL-X mesh render (TEST / MEASUREMENT INFRASTRUCTURE; never imported by the product).
 
-Restates include/pm_emage.h pm_mesh_vertex_f32 / pm_mesh_raster / pm_mesh_shade_u8 and the scene of
-emage_utils/fast_render.py, which it follows line by line where cited:
+Restates include/pm_emage.h pm_mesh_vertex_f32 / pm_mesh_raster / pm_mesh_shade_u8, one or two views per frame, and the
+scene of emage_utils/fast_render.py, which it follows line by line where cited:
   - viewport 480 x 720 per view (fast_render.py:17-24 args, :106-108 OffscreenRenderer(width, height)), the views side
     by side with the face view left (:80-92 np.hstack((fig1, fig2)), :164-176 distribute_frames, :318
     generate_silent_videos(..., vertices1_all, vertices_all, ...));

@@ -30,8 +30,7 @@ SIGNATURES = {
     "pm_attention_tc": [_p, _ll, _ll, _i, _i, _i, _p, _ll, _ll, _i, _i, _i, _p, _ll, _ll, _i, _i, _i,
                         _p, _i, _i, _i, _i, _i, _i, _p, _ll, _i, _i, _p],
     "pm_add_rows_f32": [_p, _p, _p, _i, _i, _p, _i, _i, _i, _p, _ll, _i, _i, _p],
-    "pm_add2_f32": [_p, _p, _p, _ll, _i, _p, _ll, _i, _i, _p],
-    "pm_add2_strided_f32": [_p, _ll, _p, _ll, _p, _ll, _ll, _ll, _p, _ll, _i, _i, _p],
+    "pm_add2_f32": [_p, _ll, _p, _ll, _p, _ll, _ll, _ll, _p, _ll, _i, _i, _p],
     "pm_window_input_f32": [_p, _p, _p, _p, _p, _i, _i, _i, _i, _i, _i, _ll, _p, _ll, _i, _i, _p],
     "pm_l2_argmin_f32": [_p, _ll, _i, _ll, _p, _p, _i, _i, _p, _p],
     "pm_row_argmax_f32": [_p, _ll, _i, _i, _i, _ll, _p, _p, _p],
@@ -51,13 +50,9 @@ SIGNATURES = {
                         _p, _p, _p, _i, _p, _ll, _i, _i, _p],
     "pm_smplx_skin_f32": [_p, _ll, _ll, _i, _p, _p, _p, _p, _p, _ll, _ll, _i, _p],
     "pm_motion_rep_f32": [_p, _ll, _ll, _p, _i, _i, _f, _f, _p, _p],
-    "pm_mesh_vertex_f32": [_p, _ll, _p, _ll, _i, _i, _f, _f, _f, _f, _f, _f, _f, _f, _p, _p, _p, _p, _p, _p, _p],
-    "pm_mesh_raster": [_p, _p, _i, _p, _i, _i, _p, _p],
-    "pm_mesh_shade_u8": [_p, _p, _p, _i, _p, _i, _p, _ll, _p],
-    "pm_mesh_vertex_views_f32": [_p, _ll, _p, _ll, _i, _i, _f, _f, _f, _f, _f, _f, _f, _f, _p, _p, _p, _p, _p, _p, _i,
-                                 _p],
-    "pm_mesh_raster_views": [_p, _p, _i, _p, _i, _i, _p, _i, _p],
-    "pm_mesh_shade_views_u8": [_p, _p, _p, _i, _p, _i, _p, _ll, _i, _p],
+    "pm_mesh_vertex_f32": [_p, _ll, _p, _ll, _i, _i, _f, _f, _f, _f, _f, _f, _f, _f, _p, _p, _p, _p, _p, _p, _i, _p],
+    "pm_mesh_raster": [_p, _p, _i, _p, _i, _i, _p, _i, _p],
+    "pm_mesh_shade_u8": [_p, _p, _p, _i, _p, _i, _p, _ll, _i, _p],
     "pm_time_upsample_f32": [_p, _ll, _ll, _i, _i, _i, _i, _p, _p],
 }
 

@@ -337,9 +337,9 @@ extern "C" int pm_add_rows_f32(const float* x, const float* pe, const float* spk
   PM_LAUNCH_CHECK();
 }
 
-extern "C" int pm_add2_strided_f32(const float* a, long long lda, const float* b, long long ldb, float* out,
-                                   long long ldo, long long rows, long long ch,
-                                   uint16_t* planes, long long p_ps, int p_ld, int p_nsplit, void* stream) {
+extern "C" int pm_add2_f32(const float* a, long long lda, const float* b, long long ldb, float* out, long long ldo,
+                           long long rows, long long ch,
+                           uint16_t* planes, long long p_ps, int p_ld, int p_nsplit, void* stream) {
   PM_REQUIRE(a && b && (out || planes) && rows >= 0 && ch > 0);
   PM_REQUIRE(rows <= 1 || (lda >= ch && ldb >= ch && (!out || ldo >= ch)));
   PM_REQUIRE(!planes || ((ch & 3) == 0 && ch <= 0x7fffffffLL));
@@ -356,15 +356,6 @@ extern "C" int pm_add2_strided_f32(const float* a, long long lda, const float* b
   if (f16) add2_kernel<true><<<grid, 256, 0, st>>>(a, lda, b, ldb, out, ldo, rows, ch, nv, P);
   else add2_kernel<false><<<grid, 256, 0, st>>>(a, lda, b, ldb, out, ldo, rows, ch, nv, P);
   PM_LAUNCH_CHECK();
-}
-
-extern "C" int pm_add2_f32(const float* a, const float* b, float* out, long long n, int ch,
-                           uint16_t* planes, long long p_ps, int p_ld, int p_nsplit, void* stream) {
-  PM_REQUIRE(a && b && (out || planes) && n >= 0);
-  PM_REQUIRE(!planes || (ch > 0 && (ch & 3) == 0 && n % ch == 0));
-  if (n == 0) return PM_OK;
-  const long long rows = planes ? n / ch : 1, cols = planes ? ch : n;        // the dense case of the strided add
-  return pm_add2_strided_f32(a, cols, b, cols, out, cols, rows, cols, planes, p_ps, p_ld, p_nsplit, stream);
 }
 
 extern "C" int pm_window_input_f32(const float* motion, const float* mask, const float* seed,

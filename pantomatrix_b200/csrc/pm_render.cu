@@ -1,11 +1,11 @@
 // SMPL-X mesh render (pantomatrix_b200/render.py): the frames of emage_utils/fast_render.py, one view per frame
 // (render_one_sequence_no_gt) or two side by side (render_one_sequence_with_face, render_one_sequence).  Three launches
 // per chunk of frames: pm_mesh_vertex_f32 (view transform, projection, snapping, vertex normals), pm_mesh_raster
-// (visibility keys by atomicMin) and pm_mesh_shade_u8 (Lambert shading into the RGB frame), each a two-view entry point
-// and a *_views one that takes the view count; plus pm_time_upsample_f32, the piecewise-linear frame-rate upsampling of
-// the npz writer.  Contracts and the exact rules: include/pm_emage.h; CPU restatement: oracle/render_oracle.py.  Built
-// with -fmad=false: every fp32 / fp64 product and sum is rounded on its own, so the restatement reproduces the snapped
-// coordinates and depths operation by operation.
+// (visibility keys by atomicMin) and pm_mesh_shade_u8 (Lambert shading into the RGB frame), each taking the view count;
+// plus pm_time_upsample_f32, the piecewise-linear frame-rate upsampling of the npz writer.  Contracts and the exact
+// rules: include/pm_emage.h; CPU restatement: oracle/render_oracle.py.  Built with -fmad=false: every fp32 / fp64
+// product and sum is rounded on its own, so the restatement reproduces the snapped coordinates and depths operation by
+// operation.
 #include <limits.h>
 #include <math.h>
 
@@ -275,40 +275,20 @@ extern "C" int pm_mesh_vertex_f32(const float* verts0, long long v0_fs, const fl
                                   int n_verts, int frames, float scale0, float ox0, float oy0, float oz0,
                                   float scale1, float ox1, float oy1, float oz1, const int* faces,
                                   const int* vf_ptr, const int* vf_face, int* xy, float* depth, float* normal,
-                                  void* stream) {
-  return launch_vertex(2, verts0, v0_fs, verts1, v1_fs, n_verts, frames,
-                       ViewXf{scale0, ox0, oy0, oz0, scale1, ox1, oy1, oz1}, faces, vf_ptr, vf_face, xy, depth, normal,
-                       stream);
-}
-
-extern "C" int pm_mesh_raster(const int* xy, const float* depth, int n_verts, const int* faces, int n_faces,
-                              int frames, unsigned long long* vis, void* stream) {
-  return launch_raster(2, xy, depth, n_verts, faces, n_faces, frames, vis, stream);
-}
-
-extern "C" int pm_mesh_shade_u8(const unsigned long long* vis, const int* xy, const float* normal, int n_verts,
-                                const int* faces, int frames, unsigned char* out, long long out_fs, void* stream) {
-  return launch_shade(2, vis, xy, normal, n_verts, faces, frames, out, out_fs, stream);
-}
-
-extern "C" int pm_mesh_vertex_views_f32(const float* verts0, long long v0_fs, const float* verts1, long long v1_fs,
-                                        int n_verts, int frames, float scale0, float ox0, float oy0, float oz0,
-                                        float scale1, float ox1, float oy1, float oz1, const int* faces,
-                                        const int* vf_ptr, const int* vf_face, int* xy, float* depth, float* normal,
-                                        int views, void* stream) {
+                                  int views, void* stream) {
   return launch_vertex(views, verts0, v0_fs, verts1, v1_fs, n_verts, frames,
                        ViewXf{scale0, ox0, oy0, oz0, scale1, ox1, oy1, oz1}, faces, vf_ptr, vf_face, xy, depth, normal,
                        stream);
 }
 
-extern "C" int pm_mesh_raster_views(const int* xy, const float* depth, int n_verts, const int* faces, int n_faces,
-                                    int frames, unsigned long long* vis, int views, void* stream) {
+extern "C" int pm_mesh_raster(const int* xy, const float* depth, int n_verts, const int* faces, int n_faces,
+                              int frames, unsigned long long* vis, int views, void* stream) {
   return launch_raster(views, xy, depth, n_verts, faces, n_faces, frames, vis, stream);
 }
 
-extern "C" int pm_mesh_shade_views_u8(const unsigned long long* vis, const int* xy, const float* normal, int n_verts,
-                                      const int* faces, int frames, unsigned char* out, long long out_fs, int views,
-                                      void* stream) {
+extern "C" int pm_mesh_shade_u8(const unsigned long long* vis, const int* xy, const float* normal, int n_verts,
+                                const int* faces, int frames, unsigned char* out, long long out_fs, int views,
+                                void* stream) {
   return launch_shade(views, vis, xy, normal, n_verts, faces, frames, out, out_fs, stream);
 }
 

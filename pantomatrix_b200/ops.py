@@ -247,21 +247,22 @@ def add_rows(x, pe, spk, first, second, batch, rows, ch, nsplit=0, f32=True):
 
 
 def add2(a, b, nsplit=0, f32=True):
-    """a + b.  Dense operands, or (fp32 out only) (..., ch) views with evenly spaced rows - e.g. the two column halves of
-    a BiLSTM output, read in place (pm_add2_strided_f32, same fp32 a + b).  Returns a dense tensor / Act."""
+    """a + b (pm_add2_f32).  Dense operands, or (fp32 out only) (..., ch) views with evenly spaced rows - e.g. the two
+    column halves of a BiLSTM output, read in place.  Returns a dense tensor / Act."""
     _chk(a), _chk(b)
     assert a.shape == b.shape, (a.shape, b.shape)
+    n, ch = a.numel(), a.shape[-1]
     if not (a.is_contiguous() and b.is_contiguous()):
         assert nsplit == 0, "strided add2 writes fp32 only"
-        out = torch.empty(a.shape, device=a.device, dtype=torch.float32)
-        rows, lda = _rows_ld(a)
-        _call("pm_add2_strided_f32", a.data_ptr(), lda, b.data_ptr(), _rows_ld(b)[1], out.data_ptr(), a.shape[-1],
-              rows, a.shape[-1], None, 0, 0, 0, _stream())
-        return out
-    out = torch.empty_like(a) if (f32 or not nsplit) else None
-    ch = a.shape[-1]
-    pl = _new_planes(nsplit, (a.shape[0], a.numel() // ch // a.shape[0]), ch, a.device) if nsplit else None
-    _call("pm_add2_f32", a.data_ptr(), b.data_ptr(), _ptr(out), a.numel(), ch, *_pargs(pl), _stream())
+        out, pl = torch.empty(a.shape, device=a.device, dtype=torch.float32), None
+        (rows, lda), ldb, ldo = _rows_ld(a), _rows_ld(b)[1], ch
+    else:
+        out = torch.empty_like(a) if (f32 or not nsplit) else None
+        pl = _new_planes(nsplit, (a.shape[0], n // ch // a.shape[0]), ch, a.device) if nsplit else None
+        # planes are written per row of ch; fp32 alone is one row of n, so 16-byte access does not depend on ch
+        rows, lda = (n // ch, ch) if nsplit else (1, n)
+        ch = ldb = ldo = lda
+    _call("pm_add2_f32", a.data_ptr(), lda, b.data_ptr(), ldb, _ptr(out), ldo, rows, ch, *_pargs(pl), _stream())
     return _result(out, pl, nsplit)
 
 
@@ -626,79 +627,44 @@ def motion_rep(poses, joints, dt, two_dt, out):
 
 
 def mesh_vertex(verts, views, faces, vf_csr, xy, depth, normal):
-    """View transform, projection, snapping and vertex normals of a chunk (pm_mesh_vertex_f32).  verts: one (frames, V,
-    3) view per image view, frames any stride apart; views: ((scale, (ox, oy, oz)), ...) per image view.  Writes xy
-    (frames, 2, V, 2) int32, depth (frames, 2, V) and normal (frames, 2, V, 3).  Buffers of one view, (frames, 1, ...),
-    take the single-view path (mesh_vertex_views)."""
-    if xy.shape[1] != 2:
-        return mesh_vertex_views(verts, views, faces, vf_csr, xy, depth, normal)
-    for v in verts:
-        _chk(v)
-    _chk(xy, torch.int32), _chk(depth), _chk(normal), _chk(faces, torch.int32)
-    (v0, v1), ((s0, o0), (s1, o1)) = verts, views
-    vf_ptr, vf_face = vf_csr
-    _call("pm_mesh_vertex_f32", v0.data_ptr(), v0.stride(0), v1.data_ptr(), v1.stride(0), v0.shape[1], v0.shape[0],
-          float(s0), float(o0[0]), float(o0[1]), float(o0[2]), float(s1), float(o1[0]), float(o1[1]), float(o1[2]),
-          faces.data_ptr(), vf_ptr.data_ptr(),
-          vf_face.data_ptr(), xy.data_ptr(), depth.data_ptr(), normal.data_ptr(), _stream())
-
-
-def mesh_raster(xy, depth, faces, vis):
-    """Visibility keys of a chunk (pm_mesh_raster) into vis (frames, 2, 720, 480) int64, cleared here to all ones by a
-    memset (a memset node under graph capture).  (frames, 1, ...) buffers take the single-view path."""
-    if xy.shape[1] != 2:
-        return mesh_raster_views(xy, depth, faces, vis)
-    _chk(xy, torch.int32), _chk(depth), _chk(faces, torch.int32), _chk(vis, torch.int64)
-    assert xy.is_contiguous() and depth.is_contiguous() and vis.is_contiguous()
-    _lib.call("pm_memset_async", vis.data_ptr(), 0xFF, vis.numel() * 8, _stream())
-    _call("pm_mesh_raster", xy.data_ptr(), depth.data_ptr(), xy.shape[2], faces.data_ptr(), faces.shape[0],
-          xy.shape[0], vis.data_ptr(), _stream())
-
-
-def mesh_shade(vis, xy, normal, faces, out):
-    """Shaded RGB of a chunk (pm_mesh_shade_u8) into out (frames, 720, 960, 3) uint8, frames any stride apart.
-    (frames, 1, ...) buffers take the single-view path into (frames, 720, 480, 3)."""
-    if vis.shape[1] != 2:
-        return mesh_shade_views(vis, xy, normal, faces, out)
-    _chk(vis, torch.int64), _chk(xy, torch.int32), _chk(normal), _chk(faces, torch.int32), _chk(out, torch.uint8)
-    assert out[0].is_contiguous() and normal.is_contiguous()
-    _call("pm_mesh_shade_u8", vis.data_ptr(), xy.data_ptr(), normal.data_ptr(), xy.shape[2], faces.data_ptr(),
-          vis.shape[0], out.data_ptr(), out.stride(0), _stream())
-
-
-def mesh_vertex_views(verts, views, faces, vf_csr, xy, depth, normal):
-    """mesh_vertex with xy.shape[1] (1 or 2) views per frame (pm_mesh_vertex_views_f32): verts and views hold one entry
-    per view; xy (frames, views, V, 2), depth (frames, views, V), normal (frames, views, V, 3)."""
+    """View transform, projection, snapping and vertex normals of a chunk of xy.shape[1] (1 or 2) image views per frame
+    (pm_mesh_vertex_f32).  verts: one (frames, V, 3) tensor per view, frames any stride apart; views: one (scale, (ox,
+    oy, oz)) per view.  Writes xy (frames, views, V, 2) int32, depth (frames, views, V) and normal (frames, views, V,
+    3)."""
     nviews = xy.shape[1]
     if len(verts) != nviews or len(views) != nviews:
-        raise _lib.PmError(f"mesh_vertex_views: {nviews} views need {nviews} vertex tensors and transforms")
+        raise _lib.PmError(f"mesh_vertex: {nviews} views need {nviews} vertex tensors and transforms")
     for v in verts:
         _chk(v)
     _chk(xy, torch.int32), _chk(depth), _chk(normal), _chk(faces, torch.int32)
     v0, (s0, o0) = verts[0], views[0]
     v1, (s1, o1) = (verts[1], views[1]) if nviews == 2 else (None, (0.0, (0.0, 0.0, 0.0)))
     vf_ptr, vf_face = vf_csr
-    _call("pm_mesh_vertex_views_f32", v0.data_ptr(), v0.stride(0), _ptr(v1), 0 if v1 is None else v1.stride(0),
+    _call("pm_mesh_vertex_f32", v0.data_ptr(), v0.stride(0), _ptr(v1), 0 if v1 is None else v1.stride(0),
           v0.shape[1], v0.shape[0], float(s0), float(o0[0]), float(o0[1]), float(o0[2]), float(s1), float(o1[0]),
           float(o1[1]), float(o1[2]), faces.data_ptr(), vf_ptr.data_ptr(), vf_face.data_ptr(), xy.data_ptr(),
           depth.data_ptr(), normal.data_ptr(), nviews, _stream())
 
 
-def mesh_raster_views(xy, depth, faces, vis):
-    """mesh_raster with xy.shape[1] views per frame (pm_mesh_raster_views): vis (frames, views, 720, 480) int64."""
+def mesh_raster(xy, depth, faces, vis):
+    """Visibility keys of a chunk (pm_mesh_raster) into vis (frames, views, 720, 480) int64, views = xy.shape[1],
+    cleared here to all ones by a memset (a memset node under graph capture)."""
     _chk(xy, torch.int32), _chk(depth), _chk(faces, torch.int32), _chk(vis, torch.int64)
     assert xy.is_contiguous() and depth.is_contiguous() and vis.is_contiguous() and vis.shape[1] == xy.shape[1]
     _lib.call("pm_memset_async", vis.data_ptr(), 0xFF, vis.numel() * 8, _stream())
-    _call("pm_mesh_raster_views", xy.data_ptr(), depth.data_ptr(), xy.shape[2], faces.data_ptr(), faces.shape[0],
+    _call("pm_mesh_raster", xy.data_ptr(), depth.data_ptr(), xy.shape[2], faces.data_ptr(), faces.shape[0],
           xy.shape[0], vis.data_ptr(), xy.shape[1], _stream())
 
 
-def mesh_shade_views(vis, xy, normal, faces, out):
-    """mesh_shade with vis.shape[1] views per frame (pm_mesh_shade_views_u8): out (frames, 720, views * 480, 3) uint8,
+def mesh_shade(vis, xy, normal, faces, out):
+    """Shaded RGB of a chunk (pm_mesh_shade_u8) into out (frames, 720, views * 480, 3) uint8, views = vis.shape[1],
     frames any stride apart."""
     _chk(vis, torch.int64), _chk(xy, torch.int32), _chk(normal), _chk(faces, torch.int32), _chk(out, torch.uint8)
-    assert out[0].is_contiguous() and normal.is_contiguous() and out.shape[2] == vis.shape[1] * vis.shape[3]
-    _call("pm_mesh_shade_views_u8", vis.data_ptr(), xy.data_ptr(), normal.data_ptr(), xy.shape[2], faces.data_ptr(),
+    if out.shape[2] != vis.shape[1] * vis.shape[3]:
+        raise _lib.PmError(f"mesh_shade: {vis.shape[1]} views need out {vis.shape[1] * vis.shape[3]} wide, "
+                           f"got {out.shape[2]}")
+    assert out[0].is_contiguous() and normal.is_contiguous()
+    _call("pm_mesh_shade_u8", vis.data_ptr(), xy.data_ptr(), normal.data_ptr(), xy.shape[2], faces.data_ptr(),
           vis.shape[0], out.data_ptr(), out.stride(0), vis.shape[1], _stream())
 
 

@@ -1,8 +1,8 @@
 """SMPL-X mesh frames on the GPU: the reference's face, body and prediction-beside-ground-truth views of poses.
 
 emage_utils/fast_render.py renders every frame of the SMPL-X mesh with pyrender in one of three layouts, all drawn here
-with three kernels per chunk of frames (include/pm_emage.h pm_mesh_vertex_f32 / pm_mesh_raster / pm_mesh_shade_u8 and
-their *_views forms, DESIGN.md section 10):
+with three kernels per chunk of frames, each taking the view count (include/pm_emage.h pm_mesh_vertex_f32 /
+pm_mesh_raster / pm_mesh_shade_u8, DESIGN.md section 10):
   - render_sequence: render_one_sequence_with_face (:286-321), a face close-up (only the jaw posed, the mesh scaled x7
     and moved down by 10) left of the full body, 960 x 720;
   - render_body: render_one_sequence_no_gt (:363-391), the full body alone, 480 x 720 (CaMN and DisCo output, upsampled
@@ -124,24 +124,24 @@ class MeshRenderer:
         if betas is not None:
             bm._check(betas, "betas", (batch, 300))
         n = t // FPS * FPS
+        return self._draw([(poses, betas, expression, trans, JAW_ONLY), (poses, betas, expression, trans, ALL_JOINTS)],
+                          (FACE_VIEW, BODY_VIEW), n, out)
+
+    def _draw(self, sides, views, n, out):
+        """Frames [0, n) of every clip, one image view per side (poses, betas, expression or None, trans, joint mask),
+        each side posed with its clip's frame-0 translation (remove_transl=True) and drawn with the transform(s)
+        `views`.  out: None or a contiguous (B, n, 720, 480 * len(sides), 3) uint8 tensor; returns it."""
+        batch, dev = sides[0][0].shape[0], sides[0][0].device
+        shape = (batch, n, H, len(sides) * W, 3)
         if out is None:
-            out = torch.empty(batch, n, H, VIEWS * W, 3, dtype=torch.uint8, device=poses.device)
-        elif tuple(out.shape) != (batch, n, H, VIEWS * W, 3) or out.dtype != torch.uint8 or not out.is_contiguous():
-            raise ValueError(f"out must be a contiguous ({batch}, {n}, {H}, {VIEWS * W}, 3) uint8 tensor")
+            out = torch.empty(shape, dtype=torch.uint8, device=dev)
+        elif tuple(out.shape) != shape or out.dtype != torch.uint8 or not out.is_contiguous():
+            raise ValueError(f"out must be a contiguous {shape} uint8 tensor")
         if n == 0:
             return out
-        p, e, tr = poses[:, :n], expression[:, :n], trans[:, :1].expand(batch, n, 3)     # frame stride 0: frame 0's trans
-        _, body = bm._vertices(p, betas, e, tr, ALL_JOINTS)
-        _, face = bm._vertices(p, betas, e, tr, JAW_ONLY)
-        self.render((face, body), (FACE_VIEW, BODY_VIEW), out.view(batch * n, H, VIEWS * W, 3))
-        return out
-
-    @staticmethod
-    def _out(out, shape, device):
-        if out is None:
-            return torch.empty(shape, dtype=torch.uint8, device=device)
-        if tuple(out.shape) != shape or out.dtype != torch.uint8 or not out.is_contiguous():
-            raise ValueError(f"out must be a contiguous {shape} uint8 tensor")
+        verts = [self.body_model._vertices(p[:, :n], b, None if e is None else e[:, :n], tr[:, :1].expand(batch, n, 3),
+                                           mask)[1] for p, b, e, tr, mask in sides]
+        self.render(verts, views, out.view(batch * n, *shape[2:]))
         return out
 
     @torch.no_grad()
@@ -163,16 +163,10 @@ class MeshRenderer:
             raise ValueError(f"upsample must be a positive int, got {upsample!r}")
         upsample = int(upsample)
         n = upsample * t // FPS * FPS
-        out = self._out(out, (batch, n, H, W, 3), poses.device)
-        if n == 0:
-            return out
-        if upsample > 1:
+        if upsample > 1 and n:
             poses = ops.time_upsample(poses, upsample)
             expression = None if expression is None else ops.time_upsample(expression, upsample)
-        e = None if expression is None else expression[:, :n]
-        _, body = bm._vertices(poses[:, :n], betas, e, trans[:, :1].expand(batch, n, 3), ALL_JOINTS)
-        self.render(body, BODY_VIEW, out.view(batch * n, H, W, 3))
-        return out
+        return self._draw([(poses, betas, expression, trans, ALL_JOINTS)], BODY_VIEW, n, out)
 
     @torch.no_grad()
     def render_pair(self, poses, trans, gt_poses, gt_trans, expression=None, betas=None, gt_expression=None,
@@ -199,11 +193,5 @@ class MeshRenderer:
                 bm._check(e, tag + "expression", (batch, tt, 100))
             if b is not None:
                 bm._check(b, tag + "betas", (batch, 300))
-            sides.append((p, tr, e, b))
-        out = self._out(out, (batch, n, H, VIEWS * W, 3), poses.device)
-        if n == 0:
-            return out
-        verts = [bm._vertices(p[:, :n], b, None if e is None else e[:, :n], tr[:, :1].expand(batch, n, 3), ALL_JOINTS)[1]
-                 for p, tr, e, b in sides]
-        self.render(verts, (BODY_VIEW, BODY_VIEW), out.view(batch * n, H, VIEWS * W, 3))
-        return out
+            sides.append((p, b, e, tr, ALL_JOINTS))
+        return self._draw(sides, (BODY_VIEW, BODY_VIEW), n, out)

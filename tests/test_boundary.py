@@ -72,9 +72,10 @@ def test_save_and_from_pretrained_round_trip(tmp_path):
     assert m2.quantizer.e_dim == 256 and m2.quantizer.embedding.weight.shape == (256, 256)
 
 
-def test_library_exports_every_declared_symbol():
+def test_library_exports_every_declared_symbol_at_the_header_abi_version():
     """Every function declared in include/pm_emage.h is exported by the built library and bound in
-    pantomatrix_b200._lib (no compute call is made: there is no GPU here)."""
+    pantomatrix_b200._lib, and the library reports the header's ABI version, 6 (no compute call is made: there is no
+    GPU here)."""
     from pantomatrix_b200 import _lib, build
     build.build()
     header = open(os.path.join(ROOT, "include", "pm_emage.h")).read()
@@ -84,7 +85,8 @@ def test_library_exports_every_declared_symbol():
     for name in declared:
         assert hasattr(lib, name), f"{name} declared in pm_emage.h but not exported"
     assert declared == set(_lib.SIGNATURES), declared ^ set(_lib.SIGNATURES)
-    assert _lib.load().pm_abi_version() == 5
+    assert re.search(r"^#define PM_ABI_VERSION (\d+)$", header, flags=re.M).group(1) == "6"
+    assert _lib.load().pm_abi_version() == 6
 
 
 def test_ctypes_signatures_match_the_header():

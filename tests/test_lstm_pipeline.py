@@ -1,4 +1,4 @@
-"""CaMN / DisCo captured pipeline, host side (no GPU): argument marshalling of pm_lstm_cond_f32 and pm_add2_strided_f32,
+"""CaMN / DisCo captured pipeline, host side (no GPU): argument marshalling of pm_lstm_cond_f32 and pm_add2_f32,
 CapturedLstmPipeline's input validation on buffers that live on the CPU (no graph is built), and the captured step's
 schedule (kernel_cond) against the eager one (host_cond) with the kernels emulated by tests/fake_ops.py plus a
 restatement of pm_lstm_cond_f32."""
@@ -31,16 +31,23 @@ def recorder(monkeypatch):
     return ops, calls
 
 
-def test_strided_add2_marshals_row_strides(recorder):
+def test_add2_marshals_row_strides_and_the_dense_geometry(recorder):
     ops, calls = recorder
     y = torch.zeros(3, 5, 1024)
     out = ops.add2(y[:, :, :512], y[:, :, 512:])
     name, args = calls[-1]
-    assert name == "pm_add2_strided_f32" and out.shape == (3, 5, 512) and out.is_contiguous()
+    assert name == "pm_add2_f32" and out.shape == (3, 5, 512) and out.is_contiguous()
     assert args[1] == 1024 and args[2] == y.data_ptr() + 512 * 4 and args[3] == 1024 and args[5] == 512
     assert args[6] == 15 and args[7] == 512 and args[8] is None
-    ops.add2(torch.zeros(3, 5, 512), torch.zeros(3, 5, 512))
-    assert calls[-1][0] == "pm_add2_f32"                    # dense operands keep the dense entry point
+    # dense operands: one row of n elements (16-byte access whatever ch is), or n / ch rows of ch with planes
+    ops.add2(torch.zeros(3, 5, 61), torch.zeros(3, 5, 61))
+    name, args = calls[-1]
+    assert name == "pm_add2_f32" and (args[1], args[3], args[5]) == (915,) * 3 and args[6:8] == (1, 915)
+    assert args[8] is None
+    ops.add2(torch.zeros(3, 5, 64), torch.zeros(3, 5, 64), nsplit=2)
+    name, args = calls[-1]
+    assert name == "pm_add2_f32" and (args[1], args[3], args[5]) == (64,) * 3 and args[6:8] == (15, 64)
+    assert args[8] is not None and args[11] & 0xff == 2
     with pytest.raises(Exception):                        # clip rows not evenly spaced: no single row stride
         ops.add2(torch.zeros(3, 6, 8)[:, :5], torch.zeros(3, 6, 8)[:, :5])
 

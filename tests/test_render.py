@@ -238,7 +238,7 @@ def test_chunking_covers_every_frame_once(monkeypatch):
         assert r.render((face, body)).shape == (n, render.H, 2 * render.W, 3)
 
 
-def test_render_sequence_composes_the_reference_views(monkeypatch):
+def test_render_sequence_poses_and_draws_the_face_view_then_the_body_view(monkeypatch):
     calls = []
 
     class Body:
@@ -267,7 +267,7 @@ def test_render_sequence_composes_the_reference_views(monkeypatch):
         if n == 0:
             assert not calls and not drawn
             continue
-        assert [c[4] for c in calls] == [ALL_JOINTS, 1 << 22]
+        assert [c[4] for c in calls] == [1 << 22, ALL_JOINTS]          # in view order: face left, body right
         assert all(c[:4] == ((2, n, 165), (2, n, 100), 0, True) for c in calls)
         (verts, views, o), = drawn
         assert views == (render.FACE_VIEW, render.BODY_VIEW) and o.shape == (2 * n, render.H, 2 * render.W, 3)

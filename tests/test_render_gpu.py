@@ -1,8 +1,6 @@
 """SMPL-X mesh render on the H100 against the CPU restatement (oracle/render_oracle.py): vertex stage against float64,
 visibility bit for bit, shaded values within 1, determinism, CUDA graph capture and render_sequence end to end on EMAGE
 generate() output."""
-import types
-
 import numpy as np
 import pytest
 import torch
@@ -10,40 +8,20 @@ import torch
 from body_cases import random_poses
 from oracle import render_oracle as R
 from oracle.smplx_oracle import SmplxRestatement
-from pantomatrix_b200 import ops
 from pantomatrix_b200.body_model import SmplxBodyModel
 from pantomatrix_b200.render import BODY_VIEW, FACE_VIEW, H, W, MeshRenderer
+from render_cases import DEV, posed, renderer, run_chunk, sphere, world
 from synthetic_models import SMPLX_FULL_VERTS, smplx_arrays, smplx_surface_arrays
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda"
 VIEWS = (FACE_VIEW, BODY_VIEW)
-
-
-def _renderer(v, faces):
-    return MeshRenderer(types.SimpleNamespace(n_verts=v, faces=faces, device=torch.device(DEV)))
-
-
-def _run(r, verts, views):
-    """The three kernels on one chunk: (xy, depth, normal, vis, rgb) on the host."""
-    k, nv = verts[0].shape[0], r.n_verts
-    xy = torch.empty(k, 2, nv, 2, dtype=torch.int32, device=DEV)
-    depth = torch.empty(k, 2, nv, device=DEV)
-    normal = torch.empty(k, 2, nv, 3, device=DEV)
-    vis = torch.empty(k, 2, H, W, dtype=torch.int64, device=DEV)
-    rgb = torch.empty(k, H, 2 * W, 3, dtype=torch.uint8, device=DEV)
-    ops.mesh_vertex(verts, views, r.faces, r.vf_csr, xy, depth, normal)
-    ops.mesh_raster(xy, depth, r.faces, vis)
-    ops.mesh_shade(vis, xy, normal, r.faces, rgb)
-    torch.cuda.synchronize()
-    return xy.cpu().numpy(), depth.cpu().numpy(), normal.cpu().numpy(), vis.cpu().numpy().view(np.uint64), rgb.cpu().numpy()
 
 
 def _check(verts, views, faces, normal_cond=0.0):
     """Every claim of the kernels on one chunk against the oracle.  normal_cond: normals are gated only where the float64
     sum of the face normals keeps at least that fraction of the sum of their lengths (random soups cancel)."""
-    r = _renderer(verts[0].shape[1], faces)
-    xy, depth, normal, vis, rgb = _run(r, verts, views)
+    r = renderer(verts[0].shape[1], faces)
+    xy, depth, normal, vis, rgb = run_chunk(r, verts, views)
     f = np.asarray(faces, np.int64)
     covered = 0
     for k in range(verts[0].shape[0]):
@@ -76,30 +54,11 @@ def _check(verts, views, faces, normal_cond=0.0):
     return covered
 
 
-def _world(x, frames=1):
-    return torch.as_tensor(np.asarray(x, np.float32), device=DEV).expand(frames, *np.shape(x)).contiguous()
-
-
-def _sphere(rings=24, segs=40):
-    v = [(0.0, 0.0, -1.0)]
-    for r in range(1, rings):
-        th = np.pi * r / rings
-        v += [(np.sin(th) * np.cos(p), np.sin(th) * np.sin(p), -np.cos(th)) for p in 2 * np.pi * np.arange(segs) / segs]
-    v.append((0.0, 0.0, 1.0))
-    ring = lambda r, s: 1 + r * segs + s % segs
-    f = []
-    for s in range(segs):
-        f += [(0, ring(0, s + 1), ring(0, s)), (len(v) - 1, ring(rings - 2, s), ring(rings - 2, s + 1))]
-        for r in range(rings - 2):
-            f += [(ring(r, s), ring(r + 1, s + 1), ring(r + 1, s)), (ring(r, s), ring(r, s + 1), ring(r + 1, s + 1))]
-    return np.array(v), np.array(f)
-
-
 def test_structured_meshes_against_the_oracle():
     rng = np.random.default_rng(0)
-    v, f = _sphere()
-    sphere = [_world(v * 0.4 + (0.1, 1.2, 0.3)), _world(v * 0.6 + (0.0, 1.0, 0.0))]
-    assert _check(sphere, ((1.0, (0, 0, 0)), BODY_VIEW), f) > 50000
+    v, f = sphere()
+    spheres = [world(v * 0.4 + (0.1, 1.2, 0.3)), world(v * 0.6 + (0.0, 1.0, 0.0))]
+    assert _check(spheres, ((1.0, (0, 0, 0)), BODY_VIEW), f) > 50000
     # a jittered grid of shared edges, and two equal-depth overlapping triangles plus an interpenetrating one
     n = 30
     gx, gy = np.meshgrid(np.linspace(-0.9, 0.9, n), np.linspace(0.1, 1.9, n))
@@ -111,7 +70,7 @@ def test_structured_meshes_against_the_oracle():
                     [-0.2, 1.6, 0.2], [-0.8, 0.8, -0.3], [0.8, 0.8, 0.7], [0.0, 1.2, 0.2]])
     verts = np.concatenate([grid, tie])
     faces = np.concatenate([gf, n * n + np.array([[3, 4, 5], [0, 1, 2], [6, 7, 8]])])
-    assert _check([_world(verts, 2), _world(verts, 2)], (BODY_VIEW, (1.0, (0.01, 0.003, -0.2))), faces) > 100000
+    assert _check([world(verts, 2), world(verts, 2)], (BODY_VIEW, (1.0, (0.01, 0.003, -0.2))), faces) > 100000
 
 
 def test_depth_clipping_against_the_oracle():
@@ -119,23 +78,13 @@ def test_depth_clipping_against_the_oracle():
     v = np.array([[-0.9, 0.2, 4.99], [0.9, 0.3, 4.9], [0.0, 1.8, 3.0], [-0.9, 1.9, -150.0], [0.9, 1.8, 0.0],
                   [0.2, 0.1, -20.0]])
     faces = np.array([[0, 1, 2], [3, 4, 5]])
-    assert _check([_world(v), _world(v)], (BODY_VIEW, (1.0, (0.0, 0.0, 0.02))), faces) > 10000
-
-
-def _posed(arrays, frames, seed, scale=0.3):
-    rng = np.random.default_rng(seed)
-    bm = SmplxBodyModel(arrays, DEV)
-    poses = torch.as_tensor(random_poses(rng, frames, scale).astype(np.float32), device=DEV).view(1, frames, 165)
-    trans = torch.as_tensor(rng.normal(0, 0.05, (1, frames, 3)) + (0, 1.0, 0), dtype=torch.float32, device=DEV)
-    body = bm(poses, transl=trans, vertices=True)["vertices"][0]
-    face = bm._vertices(poses, None, None, trans, 1 << 22)[1][0]
-    return bm, face, body
+    assert _check([world(v), world(v)], (BODY_VIEW, (1.0, (0.0, 0.0, 0.02))), faces) > 10000
 
 
 @pytest.mark.parametrize("kind", ["surface", "soup"])
 def test_full_size_models_in_both_views(kind):
     arrays = smplx_surface_arrays() if kind == "surface" else smplx_arrays(SMPLX_FULL_VERTS)
-    bm, face, body = _posed(arrays, 2 if kind == "surface" else 1, 5)       # the soup's oracle takes ~25 s a frame
+    bm, face, body = posed(arrays, 2 if kind == "surface" else 1, 5)       # the soup's oracle takes ~25 s a frame
     assert _check([face, body], VIEWS, arrays["f"], normal_cond=0.0 if kind == "surface" else 0.05) > 20000
 
 

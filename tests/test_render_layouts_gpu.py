@@ -1,10 +1,8 @@
 """Single-view mesh render, frame-rate upsampling and the body-only / prediction-beside-ground-truth layouts on the H100,
 against the CPU restatement (oracle/render_oracle.py, oracle/render_layouts_oracle.py) and the npz writer
 (motion_io.time_upsample_numpy): upsampling bit for bit, single-view chunks under the same gates as the two-view ones,
-two-view output bit for bit through the old and the new entry points, both layouts on the golden inputs and on CaMN,
-DisCo and EMAGE output, and CUDA graph capture."""
-import types
-
+a one-view chunk bit for bit the right half of the two-view one, both layouts on the golden inputs and on CaMN, DisCo
+and EMAGE output, and CUDA graph capture."""
 import numpy as np
 import pytest
 import torch
@@ -16,10 +14,10 @@ from oracle.smplx_oracle import SmplxRestatement
 from pantomatrix_b200 import motion_io, ops
 from pantomatrix_b200.body_model import SmplxBodyModel
 from pantomatrix_b200.render import BODY_VIEW, FACE_VIEW, H, W, MeshRenderer
+from render_cases import DEV, posed, renderer, run_chunk, sphere, world
 from synthetic_models import SMPLX_FULL_VERTS, SMPLX_SMALL_VERTS, smplx_arrays, smplx_surface_arrays
 
 pytestmark = pytest.mark.gpu
-DEV = "cuda"
 
 
 @pytest.mark.parametrize("t", [1, 2, 3, 37, 149])
@@ -36,36 +34,11 @@ def test_time_upsample_is_bit_identical_to_the_npz_writer(t, k):
     assert np.array_equal(got.cpu().numpy().view(np.uint32), want.view(np.uint32))
 
 
-def _renderer(v, faces):
-    return MeshRenderer(types.SimpleNamespace(n_verts=v, faces=faces, device=torch.device(DEV)))
-
-
-def _run(r, verts, views, views_entry=False):
-    """The three kernels on one chunk of len(verts) views: (xy, depth, normal, vis, rgb) on the host.  views_entry:
-    call the *_views entry points even for two views."""
-    k, nv, nviews = verts[0].shape[0], r.n_verts, len(verts)
-    xy = torch.empty(k, nviews, nv, 2, dtype=torch.int32, device=DEV)
-    depth = torch.empty(k, nviews, nv, device=DEV)
-    normal = torch.empty(k, nviews, nv, 3, device=DEV)
-    vis = torch.empty(k, nviews, H, W, dtype=torch.int64, device=DEV)
-    rgb = torch.empty(k, H, nviews * W, 3, dtype=torch.uint8, device=DEV)
-    if views_entry:
-        ops.mesh_vertex_views(verts, views, r.faces, r.vf_csr, xy, depth, normal)
-        ops.mesh_raster_views(xy, depth, r.faces, vis)
-        ops.mesh_shade_views(vis, xy, normal, r.faces, rgb)
-    else:
-        ops.mesh_vertex(verts, views, r.faces, r.vf_csr, xy, depth, normal)
-        ops.mesh_raster(xy, depth, r.faces, vis)
-        ops.mesh_shade(vis, xy, normal, r.faces, rgb)
-    torch.cuda.synchronize()
-    return xy.cpu().numpy(), depth.cpu().numpy(), normal.cpu().numpy(), vis.cpu().numpy().view(np.uint64), rgb.cpu().numpy()
-
-
 def _check_single(verts, view, faces, normal_cond=0.0):
     """One view per frame against the oracle: snapped coordinates within 1, normals, visibility bit for bit, RGB within
     1 on covered pixels and 0 elsewhere.  Returns the number of covered pixels."""
-    r = _renderer(verts.shape[1], faces)
-    xy, depth, normal, vis, rgb = _run(r, [verts], [view])
+    r = renderer(verts.shape[1], faces)
+    xy, depth, normal, vis, rgb = run_chunk(r, [verts], [view])
     assert rgb.shape[2] == W
     f = np.asarray(faces, np.int64)
     covered = 0
@@ -98,29 +71,10 @@ def _check_single(verts, view, faces, normal_cond=0.0):
     return covered
 
 
-def _world(x, frames=1):
-    return torch.as_tensor(np.asarray(x, np.float32), device=DEV).expand(frames, *np.shape(x)).contiguous()
-
-
-def _sphere(rings=24, segs=40):
-    v = [(0.0, 0.0, -1.0)]
-    for r in range(1, rings):
-        th = np.pi * r / rings
-        v += [(np.sin(th) * np.cos(p), np.sin(th) * np.sin(p), -np.cos(th)) for p in 2 * np.pi * np.arange(segs) / segs]
-    v.append((0.0, 0.0, 1.0))
-    ring = lambda r, s: 1 + r * segs + s % segs
-    f = []
-    for s in range(segs):
-        f += [(0, ring(0, s + 1), ring(0, s)), (len(v) - 1, ring(rings - 2, s), ring(rings - 2, s + 1))]
-        for r in range(rings - 2):
-            f += [(ring(r, s), ring(r + 1, s + 1), ring(r + 1, s)), (ring(r, s), ring(r, s + 1), ring(r + 1, s + 1))]
-    return np.array(v), np.array(f)
-
-
 def test_single_view_structured_meshes_against_the_oracle():
     rng = np.random.default_rng(0)
-    v, f = _sphere()
-    assert _check_single(_world(v * 0.6 + (0.0, 1.0, 0.0), 2), BODY_VIEW, f) > 2 * 50000
+    v, f = sphere()
+    assert _check_single(world(v * 0.6 + (0.0, 1.0, 0.0), 2), BODY_VIEW, f) > 2 * 50000
     n = 30
     gx, gy = np.meshgrid(np.linspace(-0.9, 0.9, n), np.linspace(0.1, 1.9, n))
     grid = np.stack([gx, gy, rng.normal(0, 0.05, gx.shape)], -1).reshape(-1, 3) + rng.normal(0, 2e-3, (n * n, 3))
@@ -131,45 +85,31 @@ def test_single_view_structured_meshes_against_the_oracle():
                     [-0.2, 1.6, 0.2], [-0.8, 0.8, -0.3], [0.8, 0.8, 0.7], [0.0, 1.2, 0.2]])
     verts = np.concatenate([grid, tie])
     faces = np.concatenate([gf, n * n + np.array([[3, 4, 5], [0, 1, 2], [6, 7, 8]])])
-    assert _check_single(_world(verts, 3), (1.0, (0.01, 0.003, -0.2)), faces) > 3 * 100000
+    assert _check_single(world(verts, 3), (1.0, (0.01, 0.003, -0.2)), faces) > 3 * 100000
     # depth clipping: triangles reaching behind znear and beyond zfar
     v = np.array([[-0.9, 0.2, 4.99], [0.9, 0.3, 4.9], [0.0, 1.8, 3.0], [-0.9, 1.9, -150.0], [0.9, 1.8, 0.0],
                   [0.2, 0.1, -20.0]])
-    assert _check_single(_world(v), (1.0, (0.0, 0.0, 0.02)), np.array([[0, 1, 2], [3, 4, 5]])) > 10000
-
-
-def _posed(arrays, frames, seed, scale=0.3):
-    rng = np.random.default_rng(seed)
-    bm = SmplxBodyModel(arrays, DEV)
-    poses = torch.as_tensor(random_poses(rng, frames, scale).astype(np.float32), device=DEV).view(1, frames, 165)
-    trans = torch.as_tensor(rng.normal(0, 0.05, (1, frames, 3)) + (0, 1.0, 0), dtype=torch.float32, device=DEV)
-    body = bm(poses, transl=trans, vertices=True)["vertices"][0]
-    face = bm._vertices(poses, None, None, trans, 1 << 22)[1][0]
-    return bm, face, body
+    assert _check_single(world(v), (1.0, (0.0, 0.0, 0.02)), np.array([[0, 1, 2], [3, 4, 5]])) > 10000
 
 
 @pytest.mark.parametrize("kind", ["surface", "soup"])
 def test_single_view_full_size_models(kind):
     arrays = smplx_surface_arrays() if kind == "surface" else smplx_arrays(SMPLX_FULL_VERTS)
-    _, _, body = _posed(arrays, 2 if kind == "surface" else 1, 6)
+    _, _, body = posed(arrays, 2 if kind == "surface" else 1, 6)
     assert _check_single(body, BODY_VIEW, arrays["f"], normal_cond=0.0 if kind == "surface" else 0.05) > 20000
 
 
-def test_two_views_are_bit_identical_through_the_old_and_new_entry_points():
+def test_one_view_draws_the_right_half_of_two_views_bit_for_bit():
     arrays = smplx_surface_arrays()
-    _, face, body = _posed(arrays, 11, 8)
-    r = _renderer(face.shape[1], arrays["f"])
+    _, face, body = posed(arrays, 11, 8)
+    r = renderer(face.shape[1], arrays["f"])
     for views in ((FACE_VIEW, BODY_VIEW), (BODY_VIEW, (1.0, (0.1, -0.05, 0.2)))):
-        old = _run(r, [face, body], views)
-        new = _run(r, [face, body], views, views_entry=True)
-        for a, b in zip(old, new):
-            assert np.array_equal(a, b)
-        # a single view draws exactly the right half of the two-view frame
-        one = _run(r, [body], views[1:])
-        for a, b in zip(old[:4], one[:4]):
+        two = run_chunk(r, [face, body], views)
+        one = run_chunk(r, [body], views[1:])
+        for a, b in zip(two[:4], one[:4]):
             assert np.array_equal(a[:, 1:], b)
-        assert np.array_equal(old[4][:, :, W:], one[4])
-        assert (old[4] > 0).mean() > 0.05
+        assert np.array_equal(two[4][:, :, W:], one[4])
+        assert (two[4] > 0).mean() > 0.05
 
 
 def _spy(r):
