@@ -10,8 +10,8 @@ pelvis with the SMPL-X body model: pass the model file with --smplx SMPLX_NEUTRA
 reference writer derives), or --trans-zero to write zeros instead.
 `--render` (needs --smplx) draws the reference demos' SMPL-X body view (fast_render.py render_one_sequence_no_gt: one
 480 x 720 view, whole seconds at 30 fps) of the motion upsampled to 30 fps as the npz stores it, on the GPU, with the
-translation the npz receives, and writes the frames as PNG files with Pillow next to each npz; video encoding is left to
-the user (e.g. ffmpeg -framerate 30 -i frame_%05d.png)."""
+translation the npz receives, and writes the frames as PNG files next to each npz, encoded on the GPU
+(pantomatrix_b200.png); video encoding is left to the user (e.g. ffmpeg -framerate 30 -i frame_%05d.png)."""
 import argparse
 import os
 import sys
@@ -30,11 +30,9 @@ from pantomatrix_b200.motion_io import beat_format_save, pelvis_translation  # n
 
 
 def write_frames(frames, folder):
-    """(N, 720, 480, 3) uint8 frames -> folder/frame_%05d.png."""
-    from PIL import Image
-    os.makedirs(folder, exist_ok=True)
-    for i, img in enumerate(frames.cpu().numpy()):
-        Image.fromarray(img).save(os.path.join(folder, f"frame_{i:05d}.png"))
+    """(N, 720, 480, 3) uint8 CUDA frames -> folder/frame_%05d.png, encoded on the GPU (pantomatrix_b200.png)."""
+    from pantomatrix_b200 import png
+    png.write_frames(frames, folder)
 
 
 def main():

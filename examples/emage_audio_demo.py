@@ -6,8 +6,8 @@
     python examples/emage_audio_demo.py ... --smplx SMPLX_NEUTRAL_2020.npz --render   # + <name>_frames/frame_%05d.png
 
 `--render` draws the reference demo's two-view SMPL-X frames (fast_render.py render_one_sequence_with_face: face
-close-up left, body right, whole seconds at 30 fps) on the GPU and writes them as PNG files with Pillow next to each
-npz; video encoding is left to the user (e.g. ffmpeg -framerate 30 -i frame_%05d.png).
+close-up left, body right, whole seconds at 30 fps) on the GPU and writes them as PNG files next to each npz,
+encoded on the GPU (pantomatrix_b200.png); video encoding is left to the user (e.g. ffmpeg -framerate 30 -i frame_%05d.png).
 `--checkpoint` is a local copy of the Hugging Face repo layout the reference downloads (config.json +
 model.safetensors at the top level, VQ models under emage_vq/{face,upper,lower,hands,global}).
 """
@@ -41,11 +41,9 @@ def load_models(args, device):
 
 
 def write_frames(frames, folder):
-    """(N, 720, 960, 3) uint8 frames -> folder/frame_%05d.png."""
-    from PIL import Image
-    os.makedirs(folder, exist_ok=True)
-    for i, img in enumerate(frames.cpu().numpy()):
-        Image.fromarray(img).save(os.path.join(folder, f"frame_{i:05d}.png"))
+    """(N, 720, 960, 3) uint8 CUDA frames -> folder/frame_%05d.png, encoded on the GPU (pantomatrix_b200.png)."""
+    from pantomatrix_b200 import png
+    png.write_frames(frames, folder)
 
 
 def main():

@@ -315,6 +315,39 @@ int pm_mesh_shade_u8(const unsigned long long* vis, const int* xy, const float* 
 int pm_time_upsample_f32(const float* x, long long x_bs, long long x_ts, int batch, int t, int channels, int k,
                          float* out, void* stream);
 
+/* ---- PNG encoding of RGB8 frames (pantomatrix_b200/png.py, DESIGN.md section 11) --------------------------------
+ * n_frames frames of h rows x w pixels of RGB8, each dense (row stride 3 w bytes), frame f at frames + f * f_fs.  Frame
+ * f becomes one PNG file in data + f * cap, by one rule:
+ *   scanlines: filter type 1 (Sub) on every row; S = h rows of s = 3 w + 1 bytes, byte 0 of a row 1, byte 1 + i
+ *     raw[i] - raw[i - 3] mod 256 (raw[i] for i < 3);
+ *   parse, per row, from its first byte: at frame position p the candidate distances, in the order
+ *     (1, 2, 3, 4, 5, 6, 7, 8, 9, 12, s, s - 3, s + 3, s - 6, s + 6), are valid when 1 <= d <= min(p, 32768); L_d is the
+ *     longest run <= min(258, row end - p) with S[p + j] == S[p + j - d] (overlap allowed, the source may lie in earlier
+ *     rows).  If max L_d >= 3 a match of that length at the first d reaching it, else the literal S[p];
+ *   deflate: one block, BFINAL = 1, BTYPE = 01 (fixed Huffman codes, RFC 1951 3.2.6), every row's tokens in row order,
+ *     end-of-block; codes bit-reversed into the LSB-first stream, extra bits not;
+ *   zlib: 0x78 0x01, the deflate data, Adler-32 of S big-endian;
+ *   PNG: signature, IHDR (w, h, depth 8, colour type 2, 0, 0, 0), one IDAT with the zlib stream, IEND; each chunk's
+ *     CRC-32 over its type and data.
+ * Bound: every token costs at most 9 bits per byte of S it covers, so a file has at most
+ *   ceil((3 + 9 h s + 7) / 8) + 63 bytes; every entry point requires that bound <= 2^31, cap >= it, cap a multiple of 4,
+ *   data 4-byte aligned.  Workspace: row_bits and row_adler, n_frames * h entries each.  Launch order on one stream:
+ *   pm_memset_async(data, 0, n_frames * cap), pm_png_count, pm_png_scan, pm_png_emit, pm_png_crc.
+ * pm_png_count: one thread per (frame, row): filters on the fly, parses, writes the row's bit count to row_bits and
+ *   its Adler-32 partials (sum of its bytes, sum of (s - i) x byte i, both mod 65521; wsum in the high word).
+ * pm_png_scan: one CTA per frame: row_bits becomes each row's bit offset in its slot, nbytes[f] the file's size; writes
+ *   everything but the block's data and IDAT's CRC, which it seeds with the part that does not depend on the data.
+ * pm_png_emit: one thread per (frame, row): the parse again, ORing the row's bits into the slot at its offset.
+ * pm_png_crc: one thread per 1 KiB block of IDAT's type and data: the block's CRC register moved to the chunk's end,
+ *   XORed into the CRC bytes (the CRC is linear, so the result does not depend on the order). */
+int pm_png_count(const unsigned char* frames, long long f_fs, int n_frames, int h, int w, long long* row_bits,
+                 unsigned long long* row_adler, void* stream);
+int pm_png_scan(int n_frames, int h, int w, long long* row_bits, const unsigned long long* row_adler,
+                unsigned char* data, long long cap, long long* nbytes, void* stream);
+int pm_png_emit(const unsigned char* frames, long long f_fs, int n_frames, int h, int w, const long long* row_off,
+                unsigned char* data, long long cap, void* stream);
+int pm_png_crc(int n_frames, int h, int w, unsigned char* data, long long cap, const long long* nbytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -54,6 +54,10 @@ SIGNATURES = {
     "pm_mesh_raster": [_p, _p, _i, _p, _i, _i, _p, _i, _p],
     "pm_mesh_shade_u8": [_p, _p, _p, _i, _p, _i, _p, _ll, _i, _p],
     "pm_time_upsample_f32": [_p, _ll, _ll, _i, _i, _i, _i, _p, _p],
+    "pm_png_count": [_p, _ll, _i, _i, _i, _p, _p, _p],
+    "pm_png_scan": [_i, _i, _i, _p, _p, _p, _ll, _p, _p],
+    "pm_png_emit": [_p, _ll, _i, _i, _i, _p, _p, _ll, _p],
+    "pm_png_crc": [_i, _i, _i, _p, _ll, _p, _p],
 }
 
 _lib = None

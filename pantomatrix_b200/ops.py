@@ -682,6 +682,28 @@ def time_upsample(x, k, out=None):
     return out
 
 
+# ------------------------------------------------------------------------------------------------------
+# PNG encoding
+# ------------------------------------------------------------------------------------------------------
+
+
+def png_encode(frames, data, nbytes, row_bits, row_adler):
+    """The PNG files of frames (N, H, W, 3) uint8, each frame dense, any stride apart, into the slots of data (N, cap)
+    uint8 with their sizes in nbytes (N,) int64 (include/pm_emage.h pm_png_*).  row_bits / row_adler: (N, H) int64
+    workspace.  The slots are cleared first by a memset (a memset node under graph capture), then four launches."""
+    _chk(frames, torch.uint8), _chk(data, torch.uint8), _chk(nbytes, torch.int64)
+    _chk(row_bits, torch.int64), _chk(row_adler, torch.int64)
+    n, h, w, _ = frames.shape
+    assert data.is_contiguous() and row_bits.is_contiguous() and row_adler.is_contiguous() and nbytes.is_contiguous()
+    cap, fs = data.shape[1], frames.stride(0) if n > 1 else 3 * h * w
+    _lib.call("pm_memset_async", data.data_ptr(), 0, data.numel(), _stream())
+    _call("pm_png_count", frames.data_ptr(), fs, n, h, w, row_bits.data_ptr(), row_adler.data_ptr(), _stream())
+    _call("pm_png_scan", n, h, w, row_bits.data_ptr(), row_adler.data_ptr(), data.data_ptr(), cap, nbytes.data_ptr(),
+          _stream())
+    _call("pm_png_emit", frames.data_ptr(), fs, n, h, w, row_bits.data_ptr(), data.data_ptr(), cap, _stream())
+    _call("pm_png_crc", n, h, w, data.data_ptr(), cap, nbytes.data_ptr(), _stream())
+
+
 def softmax2_mix(sel, c1, c2, out=None):
     """out[..., :] = softmax(sel[..., 0:2])[0] * c1 + [1] * c2 (out may be a column slice of a wider tensor)."""
     _chk(sel), _chk(c1), _chk(c2)
