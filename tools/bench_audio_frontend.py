@@ -15,18 +15,18 @@ Writes OUT_DIR/audio_frontend.json (and prints it):
            SMPL-X parameters, for (a) CapturedPipeline(input_rate=48000, input_channels=2, input_dtype=int16) fed the
            int16 stereo PCM, (b) host resample_poly of that PCM, then the default 16 kHz CapturedPipeline, (c) the
            default pipeline fed 16 kHz float32 directly (no front-end).  The three alternate step by step.
-  device   torch.cuda.get_device_name and nvidia-smi's name / power.limit, read in the same run.
+  device   measure.card(): the name, power limit and max SM clock of the card the run uses, read before and after
+           (device_after) in the same run.
 """
 import argparse
 import json
 import os
-import subprocess
 import sys
 import time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-HBM_GBPS = 3350.0                  # H100 SXM data sheet (700 W); not measured here
+from measure import HBM_BYTES_PER_S, alternate, card, per_call_ms  # noqa: E402
 SECONDS, FRAMES_PER_CLIP = 10, 300
 
 
@@ -66,16 +66,7 @@ def kernel_times(clips, reps):
             pcm = torch.from_numpy(_pcm(clips, rate, ch, dtype, rate + ch)).cuda()
             n_in = pcm.shape[1]
             out = torch.empty(clips, rs.n_out(n_in), device="cuda")
-            for _ in range(10):
-                rs(pcm, out=out)
-            torch.cuda.synchronize()
-            ev = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(reps)]
-            for s, e in ev:
-                s.record()
-                rs(pcm, out=out)
-                e.record()
-            torch.cuda.synchronize()
-            ms = sorted(s.elapsed_time(e) for s, e in ev)
+            ms = sorted(per_call_ms(lambda: rs(pcm, out=out), reps, warmup=10))
             med, mean = ms[len(ms) // 2], sum(ms) / len(ms)
             nbytes = pcm.numel() * pcm.element_size() + out.numel() * 4
             gbps = nbytes / (med * 1e-3) / 1e9
@@ -83,7 +74,7 @@ def kernel_times(clips, reps):
                 "clips": clips, "n_in": n_in, "n_out": out.shape[1], "up": rs.up, "down": rs.down, "taps_per_phase": rs.taps,
                 "launches": reps, "median_ms": med, "mean_ms": mean, "min_ms": ms[0],
                 "bytes_moved": nbytes, "bytes_per_output_sample": nbytes / out.numel(), "GBps": gbps,
-                "hbm_frac": gbps / HBM_GBPS, "bound": "bytes (HBM)",
+                "hbm_frac": gbps / (HBM_BYTES_PER_S / 1e9), "bound": "bytes (HBM)",
                 "fma_per_output_sample": rs.taps}
     return res
 
@@ -119,7 +110,6 @@ def e2e(clips, steps):
     staging = torch.empty(clips, n16).pin_memory()
     out_host = {k: torch.empty(clips, FRAMES_PER_CLIP, d).pin_memory() for k, d in
                 (("motion_axis_angle", 165), ("expression", 100), ("trans", 3))}
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")          # > the 50 MB L2
 
     def fetch(pred):
         for k, v in out_host.items():
@@ -134,23 +124,9 @@ def e2e(clips, steps):
         "host_resample_poly_then_16k": host_resample_then_16k,
         "16k_float32_input": lambda: fetch(cap16(audio16_pinned)[1]),
     }
-    for fn in arms.values():                                                # warm-up
-        fn()
-    torch.cuda.synchronize()
-    times = {k: [] for k in arms}
-    for i in range(steps):
-        for k, fn in arms.items():
-            flush.fill_(i & 0xFF)
-            torch.cuda.synchronize()
-            t0 = time.perf_counter()
-            fn()
-            torch.cuda.synchronize()
-            times[k].append(time.perf_counter() - t0)
-    res = {}
-    for k, ts in times.items():
-        med = sorted(ts)[len(ts) // 2]
-        res[k] = {"median_ms": 1e3 * med, "frames_per_s": clips * FRAMES_PER_CLIP / med,
-                  "runs_ms": [round(1e3 * t, 3) for t in ts]}
+    med, times = alternate(arms, steps, flush=256 << 20, clock="host")          # > the 50 MB L2
+    res = {k: {"median_ms": med[k], "frames_per_s": clips * FRAMES_PER_CLIP / (med[k] * 1e-3),
+               "runs_ms": [round(t, 3) for t in ts]} for k, ts in times.items()}
     res["config"] = {"clips": clips, "seconds_per_clip": SECONDS, "steps": steps, "h2d_bytes": {
         "gpu_front_end_48k_int16_stereo": pcm48_pinned.numel() * 2, "host_resample_poly_then_16k": staging.numel() * 4,
         "16k_float32_input": audio16_pinned.numel() * 4}, "kernels_per_replay": {
@@ -161,18 +137,6 @@ def e2e(clips, steps):
                                                   "16k_float32_input"))
     res["ratios"] = {"gpu_front_end_vs_16k_input": g / d, "gpu_front_end_vs_host_resample": g / h}
     return res
-
-
-def device_info():
-    import torch
-    info = {"torch_device_name": torch.cuda.get_device_name(0)}
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
-                           capture_output=True, text=True, timeout=30)
-        info["nvidia_smi_name_power_limit"] = q.stdout.strip()
-    except Exception as exc:
-        info["nvidia_smi_name_power_limit"] = f"unavailable: {exc!r}"
-    return info
 
 
 def main():
@@ -186,9 +150,9 @@ def main():
     if not torch.cuda.is_available():
         raise SystemExit("bench_audio_frontend.py needs a CUDA device")
     os.makedirs(args.out_dir, exist_ok=True)
-    res = {"device": device_info(), "kernel": kernel_times(args.clips, max(args.reps, 200)),
+    res = {"device": card(), "kernel": kernel_times(args.clips, max(args.reps, 200)),
            "host": host_times(args.clips), "e2e": e2e(args.clips, max(args.steps, 10))}
-    res["device_after"] = device_info()
+    res["device_after"] = card()
     path = os.path.join(args.out_dir, "audio_frontend.json")
     with open(path, "w") as f:
         json.dump(res, f, indent=1)

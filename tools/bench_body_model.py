@@ -19,7 +19,6 @@ import argparse
 import json
 import os
 import statistics
-import subprocess
 import sys
 
 import numpy as np
@@ -28,32 +27,15 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
+from measure import HBM_BYTES_PER_S, card, mean_ms  # noqa: E402
 from oracle.smplx_oracle import SmplxRestatement, forward_poses  # noqa: E402
 from pantomatrix_b200 import ops  # noqa: E402
 from pantomatrix_b200.body_model import ALL_JOINTS, SmplxBodyModel  # noqa: E402
 from pantomatrix_b200.emage_audio import engine  # noqa: E402
 from synthetic_models import SMPLX_FULL_VERTS, smplx_arrays  # noqa: E402
 
-PEAK_TC, PEAK_F32, PEAK_BW = 989e12, 67e12, 3.35e12
+PEAK_TC, PEAK_F32 = 989e12, 67e12
 MMAS = {"fp16x3": 3, "bf16x6": 6, "fp32": 1}
-
-
-def card():
-    """Name, power limit and max SM clock of the device the run uses (selected by UUID: a host may hold cards set to
-    different power limits)."""
-    q = ["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"]
-    out = subprocess.run(q + [f"--id=GPU-{torch.cuda.get_device_properties(0).uuid}"], capture_output=True, text=True)
-    return {"name": torch.cuda.get_device_name(0), "name_power_limit_max_sm_clock": out.stdout.strip() or None}
-
-
-def timed(fn, iters):
-    s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    s.record()
-    for _ in range(iters):
-        fn()
-    e.record()
-    e.synchronize()
-    return s.elapsed_time(e) / iters * 1e-3
 
 
 def main():
@@ -100,7 +82,7 @@ def main():
     times = {k: [] for k in arms}
     for _ in range(args.reps):
         for k, (fn, iters) in arms.items():
-            times[k].append(timed(fn, iters))
+            times[k].append(mean_ms(fn, iters) * 1e-3)
     med = {k: statistics.median(v) for k, v in times.items()}
     spread = {k: (min(v), max(v)) for k, v in times.items()}
     # the GEMM in the other engine precisions (same operand format as each precision's FK output)
@@ -109,7 +91,7 @@ def main():
         fk()
         gemm()
         torch.cuda.synchronize()
-        med["gemm_" + p] = statistics.median(timed(gemm, 3 if p == "fp32" else 10) for _ in range(3))
+        med["gemm_" + p] = statistics.median(mean_ms(gemm, 3 if p == "fp32" else 10) * 1e-3 for _ in range(3))
     engine.set_precision("fp16x3")
     flop = 2.0 * rows * 886 * 3 * nv
     res = {
@@ -123,7 +105,7 @@ def main():
         "gemm_share_of_peak": {p: flop / med["gemm_" + p] / (PEAK_F32 if p == "fp32" else PEAK_TC) for p in MMAS},
         "gemm_mmas_per_product": MMAS,
         "skin_gb_per_s": 24.0 * rows * nv / med["skin"] / 1e9,
-        "skin_share_of_hbm": 24.0 * rows * nv / med["skin"] / PEAK_BW,
+        "skin_share_of_hbm": 24.0 * rows * nv / med["skin"] / HBM_BYTES_PER_S,
     }
     with open(args.out, "w") as fh:
         json.dump(res, fh, indent=1)

@@ -1,7 +1,8 @@
 """Microbenchmark of pm_tapgemm_tc on the EMAGE shapes (warm L2, CUDA events around CUDA-graph replays).
     python tools/bench_gemm.py [shape-substring] [fp16]      # fp16: two fp16 planes (the default engine) only
 Each shape is timed with the N tile chosen automatically ("auto", the time the engine sees) and forced to 64 and to
-128 columns (all three give bit-identical results)."""
+128 columns (all three give bit-identical results).  The first line printed is the card record."""
+import json
 import math
 import os
 import sys
@@ -10,6 +11,7 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+from measure import card, graph_us  # noqa: E402
 from pantomatrix_b200 import ops  # noqa: E402
 
 SHAPES = [  # name, batch, rows, cin, cout, taps, pad
@@ -40,6 +42,7 @@ def main():
     fp16 = len(sys.argv) > 2 and sys.argv[2] == "fp16"
     if fp16:
         ops.set_plane_format("fp16")
+    print("card", json.dumps(card()))
     print(f"plane format {ops.plane_format()}")
     print(f"{'shape':34s} {'ns':>2s} {'out':>4s} {'us':>9s} {'TFLOP/s(alg)':>13s} {'bf16-equiv':>10s} "
           f"{'us BN=64':>9s} {'us BN=128':>9s}")
@@ -58,30 +61,14 @@ def main():
                 kw = dict(rows_out=rows_out, pad=pad, act=ops.ACT_RELU, out_nsplit=ns if out_mode == "f+p" else 0)
                 out = torch.empty(b, rows_out, cout, device="cuda")
                 kw["out"] = out
-                us = {tile: _time(a, pw, bias, tile, kw) for tile in (0, 64, 128) if tile != 128 or pw.w_rows % 128 == 0}
+                # 20 back-to-back launches replayed as a graph: GPU time, not Python / ctypes / descriptor-encode time
+                us = {tile: graph_us(lambda: ops.tapgemm_tc(a, pw, bias, tile=tile, **kw))[0]
+                      for tile in (0, 64, 128) if tile != 128 or pw.w_rows % 128 == 0}
                 fl = 2.0 * b * rows_out * cout * cin * taps
                 mult = {1: 1, 2: 3, 3: 6}[ns]          # tensor-core products per fp32 product
                 print(f"{name:34s} {ns:2d} {out_mode:>4s} {us[0]:9.1f} {fl / us[0] / 1e6:13.1f} {fl * mult / us[0] / 1e6:10.1f} "
                       f"{us[64]:9.1f} {us.get(128, float('nan')):9.1f}")
 
-
-def _time(a, pw, bias, tile, kw):
-    for _ in range(3):
-        ops.tapgemm_tc(a, pw, bias, tile=tile, **kw)
-    torch.cuda.synchronize()
-    graph = torch.cuda.CUDAGraph()          # 20 back-to-back launches replayed as a graph: GPU time,
-    with torch.cuda.graph(graph):           # not Python / ctypes / descriptor-encode time
-        for _ in range(20):
-            ops.tapgemm_tc(a, pw, bias, tile=tile, **kw)
-    graph.replay()
-    s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    torch.cuda.synchronize()
-    s.record()
-    for _ in range(3):
-        graph.replay()
-    e.record()
-    torch.cuda.synchronize()
-    return s.elapsed_time(e) / 60 * 1e3
 
 if __name__ == "__main__":
     main()

@@ -1,5 +1,6 @@
 """Throughput of the CaMN (batch 64) and DisCo (batch 32) paths, BASELINE configs[2], [3]: emitted 15-fps frames per
-second for 10 s clips, CUDA-event timed (eager launches), next to the CPU oracle on a bounded sample.  JSON lines."""
+second for 10 s clips, CUDA-event timed (eager launches), next to the CPU oracle on a bounded sample.  JSON lines, each
+with the card record."""
 import json
 import os
 import sys
@@ -14,10 +15,12 @@ from synthetic_models import build_lstm_product  # noqa: E402
 from oracle import lstm_oracle as L  # noqa: E402
 from oracle.weights import make_lstm_checkpoint, synth_audio  # noqa: E402
 from pantomatrix_b200.emage_audio import engine  # noqa: E402
+from measure import card, mean_ms  # noqa: E402
 
 
 def main():
     torch.set_num_threads(min(16, os.cpu_count()))
+    dev = card()
     for kind, bs in (("camn", 64), ("disco", 32)):
         model = build_lstm_product(kind)
         audio = torch.from_numpy(synth_audio(bs, 160000, 7)).cuda()
@@ -25,13 +28,7 @@ def main():
         for _ in range(3):
             out = model(audio, spk)
         torch.cuda.synchronize()
-        s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        s.record()
-        for _ in range(5):
-            out = model(audio, spk)
-        e.record()
-        torch.cuda.synchronize()
-        ms = s.elapsed_time(e) / 5
+        ms = mean_ms(lambda: model(audio, spk), 5)
         frames = bs * out["motion"].shape[1]
         sd, cfg = make_lstm_checkpoint(kind, 0)
         a8 = torch.from_numpy(synth_audio(8, 160000, 7))
@@ -41,7 +38,7 @@ def main():
             t0 = time.perf_counter()
             fwd(sd, cfg, a8, torch.zeros(8, 1, dtype=torch.long))
             cpu_s = time.perf_counter() - t0
-        print(json.dumps({"model": kind, "batch": bs, "frames_per_clip": int(out["motion"].shape[1]), "precision": engine.get_precision(),
+        print(json.dumps({"card": dev, "model": kind, "batch": bs, "frames_per_clip": int(out["motion"].shape[1]), "precision": engine.get_precision(),
                           "ms_per_batch": ms, "frames_per_s_15fps": frames / ms * 1e3,
                           "cpu_oracle_frames_per_s": 8 * out["motion"].shape[1] / cpu_s, "cpu_threads": torch.get_num_threads()}))
 

@@ -7,7 +7,8 @@
   e2e       CaMN at batch 64 from pinned 48 kHz int16 stereo: CapturedLstmPipeline(input_rate=48000, input_channels=2,
             input_dtype=int16) against the host reader's resample_poly (audio_io.load_audio's host path) followed by
             eager forward().  Same events, so the host resampling is inside the timed span.
-  device    torch.cuda.get_device_name and nvidia-smi's name / power.limit, read in the same run.
+  device    measure.card(): the name, power limit and max SM clock of the card the run uses, read before and after
+            (device_after) in the same run.
 Medians over --steps; frames are 15-fps output frames.  Writes OUT_DIR/lstm_pipeline.json and prints it."""
 import argparse
 import json
@@ -17,27 +18,9 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tools"))
+from measure import alternate, card  # noqa: E402
 SECONDS = 10
-
-
-def _timed(arms, steps):
-    """{name: fn}: every step runs each arm once, in turn, after an L2 flush; returns medians in ms."""
-    import torch
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")          # > the 50 MB L2
-    for fn in arms.values():
-        fn()
-    torch.cuda.synchronize()
-    times = {k: [] for k in arms}
-    for i in range(steps):
-        for k, fn in arms.items():
-            flush.fill_(i & 0xFF)
-            s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            s.record()
-            fn()
-            e.record()
-            torch.cuda.synchronize()
-            times[k].append(s.elapsed_time(e))
-    return {k: sorted(v)[len(v) // 2] for k, v in times.items()}, times
+FLUSH = 256 << 20                  # > the 50 MB L2
 
 
 def step_arms(steps):
@@ -55,7 +38,8 @@ def step_arms(steps):
             audio = torch.from_numpy(synth_audio(bs, n, 7)).cuda()
             spk = torch.zeros(bs, 1, dtype=torch.long, device="cuda")
             pipe = CapturedLstmPipeline(model, bs, n)
-            med, runs = _timed({"eager": lambda: model(audio, spk), "captured": lambda: pipe(audio, spk)}, steps)
+            med, runs = alternate({"eager": lambda: model(audio, spk), "captured": lambda: pipe(audio, spk)}, steps,
+                                  flush=FLUSH, clock="events")
             res[f"{kind} batch {bs}"] = {
                 "eager_ms": med["eager"], "captured_ms": med["captured"], "speedup": med["eager"] / med["captured"],
                 "eager_frames_per_s": bs * t / med["eager"] * 1e3, "captured_frames_per_s": bs * t / med["captured"] * 1e3,
@@ -85,8 +69,8 @@ def e2e(steps, bs=64):
         staging.copy_(torch.from_numpy(_host_front_end(pcm, 48000)))
         model(staging.cuda(non_blocking=True), spk)
 
-    med, runs = _timed({"captured_48k_int16_stereo": lambda: pipe(pinned, spk), "host_resample_then_eager": host_then_eager},
-                       steps)
+    med, runs = alternate({"captured_48k_int16_stereo": lambda: pipe(pinned, spk),
+                           "host_resample_then_eager": host_then_eager}, steps, flush=FLUSH, clock="events")
     return {"model": "camn", "batch": bs, **{f"{k}_ms": v for k, v in med.items()},
             **{f"{k}_frames_per_s": bs * t / v * 1e3 for k, v in med.items()},
             "speedup": med["host_resample_then_eager"] / med["captured_48k_int16_stereo"],
@@ -101,13 +85,12 @@ def main():
     import torch
     if not torch.cuda.is_available():
         raise SystemExit("bench_lstm_pipeline.py needs a CUDA device")
-    from bench_audio_frontend import device_info
     from pantomatrix_b200.emage_audio import engine
     os.makedirs(args.out_dir, exist_ok=True)
-    res = {"device": device_info(), "precision": engine.get_precision(), "seconds_per_clip": SECONDS,
+    res = {"device": card(), "precision": engine.get_precision(), "seconds_per_clip": SECONDS,
            "timer": "CUDA events around each step, 256 MB L2 flush before it (outside the events), arms alternating, medians",
            "step": step_arms(args.steps), "e2e": e2e(max(3, args.steps // 4))}
-    res["device_after"] = device_info()
+    res["device_after"] = card()
     with open(os.path.join(args.out_dir, "lstm_pipeline.json"), "w") as f:
         json.dump(res, f, indent=1)
     print(json.dumps(res))

@@ -22,7 +22,6 @@ import os
 import platform
 import shutil
 import statistics
-import subprocess
 import sys
 import tempfile
 import time
@@ -34,21 +33,13 @@ from PIL import Image
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
+from measure import HBM_BYTES_PER_S, card, event_ms  # noqa: E402
 from oracle.weights import synth_audio  # noqa: E402
 from pantomatrix_b200 import _lib, ops, png  # noqa: E402
 from pantomatrix_b200.body_model import SmplxBodyModel  # noqa: E402
 from pantomatrix_b200.pipeline import generate  # noqa: E402
 from pantomatrix_b200.render import MeshRenderer  # noqa: E402
 from synthetic_models import build_lstm_product, build_product, smplx_surface_arrays  # noqa: E402
-
-PEAK_BW = 3.35e12
-
-
-def card():
-    q = ["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"]
-    out = subprocess.run(q + [f"--id=GPU-{torch.cuda.get_device_properties(0).uuid}"], capture_output=True, text=True)
-    return {"name": torch.cuda.get_device_name(0), "name_power_limit_max_sm_clock": out.stdout.strip() or None}
-
 
 def host_cpu():
     model = None
@@ -59,15 +50,6 @@ def host_cpu():
         pass
     return {"model": model or f"not reported in /proc/cpuinfo ({platform.machine()})", "threads": os.cpu_count(),
             "pillow_threads_used": 1}
-
-
-def event_ms(fn):
-    s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    s.record()
-    fn()
-    e.record()
-    e.synchronize()
-    return s.elapsed_time(e)
 
 
 def stages(frames, data, nbytes, reps):
@@ -124,7 +106,7 @@ def arm(frames, reps, pillow_frames):
             "encode_ms_per_frame": med / n, "frames_per_s": n / (med * 1e-3),
             "bytes_per_frame_mean": float(sizes.mean()), "bytes_per_frame_min": int(sizes.min()),
             "bytes_per_frame_max": int(sizes.max()), "slot_bytes": int(data.shape[1]),
-            "least_bytes": least, "share_of_3.35TBps": least / (med * 1e-3) / PEAK_BW,
+            "least_bytes": least, "share_of_3.35TBps": least / (med * 1e-3) / HBM_BYTES_PER_S,
             "stage_ms_median": stages(frames, data, nbytes, reps),
             "pillow_host": pillow(frames, pillow_frames) if pillow_frames else "not measured"}
 

@@ -24,7 +24,6 @@ import argparse
 import json
 import os
 import statistics
-import subprocess
 import sys
 import time
 
@@ -33,6 +32,7 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
+from measure import HBM_BYTES_PER_S, card, event_ms  # noqa: E402
 from oracle.weights import synth_audio  # noqa: E402
 from pantomatrix_b200 import ops  # noqa: E402
 from pantomatrix_b200.body_model import ALL_JOINTS, SmplxBodyModel  # noqa: E402
@@ -41,23 +41,7 @@ from pantomatrix_b200.render import CHUNK, FACE_VIEW, BODY_VIEW, H, JAW_ONLY, VI
 from synthetic_models import (SMPLX_FULL_VERTS, build_lstm_product, build_product, smplx_arrays,  # noqa: E402
                               smplx_surface_arrays)
 
-PEAK_BW = 3.35e12
 SOUP_BUDGET_S = 5.0       # the soup's 8-clip run is skipped when one clip already takes longer than this
-
-
-def card():
-    q = ["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"]
-    out = subprocess.run(q + [f"--id=GPU-{torch.cuda.get_device_properties(0).uuid}"], capture_output=True, text=True)
-    return {"name": torch.cuda.get_device_name(0), "name_power_limit_max_sm_clock": out.stdout.strip() or None}
-
-
-def event_ms(fn):
-    s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    s.record()
-    fn()
-    e.record()
-    e.synchronize()
-    return s.elapsed_time(e)
 
 
 def kernels(r, verts, views, reps):
@@ -83,7 +67,7 @@ def kernels(r, verts, views, reps):
     for k, t in times.items():
         med = statistics.median(t)
         res[k] = {"ms_per_chunk_median": med, "ms_per_chunk_max": max(t), "least_bytes_per_chunk": least[k],
-                  "share_of_3.35TBps": least[k] / (med * 1e-3) / PEAK_BW}
+                  "share_of_3.35TBps": least[k] / (med * 1e-3) / HBM_BYTES_PER_S}
     return res
 
 

@@ -6,8 +6,10 @@
 Stamps, one set per CTA (= per output tile), written by the first consumer warp (cycles of the CTA's SM clock, relative
 to kernel entry of that CTA): prologue done, first operand stage landed, all MMAs issued, accumulators complete, this
 warp's epilogue issued, all consumer warps done.  The launch uses the automatically chosen N tile.  The launch-to-launch
-period (CUDA events around a replayed graph of 20 launches) minus the in-kernel span is launch / drain / tail cost."""
+period (CUDA events around a replayed graph of 20 launches) minus the in-kernel span is launch / drain / tail cost.
+The first line printed is the card record."""
 import ctypes
+import json
 import math
 import os
 import sys
@@ -17,6 +19,7 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+from measure import card, graph_us  # noqa: E402
 from pantomatrix_b200 import _lib, ops  # noqa: E402
 
 SHAPES = [  # name, batch, rows, cin, cout, taps, pad, fp32 residual
@@ -41,6 +44,7 @@ def main():
         sys.exit("not an instrumented build: set PM_EMAGE_LIB to the -DPM_TC_TIMING variant")
     lib.pm_tc_timing_read.argtypes = [ctypes.c_void_p]
     buf = np.zeros((4096, 8), dtype=np.uint64)
+    print("card", json.dumps(card()))
     print(f"{'shape':28s} ns out  CTAs | cycles after entry (mean over CTAs): " + " | ".join(NAMES) +
           " || span max (cyc) | period us | span us @period clock")
     only = sys.argv[1] if len(sys.argv) > 1 else ""
@@ -65,24 +69,11 @@ def main():
                     kw["want_f32"] = False
                 else:
                     kw["out"] = torch.empty(b, rows_out, cout, device="cuda")
-                for _ in range(3):
-                    ops.tapgemm_tc(a, pw, bias, **kw)
-                graph = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(graph):
-                    for _ in range(20):
-                        ops.tapgemm_tc(a, pw, bias, **kw)
-                graph.replay()
-                s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                torch.cuda.synchronize()
-                s.record()
-                for _ in range(3):
-                    graph.replay()
-                e.record()
-                torch.cuda.synchronize()
-                period_us = s.elapsed_time(e) / 60 * 1e3
+                period_us, graph = graph_us(lambda: ops.tapgemm_tc(a, pw, bias, **kw))
                 assert lib.pm_tc_timing_reset() == 0
                 graph.replay()                                  # stamps of the last (warm, back-to-back) launch survive
                 assert lib.pm_tc_timing_read(buf.ctypes.data) == 0
+                del graph                                       # free its memory pool before the next shape's capture
                 st = buf[buf[:, 0] != 0].astype(np.int64)
                 d = st[:, 1:7] - st[:, :1]
                 span = d[:, 5]
