@@ -4,6 +4,7 @@
     python examples/camn_disco_demo.py --model camn --checkpoint /path/to/camn_audio --audio_folder ./wavs
     python examples/camn_disco_demo.py --model disco --synthetic --audio_folder ./wavs
     python examples/camn_disco_demo.py ... --smplx SMPLX_NEUTRAL_2020.npz --render   # + <name>_frames/frame_%05d.png
+    python examples/camn_disco_demo.py ... --smplx SMPLX_NEUTRAL_2020.npz --video    # + <name>_output.mp4
 
 These models emit the upper body + hands only and no translation; like the reference demos the npz writer places the
 pelvis with the SMPL-X body model: pass the model file with --smplx SMPLX_NEUTRAL_2020.npz (the translation the
@@ -11,7 +12,9 @@ reference writer derives), or --trans-zero to write zeros instead.
 `--render` (needs --smplx) draws the reference demos' SMPL-X body view (fast_render.py render_one_sequence_no_gt: one
 480 x 720 view, whole seconds at 30 fps) of the motion upsampled to 30 fps as the npz stores it, on the GPU, with the
 translation the npz receives, and writes the frames as PNG files next to each npz, encoded on the GPU
-(pantomatrix_b200.png); video encoding is left to the user (e.g. ffmpeg -framerate 30 -i frame_%05d.png)."""
+(pantomatrix_b200.png).  `--video` (needs --smplx) encodes the same frames as H.264 on the GPU (pantomatrix_b200.video)
+and writes <npz base>.mp4 (30 fps, silent) beside each npz; to add the audio track:
+ffmpeg -i video.mp4 -i audio.wav -map 0:v -map 1:a -c:v copy -shortest out.mp4"""
 import argparse
 import os
 import sys
@@ -45,18 +48,21 @@ def main():
     ap.add_argument("--trans-zero", action="store_true")
     ap.add_argument("--smplx", default=None, metavar="PATH", help="SMPL-X model file (SMPLX_NEUTRAL_2020.npz)")
     ap.add_argument("--render", action="store_true")
+    ap.add_argument("--video", action="store_true", help="write <npz base>.mp4 (needs --smplx)")
     args = ap.parse_args()
     if not args.trans_zero and args.smplx is None:
         ap.error("the npz needs a pelvis translation: pass --smplx SMPLX_NEUTRAL_2020.npz, or --trans-zero to write zeros")
     if args.render and args.smplx is None:
         ap.error("--render needs --smplx SMPLX_NEUTRAL_2020.npz")
+    if args.video and args.smplx is None:
+        ap.error("--video needs --smplx SMPLX_NEUTRAL_2020.npz")
     device = torch.device("cuda")
     body_model = renderer = None
     if args.smplx is not None:
         from pantomatrix_b200.body_model import SmplxBodyModel
         smplx_model = SmplxBodyModel.from_npz(args.smplx, device)
         body_model = None if args.trans_zero else smplx_model
-        if args.render:
+        if args.render or args.video:
             from pantomatrix_b200.render import MeshRenderer
             renderer = MeshRenderer(smplx_model)
     if args.synthetic:
@@ -80,8 +86,12 @@ def main():
             # the npz's translation: the writer's pelvis placement (betas zero), or zeros under --trans-zero
             pelvis = np.zeros(3, np.float32) if trans is not None else pelvis_translation(body_model, np.zeros(300, np.float32))
             tr = torch.as_tensor(pelvis, device=device).expand(1, t, 3)
-            write_frames(renderer.render_body(aa.reshape(1, t, -1), tr, upsample=30 // fps)[0],
-                         os.path.splitext(npz)[0] + "_frames")
+            drawn = renderer.render_body(aa.reshape(1, t, -1), tr, upsample=30 // fps)[0]
+            if args.render:
+                write_frames(drawn, os.path.splitext(npz)[0] + "_frames")
+            if args.video:
+                from pantomatrix_b200 import video
+                video.write_mp4(drawn, os.path.splitext(npz)[0] + ".mp4", fps=30)
         frames += t
     print(f"generate total {frames / fps:.2f} seconds motion in {time.time() - t0:.2f} seconds, saved in {args.save_folder}")
 

@@ -4,10 +4,13 @@
     python examples/emage_audio_demo.py --checkpoint /path/to/emage_audio --audio_folder ./wavs --save_folder ./out
     python examples/emage_audio_demo.py --synthetic --audio_folder ./wavs            # seeded random weights (no network)
     python examples/emage_audio_demo.py ... --smplx SMPLX_NEUTRAL_2020.npz --render   # + <name>_frames/frame_%05d.png
+    python examples/emage_audio_demo.py ... --smplx SMPLX_NEUTRAL_2020.npz --video    # + <name>_output.mp4
 
 `--render` draws the reference demo's two-view SMPL-X frames (fast_render.py render_one_sequence_with_face: face
 close-up left, body right, whole seconds at 30 fps) on the GPU and writes them as PNG files next to each npz,
-encoded on the GPU (pantomatrix_b200.png); video encoding is left to the user (e.g. ffmpeg -framerate 30 -i frame_%05d.png).
+encoded on the GPU (pantomatrix_b200.png).  `--video` (needs --smplx) encodes the same frames as H.264 on the GPU
+(pantomatrix_b200.video) and writes <npz base>.mp4 (30 fps, silent) beside each npz; to add the audio track:
+ffmpeg -i video.mp4 -i audio.wav -map 0:v -map 1:a -c:v copy -shortest out.mp4
 `--checkpoint` is a local copy of the Hugging Face repo layout the reference downloads (config.json +
 model.safetensors at the top level, VQ models under emage_vq/{face,upper,lower,hands,global}).
 """
@@ -52,18 +55,21 @@ def main():
     ap.add_argument("--save_folder", default="./examples/motion")
     ap.add_argument("--checkpoint", default=None)
     ap.add_argument("--synthetic", action="store_true")
-    ap.add_argument("--smplx", default=None, help="SMPLX_NEUTRAL_2020.npz (needed by --render)")
+    ap.add_argument("--smplx", default=None, help="SMPLX_NEUTRAL_2020.npz (needed by --render and --video)")
     ap.add_argument("--render", action="store_true")
+    ap.add_argument("--video", action="store_true", help="write <npz base>.mp4 (needs --smplx)")
     args = ap.parse_args()
     if not args.synthetic and not args.checkpoint:
         ap.error("give --checkpoint DIR or --synthetic")
     if args.render and not args.smplx:
         ap.error("--render needs --smplx SMPLX_NEUTRAL_2020.npz")
+    if args.video and not args.smplx:
+        ap.error("--video needs --smplx SMPLX_NEUTRAL_2020.npz")
     os.makedirs(args.save_folder, exist_ok=True)
     device = torch.device("cuda")                      # no CPU fallback by design
     model, motion_vq = load_models(args, device)
     renderer = None
-    if args.render:
+    if args.render or args.video:
         from pantomatrix_b200.body_model import SmplxBodyModel
         from pantomatrix_b200.render import MeshRenderer
         renderer = MeshRenderer(SmplxBodyModel.from_npz(args.smplx, device))
@@ -79,8 +85,12 @@ def main():
                          expressions=pred["expression"].cpu().numpy().reshape(t, -1),
                          trans=pred["trans"].cpu().numpy().reshape(t, -1))
         if renderer is not None:
-            write_frames(renderer.render_sequence(pred["motion_axis_angle"], pred["expression"], pred["trans"])[0],
-                         os.path.splitext(npz)[0] + "_frames")
+            drawn = renderer.render_sequence(pred["motion_axis_angle"], pred["expression"], pred["trans"])[0]
+            if args.render:
+                write_frames(drawn, os.path.splitext(npz)[0] + "_frames")
+            if args.video:
+                from pantomatrix_b200 import video
+                video.write_mp4(drawn, os.path.splitext(npz)[0] + ".mp4", fps=30)
         frames += t
     print(f"generate total {frames / fps:.2f} seconds motion in {time.time() - t0:.2f} seconds")
 

@@ -348,6 +348,36 @@ int pm_png_emit(const unsigned char* frames, long long f_fs, int n_frames, int h
                 unsigned char* data, long long cap, void* stream);
 int pm_png_crc(int n_frames, int h, int w, unsigned char* data, long long cap, const long long* nbytes, void* stream);
 
+/* ---- H.264 encoding of RGB8 frames (pantomatrix_b200/video.py, DESIGN.md section 12) ----------------------------
+ * n_frames frames of h rows x w pixels of RGB8 (h, w multiples of 16; at most 36864 macroblocks and 543 per side,
+ * level 5.1), each dense, frame f at frames + f * f_fs and at index f mod clip_len of its clip.  Frame f becomes one
+ * sample in data + f * cap, by one rule:
+ *   colour: Y = ((66 R + 129 G + 25 B + 128) >> 8) + 16 per pixel; with Rs, Gs, Bs the sums over each 2x2 block,
+ *     Cb = ((-38 Rs - 74 Gs + 112 Bs + 512) >> 10) + 128, Cr = ((112 Rs - 94 Gs - 18 Bs + 512) >> 10) + 128 (>> floors);
+ *   stream: Constrained Baseline (profile 66, constraint_set0/1), level 5.1, CAVLC, 4:2:0; SPS and PPS are built on
+ *     the host (video.sps / video.pps);
+ *   picture: IDR, nal_ref_idc 3, idr_pic_id = (f mod clip_len) mod 2; one I slice (slice_type 7) per macroblock row:
+ *     first_mb_in_slice = row w / 16, frame_num 0, slice_qp_delta = qp - 26, disable_deblocking_filter_idc 1;
+ *   macroblock: Intra16x16 with mb_qp_delta 0, chroma DC; luma DC (left column mean, 128 in column 0) or, when the left
+ *     macroblock exists and its SAD against the source Y is strictly lower, Horizontal.  qbits = 15 + qp / 6,
+ *     f = 2^qbits / 3, MF the standard table by position class; AC level = sgn(W) ((|W| MF + f) >> qbits); luma DC
+ *     D = H4 WD H4, level = sgn(D) (((|D| >> 1) MF0 + 2 f) >> (qbits + 1)); chroma DC D = H2 WD H2, level =
+ *     sgn(D) ((|D| MF0 + 2 f) >> (qbits + 1)) at QPc (table 8-15, offset 0).  cbpLuma 15 if any AC level, else 0;
+ *     cbpChroma 2 if any chroma AC level, else 1 if any chroma DC level, else 0.  Reconstruction per 8.5 bit for bit;
+ *   I_PCM (mb_type 25, source samples) instead, when the Intra16x16 macroblock_layer() would pass 3200 bits or a level
+ *     would need level_prefix > 15;
+ *   framing: each slice one NAL unit with emulation prevention, prefixed by its length (4 bytes, big-endian).
+ * Bound: a slice has at most P = ceil((62 + 3200 w / 16 + 8) / 8) RBSP bytes and P / 2 emulation prevention bytes, so
+ *   slice_cap >= slice_bound = 4 + P + P / 2 and cap >= (h / 16) slice_bound.  Launch order on one stream:
+ *   pm_memset_async(data, 0, n_frames * cap), pm_h264_encode, pm_h264_gather.
+ * pm_h264_encode: one warp per (frame, row): the slice into scratch + (f h / 16 + row) slice_cap, its length prefix
+ *   included, and its byte count into slice_bytes.
+ * pm_h264_gather: one CTA per (frame, row): the slice copied to its offset in the frame's slot; nbytes[f] the sum. */
+int pm_h264_encode(const unsigned char* frames, long long f_fs, int n_frames, int clip_len, int h, int w, int qp,
+                   unsigned char* scratch, long long slice_cap, int* slice_bytes, void* stream);
+int pm_h264_gather(int n_frames, int h, int w, const unsigned char* scratch, long long slice_cap,
+                   const int* slice_bytes, unsigned char* data, long long cap, long long* nbytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

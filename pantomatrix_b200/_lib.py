@@ -58,6 +58,8 @@ SIGNATURES = {
     "pm_png_scan": [_i, _i, _i, _p, _p, _p, _ll, _p, _p],
     "pm_png_emit": [_p, _ll, _i, _i, _i, _p, _p, _ll, _p],
     "pm_png_crc": [_i, _i, _i, _p, _ll, _p, _p],
+    "pm_h264_encode": [_p, _ll, _i, _i, _i, _i, _i, _p, _ll, _p, _p],
+    "pm_h264_gather": [_i, _i, _i, _p, _ll, _p, _p, _ll, _p, _p],
 }
 
 _lib = None

@@ -704,6 +704,28 @@ def png_encode(frames, data, nbytes, row_bits, row_adler):
     _call("pm_png_crc", n, h, w, data.data_ptr(), cap, nbytes.data_ptr(), _stream())
 
 
+# ------------------------------------------------------------------------------------------------------
+# H.264 encoding
+# ------------------------------------------------------------------------------------------------------
+
+
+def h264_encode(frames, clip_len, qp, data, nbytes, scratch, sizes):
+    """The H.264 samples of frames (N, H, W, 3) uint8, each frame dense, any stride apart, frame i at index i % clip_len
+    of its clip, into the slots of data (N, cap) uint8 with their sizes in nbytes (N,) int64 (include/pm_emage.h
+    pm_h264_*).  scratch (N, H / 16, slice_cap) uint8 and sizes (N, H / 16) int32: workspace, one slice per row.  The
+    slots are cleared first by a memset (a memset node under graph capture), then two launches."""
+    _chk(frames, torch.uint8), _chk(data, torch.uint8), _chk(nbytes, torch.int64)
+    _chk(scratch, torch.uint8), _chk(sizes, torch.int32)
+    n, h, w, _ = frames.shape
+    assert data.is_contiguous() and nbytes.is_contiguous() and scratch.is_contiguous() and sizes.is_contiguous()
+    cap, fs, slice_cap = data.shape[1], frames.stride(0) if n > 1 else 3 * h * w, scratch.shape[2]
+    _lib.call("pm_memset_async", data.data_ptr(), 0, data.numel(), _stream())
+    _call("pm_h264_encode", frames.data_ptr(), fs, n, clip_len, h, w, qp, scratch.data_ptr(), slice_cap,
+          sizes.data_ptr(), _stream())
+    _call("pm_h264_gather", n, h, w, scratch.data_ptr(), slice_cap, sizes.data_ptr(), data.data_ptr(), cap,
+          nbytes.data_ptr(), _stream())
+
+
 def softmax2_mix(sel, c1, c2, out=None):
     """out[..., :] = softmax(sel[..., 0:2])[0] * c1 + [1] * c2 (out may be a column slice of a wider tensor)."""
     _chk(sel), _chk(c1), _chk(c2)
