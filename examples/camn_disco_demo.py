@@ -5,6 +5,7 @@
     python examples/camn_disco_demo.py --model disco --synthetic --audio_folder ./wavs
     python examples/camn_disco_demo.py ... --smplx SMPLX_NEUTRAL_2020.npz --render   # + <name>_frames/frame_%05d.png
     python examples/camn_disco_demo.py ... --smplx SMPLX_NEUTRAL_2020.npz --video    # + <name>_output.mp4
+    python examples/camn_disco_demo.py ... --smplx SMPLX_NEUTRAL_2020.npz --video --with-audio   # the mp4 with sound
 
 These models emit the upper body + hands only and no translation; like the reference demos the npz writer places the
 pelvis with the SMPL-X body model: pass the model file with --smplx SMPLX_NEUTRAL_2020.npz (the translation the
@@ -13,8 +14,9 @@ reference writer derives), or --trans-zero to write zeros instead.
 480 x 720 view, whole seconds at 30 fps) of the motion upsampled to 30 fps as the npz stores it, on the GPU, with the
 translation the npz receives, and writes the frames as PNG files next to each npz, encoded on the GPU
 (pantomatrix_b200.png).  `--video` (needs --smplx) encodes the same frames as H.264 on the GPU (pantomatrix_b200.video)
-and writes <npz base>.mp4 (30 fps, silent) beside each npz; to add the audio track:
-ffmpeg -i video.mp4 -i audio.wav -map 0:v -map 1:a -c:v copy -shortest out.mp4"""
+and writes <npz base>.mp4 (30 fps) beside each npz, silent unless `--with-audio` is given: that reads the WAV at its
+own rate and channel count and writes it into the file as a FLAC track encoded on the GPU (pantomatrix_b200.flac),
+trimmed to the video's length."""
 import argparse
 import os
 import sys
@@ -38,6 +40,13 @@ def write_frames(frames, folder):
     png.write_frames(frames, folder)
 
 
+def track(path, device):
+    """(samples on the GPU, rate) of a WAV file for video.write_mp4's audio track (audio_io.track_samples)."""
+    from pantomatrix_b200.audio_io import read_pcm, track_samples
+    pcm, rate = read_pcm(path)
+    return torch.from_numpy(np.ascontiguousarray(track_samples(pcm))).to(device), rate
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--model", choices=["camn", "disco"], default="camn")
@@ -49,6 +58,7 @@ def main():
     ap.add_argument("--smplx", default=None, metavar="PATH", help="SMPL-X model file (SMPLX_NEUTRAL_2020.npz)")
     ap.add_argument("--render", action="store_true")
     ap.add_argument("--video", action="store_true", help="write <npz base>.mp4 (needs --smplx)")
+    ap.add_argument("--with-audio", action="store_true", help="put the WAV's sound in the --video file")
     args = ap.parse_args()
     if not args.trans_zero and args.smplx is None:
         ap.error("the npz needs a pelvis translation: pass --smplx SMPLX_NEUTRAL_2020.npz, or --trans-zero to write zeros")
@@ -56,6 +66,8 @@ def main():
         ap.error("--render needs --smplx SMPLX_NEUTRAL_2020.npz")
     if args.video and args.smplx is None:
         ap.error("--video needs --smplx SMPLX_NEUTRAL_2020.npz")
+    if args.with_audio and not args.video:
+        ap.error("--with-audio needs --video")
     device = torch.device("cuda")
     body_model = renderer = None
     if args.smplx is not None:
@@ -91,7 +103,8 @@ def main():
                 write_frames(drawn, os.path.splitext(npz)[0] + "_frames")
             if args.video:
                 from pantomatrix_b200 import video
-                video.write_mp4(drawn, os.path.splitext(npz)[0] + ".mp4", fps=30)
+                video.write_mp4(drawn, os.path.splitext(npz)[0] + ".mp4", fps=30,
+                                audio=track(os.path.join(args.audio_folder, name), device) if args.with_audio else None)
         frames += t
     print(f"generate total {frames / fps:.2f} seconds motion in {time.time() - t0:.2f} seconds, saved in {args.save_folder}")
 

@@ -5,12 +5,14 @@
     python examples/emage_audio_demo.py --synthetic --audio_folder ./wavs            # seeded random weights (no network)
     python examples/emage_audio_demo.py ... --smplx SMPLX_NEUTRAL_2020.npz --render   # + <name>_frames/frame_%05d.png
     python examples/emage_audio_demo.py ... --smplx SMPLX_NEUTRAL_2020.npz --video    # + <name>_output.mp4
+    python examples/emage_audio_demo.py ... --smplx SMPLX_NEUTRAL_2020.npz --video --with-audio   # the mp4 with sound
 
 `--render` draws the reference demo's two-view SMPL-X frames (fast_render.py render_one_sequence_with_face: face
 close-up left, body right, whole seconds at 30 fps) on the GPU and writes them as PNG files next to each npz,
 encoded on the GPU (pantomatrix_b200.png).  `--video` (needs --smplx) encodes the same frames as H.264 on the GPU
-(pantomatrix_b200.video) and writes <npz base>.mp4 (30 fps, silent) beside each npz; to add the audio track:
-ffmpeg -i video.mp4 -i audio.wav -map 0:v -map 1:a -c:v copy -shortest out.mp4
+(pantomatrix_b200.video) and writes <npz base>.mp4 (30 fps) beside each npz, silent unless `--with-audio` is given:
+that reads the WAV at its own rate and channel count and writes it into the file as a FLAC track encoded on the GPU
+(pantomatrix_b200.flac), trimmed to the video's length.
 `--checkpoint` is a local copy of the Hugging Face repo layout the reference downloads (config.json +
 model.safetensors at the top level, VQ models under emage_vq/{face,upper,lower,hands,global}).
 """
@@ -19,6 +21,7 @@ import os
 import sys
 import time
 
+import numpy as np
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -49,6 +52,13 @@ def write_frames(frames, folder):
     png.write_frames(frames, folder)
 
 
+def track(path, device):
+    """(samples on the GPU, rate) of a WAV file for video.write_mp4's audio track (audio_io.track_samples)."""
+    from pantomatrix_b200.audio_io import read_pcm, track_samples
+    pcm, rate = read_pcm(path)
+    return torch.from_numpy(np.ascontiguousarray(track_samples(pcm))).to(device), rate
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--audio_folder", default="./examples/audio")
@@ -58,6 +68,7 @@ def main():
     ap.add_argument("--smplx", default=None, help="SMPLX_NEUTRAL_2020.npz (needed by --render and --video)")
     ap.add_argument("--render", action="store_true")
     ap.add_argument("--video", action="store_true", help="write <npz base>.mp4 (needs --smplx)")
+    ap.add_argument("--with-audio", action="store_true", help="put the WAV's sound in the --video file")
     args = ap.parse_args()
     if not args.synthetic and not args.checkpoint:
         ap.error("give --checkpoint DIR or --synthetic")
@@ -65,6 +76,8 @@ def main():
         ap.error("--render needs --smplx SMPLX_NEUTRAL_2020.npz")
     if args.video and not args.smplx:
         ap.error("--video needs --smplx SMPLX_NEUTRAL_2020.npz")
+    if args.with_audio and not args.video:
+        ap.error("--with-audio needs --video")
     os.makedirs(args.save_folder, exist_ok=True)
     device = torch.device("cuda")                      # no CPU fallback by design
     model, motion_vq = load_models(args, device)
@@ -90,7 +103,8 @@ def main():
                 write_frames(drawn, os.path.splitext(npz)[0] + "_frames")
             if args.video:
                 from pantomatrix_b200 import video
-                video.write_mp4(drawn, os.path.splitext(npz)[0] + ".mp4", fps=30)
+                video.write_mp4(drawn, os.path.splitext(npz)[0] + ".mp4", fps=30,
+                                audio=track(os.path.join(args.audio_folder, name), device) if args.with_audio else None)
         frames += t
     print(f"generate total {frames / fps:.2f} seconds motion in {time.time() - t0:.2f} seconds")
 

@@ -378,6 +378,38 @@ int pm_h264_encode(const unsigned char* frames, long long f_fs, int n_frames, in
 int pm_h264_gather(int n_frames, int h, int w, const unsigned char* scratch, long long slice_cap,
                    const int* slice_bytes, unsigned char* data, long long cap, long long* nbytes, void* stream);
 
+/* ---- FLAC encoding of recorded samples (pantomatrix_b200/flac.py, DESIGN.md section 13) ----------------------------
+ * batch clips of n >= 1 samples x channels (1..8), clip b at pcm + b * clip_stride samples, each dense (n, channels):
+ * int16 at bps 16, or int32 holding -2^23 .. 2^23 - 1 at bps 24.  Frame k of clip b (samples 4096 k onward, the last
+ * frame may be shorter; F = ceil(n / 4096) per clip) becomes one FLAC frame in data + (b F + k) * cap, by one rule:
+ *   header: sync 0xFFF8; block-size code 1100 (4096) or 0111 with bs - 1 in 16 bits; rate code 0100..1010 for 8, 16,
+ *     22.05, 24, 32, 44.1 and 48 kHz, else 1100 (8-bit kHz) for a whole number of kHz below 256, else 1101 (16-bit
+ *     Hz); channel assignment; sample size 100 (16) or 110 (24); frame number k UTF-8 coded; CRC-8 (poly 0x07).  At
+ *     most 13 bytes (k < 2^21);
+ *   subframes, per channel (no wasted bits, no LPC): the fewest bits of CONSTANT (all samples equal), FIXED order
+ *     0..4 (order <= bs) and VERBATIM, ties to that order, then the lower order, partition order and parameter.
+ *     FIXED residuals e are coded as u = 2e (e >= 0) or -2e - 1 by partitioned Rice: partition order p in 0..8 with
+ *     2^p dividing bs and bs >> p >= order (partition 0 holds bs >> p minus order residuals); each partition's k is
+ *     the one with the fewest count (k + 1) + sum(u >> k) bits; method 00 (4-bit k <= 14) unless 01 (5-bit k <= 30)
+ *     is strictly smaller; no escape codes;
+ *   stereo: the best subframes of L, R, S = L - R (at bps + 1) and M = (L + R) >> 1 (arithmetic, at bps); the pair
+ *     with the fewest bits of independent (L R), left/side (L S), side/right (S R) and mid/side (M S), ties in that
+ *     order.  Other channel counts are independent;
+ *   end: zero bits to a byte boundary, CRC-16 (poly 0x8005) of the whole frame, big-endian.
+ * Bound: the minimum never passes independent VERBATIM, so a frame of bs samples has at most
+ *   18 + ceil(channels (8 + bps bs) / 8) bytes; cap >= that bound for bs = min(n, 4096), cap a multiple of 4, data
+ *   4-byte aligned.  An int32 frame holding a sample outside -2^23 .. 2^23 - 1 is not coded: nbytes = -1, slot zero.
+ * Workspace: rec, 66 int32 per (clip, frame, candidate), candidates = 4 (L, R, S, M) for stereo, else channels.
+ * Launch order on one stream: pm_memset_async(data, 0, batch F cap), pm_flac_analyse, pm_flac_emit.
+ * pm_flac_analyse: one CTA per (clip, frame, candidate): the candidate's best subframe (bits, type, order, p, method
+ *   and the partitions' k) into its record.
+ * pm_flac_emit: one CTA per (clip, frame): the assignment, the header, each subframe ORed into the slot at its bit
+ *   offset (a block scan of the code lengths), the CRC-16, and nbytes. */
+int pm_flac_analyse(const void* pcm, long long clip_stride, int batch, int n, int channels, int bps, int* rec,
+                    void* stream);
+int pm_flac_emit(const void* pcm, long long clip_stride, int batch, int n, int channels, int bps, int rate,
+                 const int* rec, unsigned char* data, long long cap, long long* nbytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

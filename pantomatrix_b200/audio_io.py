@@ -61,6 +61,16 @@ def read_pcm(path):
     return x.reshape(-1, channels), rate
 
 
+def track_samples(x):
+    """FLAC track samples (pantomatrix_b200/flac.py) of read_pcm's output: 16-bit PCM stays int16 (coded at 16 bits);
+    every other format becomes int32 coded at 24 bits, clamp(round-half-even(x 2^23)) to -2^23 .. 2^23 - 1, which is
+    exact for 8- and 24-bit sources."""
+    if x.dtype == np.int16:
+        return x
+    v = np.rint(x.astype(np.float64) * float(1 << 23))
+    return np.clip(v, -(1 << 23), (1 << 23) - 1).astype(np.int32)
+
+
 def _read_wav(path):
     """(float32 samples (n, channels) in [-1, 1], rate)."""
     x, rate = read_pcm(path)

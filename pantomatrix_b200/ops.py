@@ -726,6 +726,27 @@ def h264_encode(frames, clip_len, qp, data, nbytes, scratch, sizes):
           nbytes.data_ptr(), _stream())
 
 
+# ------------------------------------------------------------------------------------------------------
+# FLAC encoding
+# ------------------------------------------------------------------------------------------------------
+
+
+def flac_encode(pcm, bps, rate, data, nbytes, rec):
+    """The FLAC frames of pcm (B, n, C) int16 (bps 16) or int32 (bps 24), each clip dense, clips any stride apart,
+    into the slots of data (B F, cap) uint8 with their sizes in nbytes (B F,) int64 (include/pm_emage.h pm_flac_*).
+    rec (B F K, 66) int32: workspace, one analysis record per (clip, frame, channel candidate).  The slots are cleared
+    first by a memset (a memset node under graph capture), then two launches."""
+    _chk(pcm, torch.int16 if bps == 16 else torch.int32), _chk(data, torch.uint8), _chk(nbytes, torch.int64)
+    _chk(rec, torch.int32)
+    b, n, c = pcm.shape
+    assert data.is_contiguous() and nbytes.is_contiguous() and rec.is_contiguous()
+    cs = pcm.stride(0) if b > 1 else n * c
+    _lib.call("pm_memset_async", data.data_ptr(), 0, data.numel(), _stream())
+    _call("pm_flac_analyse", pcm.data_ptr(), cs, b, n, c, bps, rec.data_ptr(), _stream())
+    _call("pm_flac_emit", pcm.data_ptr(), cs, b, n, c, bps, rate, rec.data_ptr(), data.data_ptr(), data.shape[1],
+          nbytes.data_ptr(), _stream())
+
+
 def softmax2_mix(sel, c1, c2, out=None):
     """out[..., :] = softmax(sel[..., 0:2])[0] * c1 + [1] * c2 (out may be a column slice of a wider tensor)."""
     _chk(sel), _chk(c1), _chk(c2)

@@ -9,6 +9,7 @@ same sample alone or in any batch at the same index parity.
 
     data, nbytes = video.encode(renderer.render_sequence(poses, expression, trans))   # (B*T, cap) uint8, (B*T,) int64
     video.write_mp4(frames[0], "out/clip.mp4", fps=30)                                 # one silent clip
+    video.write_mp4(frames[0], "out/clip.mp4", fps=30, audio=(pcm, 48000))            # with a FLAC sound track
 
 Deblocking is off, so a decoder's output is the encoder's reconstruction exactly.
 """
@@ -19,7 +20,7 @@ from fractions import Fraction
 
 import torch
 
-from . import ops
+from . import flac, ops
 
 MB_BITS_LIMIT = 3200                      # 128 + RawMbBits: the most bits one macroblock_layer() may take (A.3.1)
 MAX_FS, MAX_DIM_MBS = 36864, 543          # level 5.1: MaxFS, and the most macroblocks in a row or column
@@ -197,11 +198,49 @@ def _full(kind: bytes, version: int, flags: int, *parts: bytes) -> bytes:
 _MATRIX = struct.pack(">9i", 0x10000, 0, 0, 0, 0x10000, 0, 0, 0, 0x40000000)
 
 
-def mp4_bytes(samples, h: int, w: int, fps=30) -> bytes:
-    """An MP4 file of one silent H.264 video track: samples (a list of bytes-like, each a sample as encode() writes
-    it), h x w frames at a constant fps.  ftyp, then moov (avc1 with its avcC holding the SPS and PPS, stts, stsc, stsz,
-    stco, no stss: every sample is a sync sample), then mdat, so the file plays while it downloads.  Raises ValueError
-    on no samples, fps <= 0 or a file that would pass 2^32 bytes."""
+def _chunks(sizes, starts):
+    """stsc and stco payloads of one track from its chunks' sample counts and file offsets."""
+    runs = []
+    for i, k in enumerate(sizes):
+        if not runs or runs[-1][1] != k:
+            runs.append((i + 1, k))
+    stsc = struct.pack(">I", len(runs)) + b"".join(struct.pack(">III", first, k, 1) for first, k in runs)
+    return stsc, struct.pack(">I", len(starts)) + struct.pack(f">{len(starts)}I", *starts)
+
+
+def _audio_trak(frames, info, movie_dur, stsc, stco):
+    """The sound track: fLaC sample entry with its dfLa (STREAMINFO, last-block flag set), one sample per frame."""
+    rate, channels, bps, total = flac.parse_streaminfo(info)
+    n = len(frames)
+    last = total - flac.BLOCK * (n - 1)
+    runs = [(n, flac.BLOCK)] if last == flac.BLOCK else [(n - 1, flac.BLOCK), (1, last)] if n > 1 else [(1, last)]
+    dfla = _full(b"dfLa", 0, 0, bytes([0x80, 0, 0, len(info)]), info)
+    entry = _box(b"fLaC", bytes(6), struct.pack(">H", 1), bytes(8), struct.pack(">HHHHI", channels, bps, 0, 0,
+                                                                                 rate << 16), dfla)
+    stbl = _box(b"stbl",
+                _full(b"stsd", 0, 0, struct.pack(">I", 1), entry),
+                _full(b"stts", 0, 0, struct.pack(">I", len(runs)), *(struct.pack(">II", *r) for r in runs)),
+                _full(b"stsc", 0, 0, stsc),
+                _full(b"stsz", 0, 0, struct.pack(">II", 0, n), struct.pack(f">{n}I", *map(len, frames))),
+                _full(b"stco", 0, 0, stco))
+    minf = _box(b"minf", _full(b"smhd", 0, 0, bytes(4)),
+                _box(b"dinf", _full(b"dref", 0, 0, struct.pack(">I", 1), _full(b"url ", 0, 1))), stbl)
+    mdia = _box(b"mdia",
+                _full(b"mdhd", 0, 0, struct.pack(">IIIIHH", 0, 0, rate, total, 0x55C4, 0)),
+                _full(b"hdlr", 0, 0, bytes(4), b"soun", bytes(12), b"SoundHandler\0"), minf)
+    tkhd = _full(b"tkhd", 0, 3, struct.pack(">IIIII", 0, 0, 2, 0, movie_dur), bytes(8),
+                 struct.pack(">hhhH", 0, 0, 0x100, 0), _MATRIX, struct.pack(">II", 0, 0))
+    return _box(b"trak", tkhd, mdia)
+
+
+def mp4_bytes(samples, h: int, w: int, fps=30, audio=None) -> bytes:
+    """An MP4 file of one H.264 video track: samples (a list of bytes-like, each a sample as encode() writes it), h x w
+    frames at a constant fps.  ftyp, then moov (avc1 with its avcC holding the SPS and PPS, stts, stsc, stsz, stco, no
+    stss: every sample is a sync sample), then mdat, so the file plays while it downloads.
+    audio: None (a silent file), or (frames, info), a FLAC track: its frames (bytes-like, as flac.encode writes them)
+    and their 34-byte STREAMINFO (flac.streaminfo).  The file then has a second track, and mdat holds one-second
+    chunks: each second's video samples, then the audio frames that start in that second.
+    Raises ValueError on no samples, fps <= 0 or a file that would pass 2^32 bytes."""
     check_size(h, w)
     if isinstance(fps, bool) or not isinstance(fps, (int, float, Fraction)) or not fps > 0:
         raise ValueError(f"fps must be a positive number, got {fps!r}")
@@ -215,6 +254,23 @@ def mp4_bytes(samples, h: int, w: int, fps=30) -> bytes:
     movie_dur = media_dur * 1000 // timescale
     if timescale >= 1 << 32 or media_dur >= 1 << 32 or movie_dur >= 1 << 32:
         raise ValueError(f"{n} frames at {fps} fps do not fit 32-bit MP4 durations")
+    if audio is None:
+        plan = [(0, list(range(n)))]                   # one chunk: every video sample
+        sound, audio_dur = [], 0
+    else:
+        sound, info = [bytes(f) for f in audio[0]], bytes(audio[1])
+        srate, _, _, total = flac.parse_streaminfo(info)
+        if len(info) != 34 or not sound or len(sound) != flac.frames_of(total) or total >= 1 << 32:
+            raise ValueError("audio must be (frames, STREAMINFO) of one FLAC clip of fewer than 2^32 samples")
+        audio_dur = total * 1000 // srate
+        second = {}
+        for i in range(n):
+            second.setdefault(i * delta // timescale, ([], []))[0].append(i)
+        for k in range(len(sound)):
+            second.setdefault(k * flac.BLOCK // srate, ([], []))[1].append(k)
+        plan = [(t, idx) for s in sorted(second) for t, idx in enumerate(second[s]) if idx]
+    movie = max(movie_dur, audio_dur)
+    data = (samples, sound)
     s, p = sps(h, w), pps()
     avcc = _box(b"avcC", bytes([1, 66, 0xC0, 51, 0xFF, 0xE1]), struct.pack(">H", len(s)), s,
                 bytes([1]), struct.pack(">H", len(p)), p)
@@ -223,12 +279,17 @@ def mp4_bytes(samples, h: int, w: int, fps=30) -> bytes:
                 struct.pack(">Hh", 0x18, -1), avcc)
 
     def moov(offset):
+        starts, at = ([], []), offset
+        for t, idx in plan:
+            starts[t].append(at)
+            at += sum(len(data[t][i]) for i in idx)
+        tables = [_chunks([len(idx) for t, idx in plan if t == tr], starts[tr]) for tr in (0, 1)]
         stbl = _box(b"stbl",
                     _full(b"stsd", 0, 0, struct.pack(">I", 1), avc1),
                     _full(b"stts", 0, 0, struct.pack(">III", 1, n, delta)),
-                    _full(b"stsc", 0, 0, struct.pack(">IIII", 1, 1, n, 1)),
+                    _full(b"stsc", 0, 0, tables[0][0]),
                     _full(b"stsz", 0, 0, struct.pack(">II", 0, n), struct.pack(f">{n}I", *map(len, samples))),
-                    _full(b"stco", 0, 0, struct.pack(">II", 1, offset)))
+                    _full(b"stco", 0, 0, tables[0][1]))
         minf = _box(b"minf", _full(b"vmhd", 0, 1, bytes(8)),
                     _box(b"dinf", _full(b"dref", 0, 0, struct.pack(">I", 1), _full(b"url ", 0, 1))), stbl)
         mdia = _box(b"mdia",
@@ -236,41 +297,71 @@ def mp4_bytes(samples, h: int, w: int, fps=30) -> bytes:
                     _full(b"hdlr", 0, 0, bytes(4), b"vide", bytes(12), b"VideoHandler\0"), minf)
         tkhd = _full(b"tkhd", 0, 3, struct.pack(">IIIII", 0, 0, 1, 0, movie_dur), bytes(8),
                      struct.pack(">hhhH", 0, 0, 0, 0), _MATRIX, struct.pack(">II", w << 16, h << 16))
-        mvhd = _full(b"mvhd", 0, 0, struct.pack(">IIII", 0, 0, 1000, movie_dur), struct.pack(">IH", 0x10000, 0x100),
-                     bytes(10), _MATRIX, bytes(24), struct.pack(">I", 2))
-        return _box(b"moov", mvhd, _box(b"trak", tkhd, mdia))
+        mvhd = _full(b"mvhd", 0, 0, struct.pack(">IIII", 0, 0, 1000, movie), struct.pack(">IH", 0x10000, 0x100),
+                     bytes(10), _MATRIX, bytes(24), struct.pack(">I", 2 if audio is None else 3))
+        traks = [_box(b"trak", tkhd, mdia)]
+        if audio is not None:
+            traks.append(_audio_trak(sound, info, audio_dur, *tables[1]))
+        return _box(b"moov", mvhd, *traks)
 
     ftyp = _box(b"ftyp", b"isom", struct.pack(">I", 0x200), b"isomiso2avc1mp41")
     head = len(ftyp) + len(moov(0)) + 8
-    total = head + sum(len(x) for x in samples)
+    total = head + sum(len(x) for x in samples) + sum(len(x) for x in sound)
     if total >= 1 << 32:
         raise ValueError(f"the file would take {total} bytes, past 2^32")
-    return ftyp + moov(head) + struct.pack(">I", 8 + total - head) + b"mdat" + b"".join(samples)
+    body = b"".join(data[t][i] for t, idx in plan for i in idx)
+    return ftyp + moov(head) + struct.pack(">I", 8 + total - head) + b"mdat" + body
 
 
-def write_mp4(frames, path, fps=30, qp=20):
-    """Encode one clip (T, H, W, 3) uint8 CUDA frames and write it to path as an MP4 file (one silent video track).
-    Reads the sizes once (one synchronisation), copies only the encoded bytes to pinned host memory, waits once for
-    those copies and writes the file.  Returns path."""
+def write_mp4(frames, path, fps=30, qp=20, audio=None):
+    """Encode one clip (T, H, W, 3) uint8 CUDA frames and write it to path as an MP4 file.  audio: None (one silent
+    video track), or (pcm, rate): pcm (n, C) CUDA int16 or int32 (24-bit) samples at rate Hz, coded as a FLAC track
+    (flac.encode) and trimmed to the video's duration: the first min(n, floor(T rate / fps)) samples.  That matches
+    ffmpeg's -shortest when the audio is the longer stream; shorter audio is kept whole, and the video plays on past
+    its end in silence.  Both streams are encoded on the current stream; the sizes are read once (one
+    synchronisation), only the encoded bytes (and the samples, for the MD5) are copied to pinned host memory, and
+    the copies are waited for once.  Returns path."""
     if torch.is_tensor(frames) and frames.dim() != 4:
         raise ValueError(f"write_mp4 takes one clip (T, H, W, 3), got {tuple(frames.shape)}")
     if isinstance(fps, bool) or not isinstance(fps, (int, float, Fraction)) or not fps > 0:
         raise ValueError(f"fps must be a positive number, got {fps!r}")
+    if audio is not None:
+        pcm, rate = audio
+        flac._rate(rate)
+        if not torch.is_tensor(pcm) or pcm.dim() != 2:
+            raise ValueError("write_mp4: audio must be (pcm (n, C) CUDA tensor, rate)")
+        keep = min(pcm.shape[0], int(frames.shape[0] * rate / Fraction(fps).limit_denominator(1001)))
+        if keep < 1:
+            raise ValueError(f"write_mp4: {frames.shape[0]} frames at {fps} fps hold no sample at {rate} Hz")
+        pcm = pcm[:keep]
     data, nbytes = encode(frames, qp=qp)
     h, w = frames.shape[1:3]
-    sizes = nbytes.tolist()
-    host = torch.empty(sum(sizes), dtype=torch.uint8, pin_memory=True)
+    if audio is None:
+        sizes, sound_sizes = nbytes.tolist(), []
+    else:
+        adata, anbytes = flac.encode(pcm, rate)
+        both = torch.cat([nbytes, anbytes]).tolist()
+        sizes, sound_sizes = both[:len(nbytes)], both[len(nbytes):]
+        if min(sound_sizes) < 0:
+            raise ValueError("write_mp4: int32 audio samples must lie in -2^23 .. 2^23 - 1")
+        host_pcm = torch.empty(pcm.shape, dtype=pcm.dtype, pin_memory=True)
+        host_pcm.copy_(pcm, non_blocking=True)
+    host = torch.empty(sum(sizes) + sum(sound_sizes), dtype=torch.uint8, pin_memory=True)
     at = 0
-    for i, k in enumerate(sizes):
-        host[at:at + k].copy_(data[i, :k], non_blocking=True)
-        at += k
+    for src, ks in ((data, sizes), (adata if audio is not None else None, sound_sizes)):
+        for i, k in enumerate(ks):
+            host[at:at + k].copy_(src[i, :k], non_blocking=True)
+            at += k
     torch.cuda.current_stream(data.device).synchronize()
     flat = memoryview(host.numpy())
-    samples, at = [], 0
-    for k in sizes:
-        samples.append(flat[at:at + k])
+    pieces, at = [], 0
+    for k in sizes + sound_sizes:
+        pieces.append(flat[at:at + k])
         at += k
-    blob = mp4_bytes(samples, h, w, fps)
+    track = None
+    if audio is not None:
+        track = (pieces[len(sizes):], flac.streaminfo(host_pcm, rate, sound_sizes))
+    blob = mp4_bytes(pieces[:len(sizes)], h, w, fps, audio=track)
     with open(path, "wb") as f:
         f.write(blob)
     return path
