@@ -28,7 +28,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 from models.emage_audio import EmageAudioModel, EmageVAEConv, EmageVQModel, EmageVQVAEConv  # noqa: E402  (GPU drop-in)
-from pantomatrix_b200.audio_io import load_audio  # noqa: E402
+from pantomatrix_b200.audio_io import load_audio, read_track  # noqa: E402
 from pantomatrix_b200.motion_io import beat_format_save  # noqa: E402
 from pantomatrix_b200.pipeline import generate  # noqa: E402
 
@@ -44,19 +44,6 @@ def load_models(args, device):
     motion_vq = EmageVQModel(face_model=vq["face"], upper_model=vq["upper"], lower_model=vq["lower"],
                              hands_model=vq["hands"], global_model=glob).to(device).eval()
     return EmageAudioModel.from_pretrained(ck).to(device).eval(), motion_vq
-
-
-def write_frames(frames, folder):
-    """(N, 720, 960, 3) uint8 CUDA frames -> folder/frame_%05d.png, encoded on the GPU (pantomatrix_b200.png)."""
-    from pantomatrix_b200 import png
-    png.write_frames(frames, folder)
-
-
-def track(path, device):
-    """(samples on the GPU, rate) of a WAV file for video.write_mp4's audio track (audio_io.track_samples)."""
-    from pantomatrix_b200.audio_io import read_pcm, track_samples
-    pcm, rate = read_pcm(path)
-    return torch.from_numpy(np.ascontiguousarray(track_samples(pcm))).to(device), rate
 
 
 def main():
@@ -100,11 +87,13 @@ def main():
         if renderer is not None:
             drawn = renderer.render_sequence(pred["motion_axis_angle"], pred["expression"], pred["trans"])[0]
             if args.render:
-                write_frames(drawn, os.path.splitext(npz)[0] + "_frames")
+                from pantomatrix_b200 import png
+                png.write_frames(drawn, os.path.splitext(npz)[0] + "_frames")
             if args.video:
                 from pantomatrix_b200 import video
                 video.write_mp4(drawn, os.path.splitext(npz)[0] + ".mp4", fps=30,
-                                audio=track(os.path.join(args.audio_folder, name), device) if args.with_audio else None)
+                                audio=read_track(os.path.join(args.audio_folder, name), device)
+                                if args.with_audio else None)
         frames += t
     print(f"generate total {frames / fps:.2f} seconds motion in {time.time() - t0:.2f} seconds")
 

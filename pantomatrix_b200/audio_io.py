@@ -71,6 +71,13 @@ def track_samples(x):
     return np.clip(v, -(1 << 23), (1 << 23) - 1).astype(np.int32)
 
 
+def read_track(path, device):
+    """(samples on device, rate) of a WAV file for video.write_mp4's audio track: read_pcm, then track_samples."""
+    import torch
+    pcm, rate = read_pcm(path)
+    return torch.from_numpy(np.ascontiguousarray(track_samples(pcm))).to(device), rate
+
+
 def _read_wav(path):
     """(float32 samples (n, channels) in [-1, 1], rate)."""
     x, rate = read_pcm(path)

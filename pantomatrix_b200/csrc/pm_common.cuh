@@ -41,6 +41,16 @@ __device__ __forceinline__ float pm_act(float v, int act, float slope) {
   return v;
 }
 
+// ORs the nb (0..32) low bits of v, MSB first, into the big-endian bit stream at w at bit pos: stream byte i is byte i
+// of the buffer in memory, so the words hold the stream in its own byte order.  atomicOr keeps it independent of
+// the order in which threads write codes that share a word.
+__device__ __forceinline__ void pm_put_bits(unsigned* w, long long pos, unsigned v, int nb) {
+  if (nb == 0) return;
+  const unsigned long long x = (unsigned long long)v << (64 - (int)(pos & 31) - nb);
+  atomicOr(w + (pos >> 5), __byte_perm((unsigned)(x >> 32), 0, 0x0123));
+  if ((unsigned)x) atomicOr(w + (pos >> 5) + 1, __byte_perm((unsigned)x, 0, 0x0123));
+}
+
 __device__ __forceinline__ float pm_warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

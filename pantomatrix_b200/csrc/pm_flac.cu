@@ -182,14 +182,6 @@ __global__ void __launch_bounds__(THREADS) flac_analyse_kernel(const T* __restri
   }
 }
 
-// ORs the nb (0..32) low bits of v, MSB first, into the big-endian bit stream of the slot at bit pos.
-__device__ __forceinline__ void put(unsigned* w, long long pos, unsigned v, int nb) {
-  if (nb == 0) return;
-  const unsigned long long x = (unsigned long long)v << (64 - (int)(pos & 31) - nb);
-  atomicOr(w + (pos >> 5), __byte_perm((unsigned)(x >> 32), 0, 0x0123));
-  if ((unsigned)x) atomicOr(w + (pos >> 5) + 1, __byte_perm((unsigned)x, 0, 0x0123));
-}
-
 // a b mod x^16 + x^15 + x^2 + 1 over GF(2).
 __device__ unsigned gf_mul(unsigned a, unsigned b) {
   unsigned r = 0;
@@ -280,7 +272,7 @@ __global__ void __launch_bounds__(THREADS) flac_emit_kernel(const T* __restrict_
     }
     h[hl++] = (unsigned char)c8;
     if (!bad)
-      for (int i = 0; i < hl; ++i) put(out, 8LL * i, h[i], 8);
+      for (int i = 0; i < hl; ++i) pm_put_bits(out, 8LL * i, h[i], 8);
     sub_off[0] = 8LL * hl;
     for (int c = 0; c < nsub; ++c) sub_off[c + 1] = sub_off[c] + r0[sub_cand[c] * REC];
   }
@@ -300,20 +292,21 @@ __global__ void __launch_bounds__(THREADS) flac_emit_kernel(const T* __restrict_
     const long long pos = sub_off[c];
     const int type = r[1] & 0xff;
     if (type == CONSTANT) {
-      if (t == 0) put(out, pos, 0, 8), put(out, pos + 8, (unsigned)x[0] & mask, bpsc);
+      if (t == 0) pm_put_bits(out, pos, 0, 8), pm_put_bits(out, pos + 8, (unsigned)x[0] & mask, bpsc);
     } else if (type == VERBATIM) {
-      if (t == 0) put(out, pos, 2, 8);
-      for (int i = t; i < bs; i += THREADS) put(out, pos + 8 + (long long)i * bpsc, (unsigned)x[i] & mask, bpsc);
+      if (t == 0) pm_put_bits(out, pos, 2, 8);
+      for (int i = t; i < bs; i += THREADS)
+        pm_put_bits(out, pos + 8 + (long long)i * bpsc, (unsigned)x[i] & mask, bpsc);
     } else {
       const int o = r[1] >> 8 & 0xff, p = r[1] >> 16 & 0xff, m = r[1] >> 24;
       const unsigned char* kb = reinterpret_cast<const unsigned char*>(r + 2);
       const int plen = 4 + m, s = bs >> p;
       if (t == 0) {
-        put(out, pos, (unsigned)(8 | o) << 1, 8);
-        put(out, pos + 8 + o * bpsc, (unsigned)(m << 4 | p), 6);
-        put(out, pos + 14 + o * bpsc, kb[0], plen);
+        pm_put_bits(out, pos, (unsigned)(8 | o) << 1, 8);
+        pm_put_bits(out, pos + 8 + o * bpsc, (unsigned)(m << 4 | p), 6);
+        pm_put_bits(out, pos + 14 + o * bpsc, kb[0], plen);
       }
-      if (t < o) put(out, pos + 8 + t * bpsc, (unsigned)x[t] & mask, bpsc);
+      if (t < o) pm_put_bits(out, pos + 8 + t * bpsc, (unsigned)x[t] & mask, bpsc);
       const int lo = max(t * PER, o), hi = min(t * PER + PER, bs);
       int len = 0;
       for (int i = lo; i < hi; ++i) {
@@ -325,9 +318,9 @@ __global__ void __launch_bounds__(THREADS) flac_emit_kernel(const T* __restrict_
       long long cur = pos + 14 + o * bpsc + plen + at;
       for (int i = lo; i < hi; ++i) {
         const int j = i / s, k = kb[j];
-        if (i % s == 0 && i > 0) put(out, cur, k, plen), cur += plen;
+        if (i % s == 0 && i > 0) pm_put_bits(out, cur, k, plen), cur += plen;
         const unsigned u = zigzag(residual(x, i, o));
-        put(out, cur + (u >> k), 1u << k | (u & ((1u << k) - 1)), k + 1);
+        pm_put_bits(out, cur + (u >> k), 1u << k | (u & ((1u << k) - 1)), k + 1);
         cur += (u >> k) + 1 + k;
       }
     }
@@ -350,7 +343,7 @@ __global__ void __launch_bounds__(THREADS) flac_emit_kernel(const T* __restrict_
   if (t == 0) {
     crc = crc_part[0];
     for (int w = 1; w < THREADS / 32; ++w) crc ^= crc_part[w];
-    put(out, 8 * L, crc, 16);
+    pm_put_bits(out, 8 * L, crc, 16);
     nbytes[f] = L + 2;
   }
 }

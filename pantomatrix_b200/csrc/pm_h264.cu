@@ -4,6 +4,8 @@
 //   pm_h264_encode  one warp per (frame, macroblock row): the row's slice, emulation prevention applied, into its
 //                   scratch slot, and the slice's size;
 //   pm_h264_gather  one CTA per (frame, row): the slice's offset in the frame's sample, the copy, the frame's size.
+// A warp stages its bits in shared memory in stream byte order (pm_put_bits, as FLAC writes its slots), so whole
+// bytes leave the staging buffer as byte loads.
 // CPU restatement: oracle/h264_oracle.py.  Every byte depends only on the frame, qp and its index parity.
 #include <cub/block/block_reduce.cuh>
 
@@ -88,17 +90,14 @@ __device__ __forceinline__ int pos_class(int raster) {
   return ((r | c) & 1) == 0 ? 0 : ((r & c) & 1) ? 1 : 2;
 }
 
-// Bits of the warp's staging buffer, MSB first: stream bit k is bit 31 - (k & 31) of word k >> 5.
+// Bits of the warp's staging buffer, in stream byte order (pm_put_bits): stream byte i is byte i of the buffer, its
+// bits MSB first.  WRITE false only counts them.
 template <bool WRITE>
 struct Bits {
   unsigned* stg;
   int pos;
   __device__ __forceinline__ void put(unsigned v, int n) {   // n <= 32, v < 2^n
-    if (WRITE && n) {
-      const unsigned long long x = (unsigned long long)v << (64 - (pos & 31) - n);
-      atomicOr(stg + (pos >> 5), (unsigned)(x >> 32));
-      if ((unsigned)x) atomicOr(stg + (pos >> 5) + 1, (unsigned)x);
-    }
+    if (WRITE) pm_put_bits(stg, pos, v, n);
     pos += n;
   }
   __device__ __forceinline__ void code(unsigned short lv) { put(lv & 0xff, lv >> 8); }
@@ -227,7 +226,7 @@ struct Warp {
 };
 
 __device__ __forceinline__ unsigned stg_byte(const unsigned* stg, int i) {
-  return (stg[i >> 2] >> (24 - 8 * (i & 3))) & 0xff;
+  return reinterpret_cast<const unsigned char*>(stg)[i];
 }
 
 // Append staging bytes [0, nb) to out + at with emulation prevention; zrun: zero bytes ending the output so far
@@ -537,7 +536,7 @@ __global__ void __launch_bounds__(32 * WARPS) h264_encode_kernel(Job J) {
       for (int i = lane; i < 384; i += 32) {
         const int j = at8 + i;
         const unsigned v = i < 256 ? S.y[i] : (i < 320 ? S.cb[i - 256] : S.cr[i - 320]);
-        atomicOr(S.stg + (j >> 2), v << (24 - 8 * (j & 3)));
+        atomicOr(S.stg + (j >> 2), v << (8 * (j & 3)));
       }
       end = 8 * (at8 + 384);
     }
@@ -548,7 +547,7 @@ __global__ void __launch_bounds__(32 * WARPS) h264_encode_kernel(Job J) {
     __syncwarp();
     for (int i = lane; i <= (end >> 5) && i < STG_WORDS; i += 32) S.stg[i] = 0;
     __syncwarp();
-    if (lane == 0) S.stg[0] = keep << 24;
+    if (lane == 0) S.stg[0] = keep;
     pend = end & 7;
     // ---- the left neighbour of the next macroblock ----
     if (lane < 16) {

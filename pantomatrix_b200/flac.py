@@ -19,7 +19,7 @@ import struct
 import numpy as np
 import torch
 
-from . import ops
+from . import ops, slots
 
 BLOCK = 4096                 # samples per frame (fixed blocking)
 MAX_CHANNELS = 8
@@ -96,20 +96,8 @@ def encode(pcm, rate, out=None):
     b, n, c = pcm.shape
     f = frames_of(n)
     dev = pcm.device
-    need = max_frame_bytes(c, bps, min(n, BLOCK))
-    if out is None:
-        data = torch.empty(b * f, slot_bytes(c, bps, min(n, BLOCK)), dtype=torch.uint8, device=dev)
-        nbytes = torch.empty(b * f, dtype=torch.int64, device=dev)
-    else:
-        data, nbytes = out
-        if not (torch.is_tensor(data) and data.device == dev and data.dtype == torch.uint8 and data.dim() == 2
-                and data.shape[0] == b * f and data.shape[1] >= need and data.shape[1] % 4 == 0
-                and data.is_contiguous()):
-            raise ValueError(f"out data must be a contiguous ({b * f}, cap) uint8 tensor on {dev} with cap >= "
-                             f"{need} a multiple of 4")
-        if not (torch.is_tensor(nbytes) and nbytes.device == dev and nbytes.dtype == torch.int64
-                and tuple(nbytes.shape) == (b * f,) and nbytes.is_contiguous()):
-            raise ValueError(f"out nbytes must be a contiguous ({b * f},) int64 tensor on {dev}")
+    m = min(n, BLOCK)
+    data, nbytes = slots.output(b * f, max_frame_bytes(c, bps, m), slot_bytes(c, bps, m), dev, out)
     if b > 65535 or f * (4 if c == 2 else c) >= 1 << 31:
         raise ValueError(f"{b} clips of {f} frames are past the launch grid")
     rec = torch.empty(b * f * (4 if c == 2 else c), REC_WORDS, dtype=torch.int32, device=dev)

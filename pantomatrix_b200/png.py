@@ -18,7 +18,7 @@ import os
 
 import torch
 
-from . import ops
+from . import ops, slots
 
 FIXED_OVERHEAD = 63        # signature 8, IHDR 25, IDAT length and type 8, zlib header 2, Adler 4, IDAT CRC 4, IEND 12
 MAX_FILE_BYTES = 1 << 31
@@ -36,31 +36,6 @@ def slot_bytes(h: int, w: int) -> int:
     return (max_bytes(h, w) + 3) & ~3
 
 
-def _frames(frames):
-    if not torch.is_tensor(frames):
-        raise ValueError(f"frames must be a tensor, got {type(frames).__name__}")
-    if not frames.is_cuda:
-        raise ValueError("frames must be a CUDA tensor")
-    if frames.dtype != torch.uint8:
-        raise ValueError(f"frames must be uint8, got {frames.dtype}")
-    if frames.dim() not in (4, 5) or frames.shape[-1] != 3 or frames.shape[-2] < 1 or frames.shape[-3] < 1:
-        raise ValueError(f"frames must be (N, H, W, 3) or (B, T, H, W, 3) with H, W >= 1, got {tuple(frames.shape)}")
-    h, w = frames.shape[-3:-1]
-    if frames.stride(-1) != 1 or frames.stride(-2) != 3 or frames.stride(-3) != 3 * w:
-        raise ValueError("frames: each frame must be dense")
-    if frames.dim() == 5:
-        b, t = frames.shape[:2]
-        if b > 1 and t > 1 and frames.stride(0) != t * frames.stride(1):
-            raise ValueError("frames (B, T, H, W, 3): the clips' frames must be evenly spaced")
-        fs = frames.stride(1) if t > 1 else frames.stride(0)
-        frames = frames.as_strided((b * t, h, w, 3), (fs, 3 * w, 3, 1))
-    if frames.shape[0] > 1 and frames.stride(0) < 3 * h * w:
-        raise ValueError("frames: frames must not overlap")
-    if max_bytes(h, w) > MAX_FILE_BYTES:
-        raise ValueError(f"a {h} x {w} frame may take {max_bytes(h, w)} bytes, more than 2^31")
-    return frames
-
-
 @torch.no_grad()
 def encode(frames, out=None):
     """PNG files of frames (N, H, W, 3) or (B, T, H, W, 3) uint8 CUDA, each frame dense (a MeshRenderer result is read
@@ -69,22 +44,12 @@ def encode(frames, out=None):
     contiguous with cap >= slot_bytes(H, W) and a multiple of 4, nbytes (N,) int64 contiguous.  No host
     synchronisation; with out given the call can be captured in a CUDA graph.  Raises ValueError on a CPU tensor, a wrong
     dtype or shape, frames that are not dense, an out too small, or a frame whose bound passes 2^31 bytes."""
-    frames = _frames(frames)
+    frames, _ = slots.frames(frames)
     n, h, w, _ = frames.shape
+    if max_bytes(h, w) > MAX_FILE_BYTES:
+        raise ValueError(f"a {h} x {w} frame may take {max_bytes(h, w)} bytes, more than 2^31")
     dev = frames.device
-    if out is None:
-        data = torch.empty(n, slot_bytes(h, w), dtype=torch.uint8, device=dev)
-        nbytes = torch.empty(n, dtype=torch.int64, device=dev)
-    else:
-        data, nbytes = out
-        if not (torch.is_tensor(data) and data.device == dev and data.dtype == torch.uint8 and data.dim() == 2
-                and data.shape[0] == n and data.shape[1] >= max_bytes(h, w) and data.shape[1] % 4 == 0
-                and data.is_contiguous()):
-            raise ValueError(f"out data must be a contiguous ({n}, cap) uint8 tensor on {dev} with cap >= "
-                             f"{max_bytes(h, w)} a multiple of 4")
-        if not (torch.is_tensor(nbytes) and nbytes.device == dev and nbytes.dtype == torch.int64
-                and tuple(nbytes.shape) == (n,) and nbytes.is_contiguous()):
-            raise ValueError(f"out nbytes must be a contiguous ({n},) int64 tensor on {dev}")
+    data, nbytes = slots.output(n, max_bytes(h, w), slot_bytes(h, w), dev, out)
     if n == 0:
         return data, nbytes
     row_bits = torch.empty(n, h, dtype=torch.int64, device=dev)
@@ -102,19 +67,10 @@ def write_frames(frames, folder, pattern="frame_%05d.png"):
     paths = []
     if not sizes:
         return paths
-    # each file's bytes straight from its slot into one pinned host buffer, then one wait for the copies
-    host = torch.empty(sum(sizes), dtype=torch.uint8, pin_memory=True)
-    at = 0
-    for i, k in enumerate(sizes):
-        host[at:at + k].copy_(data[i, :k], non_blocking=True)
-        at += k
-    torch.cuda.current_stream(data.device).synchronize()
-    flat = host.numpy()
-    at = 0
-    for i, k in enumerate(sizes):
+    (files,) = slots.to_host((data, sizes))
+    for i, blob in enumerate(files):
         path = os.path.join(folder, pattern % i)
         with open(path, "wb") as f:
-            f.write(flat[at:at + k].tobytes())
-        at += k
+            f.write(blob)
         paths.append(path)
     return paths

@@ -20,7 +20,7 @@ from fractions import Fraction
 
 import torch
 
-from . import flac, ops
+from . import flac, ops, slots
 
 MB_BITS_LIMIT = 3200                      # 128 + RawMbBits: the most bits one macroblock_layer() may take (A.3.1)
 MAX_FS, MAX_DIM_MBS = 36864, 543          # level 5.1: MaxFS, and the most macroblocks in a row or column
@@ -60,6 +60,13 @@ def _qp(qp) -> int:
     if isinstance(qp, bool) or not isinstance(qp, int) or not 0 <= qp <= 51:
         raise ValueError(f"qp must be an int in 0..51, got {qp!r}")
     return qp
+
+
+def _fps(fps) -> Fraction:
+    """The frame rate as the MP4 file states it: timescale / sample duration, a denominator of at most 1001."""
+    if isinstance(fps, bool) or not isinstance(fps, (int, float, Fraction)) or not fps > 0:
+        raise ValueError(f"fps must be a positive number, got {fps!r}")
+    return Fraction(fps).limit_denominator(1001)
 
 
 # ---- parameter sets, built on the host (the CPU restatement of the rule builds its own) ----
@@ -122,33 +129,6 @@ def pps() -> bytes:
 
 # ---- encoding on the GPU ----
 
-def _frames(frames):
-    if not torch.is_tensor(frames):
-        raise ValueError(f"frames must be a tensor, got {type(frames).__name__}")
-    if not frames.is_cuda:
-        raise ValueError("frames must be a CUDA tensor")
-    if frames.dtype != torch.uint8:
-        raise ValueError(f"frames must be uint8, got {frames.dtype}")
-    if frames.dim() not in (4, 5) or frames.shape[-1] != 3:
-        raise ValueError(f"frames must be (N, H, W, 3) or (B, T, H, W, 3), got {tuple(frames.shape)}")
-    h, w = frames.shape[-3:-1]
-    check_size(h, w)
-    if frames.stride(-1) != 1 or frames.stride(-2) != 3 or frames.stride(-3) != 3 * w:
-        raise ValueError("frames: each frame must be dense")
-    if frames.dim() == 5:
-        b, t = frames.shape[:2]
-        if b > 1 and t > 1 and frames.stride(0) != t * frames.stride(1):
-            raise ValueError("frames (B, T, H, W, 3): the clips' frames must be evenly spaced")
-        fs = frames.stride(1) if t > 1 else frames.stride(0)
-        clip_len = t
-        frames = frames.as_strided((b * t, h, w, 3), (fs, 3 * w, 3, 1))
-    else:
-        clip_len = frames.shape[0]
-    if frames.shape[0] > 1 and frames.stride(0) < 3 * h * w:
-        raise ValueError("frames: frames must not overlap")
-    return frames, max(clip_len, 1)
-
-
 @torch.no_grad()
 def encode(frames, qp=20, out=None):
     """H.264 samples of frames (N, H, W, 3) or (B, T, H, W, 3) uint8 CUDA, each frame dense (a MeshRenderer result is
@@ -160,22 +140,11 @@ def encode(frames, qp=20, out=None):
     captured in a CUDA graph.  Raises ValueError on a CPU tensor, a wrong dtype or shape, H or W not a multiple of 16,
     a frame past level 5.1, frames that are not dense, qp outside 0..51 or an out too small."""
     qp = _qp(qp)
-    frames, clip_len = _frames(frames)
+    frames, clip_len = slots.frames(frames)
     n, h, w, _ = frames.shape
+    check_size(h, w)
     dev = frames.device
-    if out is None:
-        data = torch.empty(n, slot_bytes(h, w), dtype=torch.uint8, device=dev)
-        nbytes = torch.empty(n, dtype=torch.int64, device=dev)
-    else:
-        data, nbytes = out
-        if not (torch.is_tensor(data) and data.device == dev and data.dtype == torch.uint8 and data.dim() == 2
-                and data.shape[0] == n and data.shape[1] >= max_bytes(h, w) and data.shape[1] % 4 == 0
-                and data.is_contiguous()):
-            raise ValueError(f"out data must be a contiguous ({n}, cap) uint8 tensor on {dev} with cap >= "
-                             f"{max_bytes(h, w)} a multiple of 4")
-        if not (torch.is_tensor(nbytes) and nbytes.device == dev and nbytes.dtype == torch.int64
-                and tuple(nbytes.shape) == (n,) and nbytes.is_contiguous()):
-            raise ValueError(f"out nbytes must be a contiguous ({n},) int64 tensor on {dev}")
+    data, nbytes = slots.output(n, max_bytes(h, w), slot_bytes(h, w), dev, out)
     if n == 0:
         return data, nbytes
     scratch = torch.empty(n, h // 16, slice_bytes(w), dtype=torch.uint8, device=dev)
@@ -208,28 +177,28 @@ def _chunks(sizes, starts):
     return stsc, struct.pack(">I", len(starts)) + struct.pack(f">{len(starts)}I", *starts)
 
 
-def _audio_trak(frames, info, movie_dur, stsc, stco):
-    """The sound track: fLaC sample entry with its dfLa (STREAMINFO, last-block flag set), one sample per frame."""
-    rate, channels, bps, total = flac.parse_streaminfo(info)
-    n = len(frames)
-    last = total - flac.BLOCK * (n - 1)
-    runs = [(n, flac.BLOCK)] if last == flac.BLOCK else [(n - 1, flac.BLOCK), (1, last)] if n > 1 else [(1, last)]
-    dfla = _full(b"dfLa", 0, 0, bytes([0x80, 0, 0, len(info)]), info)
-    entry = _box(b"fLaC", bytes(6), struct.pack(">H", 1), bytes(8), struct.pack(">HHHHI", channels, bps, 0, 0,
-                                                                                 rate << 16), dfla)
+def _trak(track_id, duration, volume, size, timescale, media_dur, handler, media_header, entry, stts, sample_sizes,
+          chunks):
+    """One track: tkhd (its duration in movie ticks, volume, size (w, h)), then mdia: mdhd (timescale and duration),
+    hdlr (handler: type and name), and minf holding the media header box, dinf with its dref, and stbl: stsd with the
+    sample entry, the stts payload, the stsc and stco payloads of _chunks (chunks), stsz of the samples' sizes."""
+    n = len(sample_sizes)
+    stsc, stco = chunks
     stbl = _box(b"stbl",
                 _full(b"stsd", 0, 0, struct.pack(">I", 1), entry),
-                _full(b"stts", 0, 0, struct.pack(">I", len(runs)), *(struct.pack(">II", *r) for r in runs)),
+                _full(b"stts", 0, 0, stts),
                 _full(b"stsc", 0, 0, stsc),
-                _full(b"stsz", 0, 0, struct.pack(">II", 0, n), struct.pack(f">{n}I", *map(len, frames))),
+                _full(b"stsz", 0, 0, struct.pack(">II", 0, n), struct.pack(f">{n}I", *sample_sizes)),
                 _full(b"stco", 0, 0, stco))
-    minf = _box(b"minf", _full(b"smhd", 0, 0, bytes(4)),
+    minf = _box(b"minf", media_header,
                 _box(b"dinf", _full(b"dref", 0, 0, struct.pack(">I", 1), _full(b"url ", 0, 1))), stbl)
+    kind, name = handler
     mdia = _box(b"mdia",
-                _full(b"mdhd", 0, 0, struct.pack(">IIIIHH", 0, 0, rate, total, 0x55C4, 0)),
-                _full(b"hdlr", 0, 0, bytes(4), b"soun", bytes(12), b"SoundHandler\0"), minf)
-    tkhd = _full(b"tkhd", 0, 3, struct.pack(">IIIII", 0, 0, 2, 0, movie_dur), bytes(8),
-                 struct.pack(">hhhH", 0, 0, 0x100, 0), _MATRIX, struct.pack(">II", 0, 0))
+                _full(b"mdhd", 0, 0, struct.pack(">IIIIHH", 0, 0, timescale, media_dur, 0x55C4, 0)),
+                _full(b"hdlr", 0, 0, bytes(4), kind, bytes(12), name), minf)
+    w, h = size
+    tkhd = _full(b"tkhd", 0, 3, struct.pack(">IIIII", 0, 0, track_id, 0, duration), bytes(8),
+                 struct.pack(">hhhH", 0, 0, volume, 0), _MATRIX, struct.pack(">II", w << 16, h << 16))
     return _box(b"trak", tkhd, mdia)
 
 
@@ -242,12 +211,10 @@ def mp4_bytes(samples, h: int, w: int, fps=30, audio=None) -> bytes:
     chunks: each second's video samples, then the audio frames that start in that second.
     Raises ValueError on no samples, fps <= 0 or a file that would pass 2^32 bytes."""
     check_size(h, w)
-    if isinstance(fps, bool) or not isinstance(fps, (int, float, Fraction)) or not fps > 0:
-        raise ValueError(f"fps must be a positive number, got {fps!r}")
+    rate = _fps(fps)
     samples = [bytes(s) for s in samples]
     if not samples:
         raise ValueError("mp4_bytes needs at least one sample")
-    rate = Fraction(fps).limit_denominator(1001)
     timescale, delta = rate.numerator, rate.denominator
     n = len(samples)
     media_dur = n * delta
@@ -259,10 +226,18 @@ def mp4_bytes(samples, h: int, w: int, fps=30, audio=None) -> bytes:
         sound, audio_dur = [], 0
     else:
         sound, info = [bytes(f) for f in audio[0]], bytes(audio[1])
-        srate, _, _, total = flac.parse_streaminfo(info)
-        if len(info) != 34 or not sound or len(sound) != flac.frames_of(total) or total >= 1 << 32:
+        srate, channels, bps, pcm_n = flac.parse_streaminfo(info)
+        if len(info) != 34 or not sound or len(sound) != flac.frames_of(pcm_n) or pcm_n >= 1 << 32:
             raise ValueError("audio must be (frames, STREAMINFO) of one FLAC clip of fewer than 2^32 samples")
-        audio_dur = total * 1000 // srate
+        audio_dur = pcm_n * 1000 // srate
+        # one sample per FLAC frame: fLaC sample entry with its dfLa (STREAMINFO, last-block flag set)
+        nf, last = len(sound), pcm_n - flac.BLOCK * (len(sound) - 1)
+        runs = ([(nf, flac.BLOCK)] if last == flac.BLOCK
+                else [(nf - 1, flac.BLOCK), (1, last)] if nf > 1 else [(1, last)])
+        dfla = _full(b"dfLa", 0, 0, bytes([0x80, 0, 0, len(info)]), info)
+        fla = _box(b"fLaC", bytes(6), struct.pack(">H", 1), bytes(8),
+                   struct.pack(">HHHHI", channels, bps, 0, 0, srate << 16), dfla)
+        sound_stts = struct.pack(">I", len(runs)) + b"".join(struct.pack(">II", *r) for r in runs)
         second = {}
         for i in range(n):
             second.setdefault(i * delta // timescale, ([], []))[0].append(i)
@@ -284,24 +259,14 @@ def mp4_bytes(samples, h: int, w: int, fps=30, audio=None) -> bytes:
             starts[t].append(at)
             at += sum(len(data[t][i]) for i in idx)
         tables = [_chunks([len(idx) for t, idx in plan if t == tr], starts[tr]) for tr in (0, 1)]
-        stbl = _box(b"stbl",
-                    _full(b"stsd", 0, 0, struct.pack(">I", 1), avc1),
-                    _full(b"stts", 0, 0, struct.pack(">III", 1, n, delta)),
-                    _full(b"stsc", 0, 0, tables[0][0]),
-                    _full(b"stsz", 0, 0, struct.pack(">II", 0, n), struct.pack(f">{n}I", *map(len, samples))),
-                    _full(b"stco", 0, 0, tables[0][1]))
-        minf = _box(b"minf", _full(b"vmhd", 0, 1, bytes(8)),
-                    _box(b"dinf", _full(b"dref", 0, 0, struct.pack(">I", 1), _full(b"url ", 0, 1))), stbl)
-        mdia = _box(b"mdia",
-                    _full(b"mdhd", 0, 0, struct.pack(">IIIIHH", 0, 0, timescale, media_dur, 0x55C4, 0)),
-                    _full(b"hdlr", 0, 0, bytes(4), b"vide", bytes(12), b"VideoHandler\0"), minf)
-        tkhd = _full(b"tkhd", 0, 3, struct.pack(">IIIII", 0, 0, 1, 0, movie_dur), bytes(8),
-                     struct.pack(">hhhH", 0, 0, 0, 0), _MATRIX, struct.pack(">II", w << 16, h << 16))
         mvhd = _full(b"mvhd", 0, 0, struct.pack(">IIII", 0, 0, 1000, movie), struct.pack(">IH", 0x10000, 0x100),
                      bytes(10), _MATRIX, bytes(24), struct.pack(">I", 2 if audio is None else 3))
-        traks = [_box(b"trak", tkhd, mdia)]
+        traks = [_trak(1, movie_dur, 0, (w, h), timescale, media_dur, (b"vide", b"VideoHandler\0"),
+                       _full(b"vmhd", 0, 1, bytes(8)), avc1, struct.pack(">III", 1, n, delta),
+                       [len(x) for x in samples], tables[0])]
         if audio is not None:
-            traks.append(_audio_trak(sound, info, audio_dur, *tables[1]))
+            traks.append(_trak(2, audio_dur, 0x100, (0, 0), srate, pcm_n, (b"soun", b"SoundHandler\0"),
+                               _full(b"smhd", 0, 0, bytes(4)), fla, sound_stts, [len(x) for x in sound], tables[1]))
         return _box(b"moov", mvhd, *traks)
 
     ftyp = _box(b"ftyp", b"isom", struct.pack(">I", 0x200), b"isomiso2avc1mp41")
@@ -323,21 +288,21 @@ def write_mp4(frames, path, fps=30, qp=20, audio=None):
     the copies are waited for once.  Returns path."""
     if torch.is_tensor(frames) and frames.dim() != 4:
         raise ValueError(f"write_mp4 takes one clip (T, H, W, 3), got {tuple(frames.shape)}")
-    if isinstance(fps, bool) or not isinstance(fps, (int, float, Fraction)) or not fps > 0:
-        raise ValueError(f"fps must be a positive number, got {fps!r}")
+    frame_rate = _fps(fps)
     if audio is not None:
         pcm, rate = audio
         flac._rate(rate)
         if not torch.is_tensor(pcm) or pcm.dim() != 2:
             raise ValueError("write_mp4: audio must be (pcm (n, C) CUDA tensor, rate)")
-        keep = min(pcm.shape[0], int(frames.shape[0] * rate / Fraction(fps).limit_denominator(1001)))
+        keep = min(pcm.shape[0], int(frames.shape[0] * rate / frame_rate))
         if keep < 1:
             raise ValueError(f"write_mp4: {frames.shape[0]} frames at {fps} fps hold no sample at {rate} Hz")
         pcm = pcm[:keep]
     data, nbytes = encode(frames, qp=qp)
     h, w = frames.shape[1:3]
     if audio is None:
-        sizes, sound_sizes = nbytes.tolist(), []
+        (pieces,) = slots.to_host((data, nbytes.tolist()))
+        track = None
     else:
         adata, anbytes = flac.encode(pcm, rate)
         both = torch.cat([nbytes, anbytes]).tolist()
@@ -345,23 +310,10 @@ def write_mp4(frames, path, fps=30, qp=20, audio=None):
         if min(sound_sizes) < 0:
             raise ValueError("write_mp4: int32 audio samples must lie in -2^23 .. 2^23 - 1")
         host_pcm = torch.empty(pcm.shape, dtype=pcm.dtype, pin_memory=True)
-        host_pcm.copy_(pcm, non_blocking=True)
-    host = torch.empty(sum(sizes) + sum(sound_sizes), dtype=torch.uint8, pin_memory=True)
-    at = 0
-    for src, ks in ((data, sizes), (adata if audio is not None else None, sound_sizes)):
-        for i, k in enumerate(ks):
-            host[at:at + k].copy_(src[i, :k], non_blocking=True)
-            at += k
-    torch.cuda.current_stream(data.device).synchronize()
-    flat = memoryview(host.numpy())
-    pieces, at = [], 0
-    for k in sizes + sound_sizes:
-        pieces.append(flat[at:at + k])
-        at += k
-    track = None
-    if audio is not None:
-        track = (pieces[len(sizes):], flac.streaminfo(host_pcm, rate, sound_sizes))
-    blob = mp4_bytes(pieces[:len(sizes)], h, w, fps, audio=track)
+        host_pcm.copy_(pcm, non_blocking=True)          # done by the time to_host's one synchronisation returns
+        pieces, sound = slots.to_host((data, sizes), (adata, sound_sizes))
+        track = (sound, flac.streaminfo(host_pcm, rate, sound_sizes))
+    blob = mp4_bytes(pieces, h, w, fps, audio=track)
     with open(path, "wb") as f:
         f.write(blob)
     return path

@@ -67,6 +67,19 @@ def test_card_without_a_working_nvidia_smi_is_a_record(fake_device, monkeypatch,
         assert smi.startswith("unavailable: ")
 
 
+def test_launch_ms_times_each_launch_in_order_and_takes_medians(monkeypatch):
+    ran, ms = [], iter([5.0, 1.0, 3.0, 2.0, 4.0, 9.0])
+
+    def event_ms(fn):
+        fn()
+        return next(ms)
+
+    monkeypatch.setattr(measure, "event_ms", event_ms)
+    got = measure.launch_ms({"a": lambda: ran.append("a"), "b": lambda: ran.append("b")}, 3)
+    assert ran == ["a", "b"] * 3
+    assert got == {"a": 4.0, "b": 2.0}
+
+
 def _own_measurement(path):
     """Names of the CUDA-event constructions and nvidia-smi invocations in one tool's source."""
     found = []

@@ -26,7 +26,7 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-from measure import card, event_ms  # noqa: E402
+from measure import card, event_ms, launch_ms  # noqa: E402
 from pantomatrix_b200 import _lib, flac, ops, video  # noqa: E402
 from pantomatrix_b200.body_model import SmplxBodyModel  # noqa: E402
 from pantomatrix_b200.render import MeshRenderer  # noqa: E402
@@ -63,13 +63,9 @@ def arm(pcm, rate, reps):
         "emit": lambda: _lib.call("pm_flac_emit", pcm.data_ptr(), cs, b, n, c, 16, rate, rec.data_ptr(),
                                   data.data_ptr(), data.shape[1], nbytes.data_ptr(), st),
     }
-    times = {k: [] for k in calls}
-    for _ in range(reps):
-        for k, fn in calls.items():
-            times[k].append(event_ms(fn))
     return {"clips": b, "samples": n, "channels": c, "rate": rate, "frames": b * f,
             "encode_ms_median": statistics.median(ms), "encode_ms_all": ms,
-            "stage_ms_median": {k: statistics.median(v) for k, v in times.items()},
+            "stage_ms_median": launch_ms(calls, reps),
             "coded_bytes": coded, "raw_bytes": b * n * c * 2, "coded_fraction_of_raw": coded / (b * n * c * 2)}
 
 

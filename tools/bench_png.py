@@ -33,7 +33,7 @@ from PIL import Image
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-from measure import HBM_BYTES_PER_S, card, event_ms  # noqa: E402
+from measure import HBM_BYTES_PER_S, card, event_ms, launch_ms  # noqa: E402
 from oracle.weights import synth_audio  # noqa: E402
 from pantomatrix_b200 import _lib, ops, png  # noqa: E402
 from pantomatrix_b200.body_model import SmplxBodyModel  # noqa: E402
@@ -67,11 +67,7 @@ def stages(frames, data, nbytes, reps):
                                   st),
         "crc": lambda: _lib.call("pm_png_crc", n, h, w, data.data_ptr(), cap, nbytes.data_ptr(), st),
     }
-    times = {k: [] for k in calls}
-    for _ in range(reps):
-        for k, fn in calls.items():
-            times[k].append(event_ms(fn))
-    return {k: statistics.median(v) for k, v in times.items()}
+    return launch_ms(calls, reps)
 
 
 def pillow(frames, count):

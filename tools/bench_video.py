@@ -29,7 +29,7 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-from measure import card, event_ms  # noqa: E402
+from measure import card, event_ms, launch_ms  # noqa: E402
 from oracle.weights import synth_audio  # noqa: E402
 from pantomatrix_b200 import _lib, ops, png, video  # noqa: E402
 from pantomatrix_b200.body_model import SmplxBodyModel  # noqa: E402
@@ -54,11 +54,7 @@ def stages(frames, clip_len, data, nbytes, reps):
         "gather": lambda: _lib.call("pm_h264_gather", n, h, w, scratch.data_ptr(), sc, sizes.data_ptr(),
                                     data.data_ptr(), cap, nbytes.data_ptr(), st),
     }
-    times = {k: [] for k in calls}
-    for _ in range(reps):
-        for k, fn in calls.items():
-            times[k].append(event_ms(fn))
-    return {k: statistics.median(v) for k, v in times.items()}
+    return launch_ms(calls, reps)
 
 
 def arm(frames, reps):

@@ -2,6 +2,7 @@
 
 Each timer keeps the methodology of the tools that use it; where tools differ (warm-up counts, repetitions, clock),
 they say so through arguments."""
+import statistics
 import subprocess
 import time
 
@@ -51,6 +52,16 @@ def per_call_ms(fn, reps, warmup):
         e.record()
     torch.cuda.synchronize()
     return [s.elapsed_time(e) for s, e in ev]
+
+
+def launch_ms(calls, reps):
+    """{name: median ms} of the launches in calls ({name: fn}): `reps` rounds, each timing every launch once by
+    event_ms, in insertion order."""
+    times = {k: [] for k in calls}
+    for _ in range(reps):
+        for k, fn in calls.items():
+            times[k].append(event_ms(fn))
+    return {k: statistics.median(v) for k, v in times.items()}
 
 
 def mean_ms(fn, iters):
