@@ -36,6 +36,7 @@ extern "C" {
 #define PM_ABI_VERSION 6
 #define PM_FMT_F16 0x100
 #define PM_TC_TILE_SHIFT 16   /* pm_tapgemm_tc: N tile override in bits 16-23 of `nsplit` */
+#define PM_TC_STORE_LOOP (1 << 24)   /* pm_tapgemm_tc: bit 24 of `nsplit` forces the per-element store loop */
 int pm_abi_version(void);
 /* cudaMemsetAsync on `stream` (a memset node under graph capture, not a kernel): zeroed slack rows, flags */
 int pm_memset_async(void* ptr, int value, long long bytes, void* stream);
@@ -66,7 +67,9 @@ int pm_tapgemm_f32(const float* A, long long a_bs, int lda, int batch, int rows_
  * the shape and the SM count unless (nsplit >> PM_TC_TILE_SHIFT) & 0xff forces it: 1 = 64, 2 = 128 columns (tests,
  * A/B runs).  Both tiles give bit-identical results.  lda, ldw, a_bs, a_ps, w_ps must be multiples
  * of 8 elements (TMA 16-byte rule).  The activation is applied to columns < act_cols only (<=0: all).
- * The epilogue writes the fp32 result and/or its bf16 split planes (out_f32 / out_bf16 nullable).
+ * The epilogue writes the fp32 result and/or its bf16 split planes (out_f32 / out_bf16 nullable): by TMA stores
+ * where every output view has a 16-byte aligned base and strides (and a residual, if any, too), otherwise per
+ * element; nsplit | PM_TC_STORE_LOOP forces the per-element loop (tests, A/B runs).  Both give the same bits.
  * Operands are staged by TMA (cp.async.bulk.tensor, zero fill for padding rows, tap shift folded into the
  * row coordinate); descriptors are built on the host inside this call from the raw pointers.
  * `prefetch` (nullable, 16-byte aligned): prefetch_bytes of global memory - the NEXT GEMM's packed weights - are

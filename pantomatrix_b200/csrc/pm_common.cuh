@@ -106,32 +106,54 @@ __device__ __forceinline__ float pm_f16_head(float v) {
   return __uint_as_float((__float_as_uint(v) + 0x00001000u) & 0xFFFFE000u);
 }
 
-// Successive planes are peeled off a running remainder: no dynamically indexed temporaries (they would live in
-// local memory).
-template <bool F16>
-__device__ __forceinline__ void pm_store_planes_t(const PmPlanes& P, long long row, int c, float v) {
+// The split rule itself, in registers, for two values at once (two adjacent channels): w[pl] holds plane pl of x in
+// its low and of y in its high 16 bits, for pl < nsplit.  fp16: both are pre-scaled by PM_F16_ACT_SCALE first, and
+// two planes take the pm_f16_head head; otherwise each plane is the running remainder rounded to nearest even.
+// Every plane writer goes through it (pm_store_planes*_t, the tap-GEMM's TMA-store epilogue).  Successive planes are
+// peeled off a running remainder under a fully unrolled loop: no dynamically indexed temporaries (they would live in
+// local memory).  The pre-scale is __fmul_rn so that no caller's code can contract it into a following subtraction.
+// NS > 0 fixes the plane count at compile time (then `nsplit` is ignored); NS = 0 reads it from `nsplit`.
+template <bool F16, int NS = 0>
+__device__ __forceinline__ void pm_split_pair_t(float x, float y, int nsplit, uint32_t (&w)[3]) {
+  if constexpr (NS > 0) nsplit = NS;
   if constexpr (F16) {
-    __half* o = reinterpret_cast<__half*>(P.ptr) + row * P.ld + c;
-    v *= PM_F16_ACT_SCALE;
-    if (P.nsplit <= 2) {
-      const float f0 = P.nsplit == 2 ? pm_f16_head(v) : v;
-      o[0] = __float2half_rn(f0);
-      if (P.nsplit == 2) o[P.ps] = __float2half_rn(v - f0);
-    } else {
-      for (int pl = 0; pl < P.nsplit; ++pl) {
-        const __half h = __float2half_rn(v);
-        o[(long long)pl * P.ps] = h;
-        v -= __half2float(h);
+    x = __fmul_rn(x, PM_F16_ACT_SCALE);
+    y = __fmul_rn(y, PM_F16_ACT_SCALE);
+    if (nsplit == 2) {
+      const float fx = pm_f16_head(x), fy = pm_f16_head(y);
+      const __half2 a = __floats2half2_rn(fx, fy), b = __floats2half2_rn(x - fx, y - fy);   // a is exact
+      w[0] = *reinterpret_cast<const uint32_t*>(&a);
+      w[1] = *reinterpret_cast<const uint32_t*>(&b);
+      return;
+    }
+#pragma unroll
+    for (int pl = 0; pl < 3; ++pl) {
+      if (pl < nsplit) {
+        const __half2 h = __floats2half2_rn(x, y);
+        w[pl] = *reinterpret_cast<const uint32_t*>(&h);
+        x -= __low2float(h); y -= __high2float(h);
       }
     }
   } else {
-    __nv_bfloat16* o = P.ptr + row * P.ld + c;
-    for (int pl = 0; pl < P.nsplit; ++pl) {
-      const __nv_bfloat16 h = __float2bfloat16_rn(v);
-      o[(long long)pl * P.ps] = h;
-      v -= __bfloat162float(h);
+#pragma unroll
+    for (int pl = 0; pl < 3; ++pl) {
+      if (pl < nsplit) {
+        const __nv_bfloat162 h = __floats2bfloat162_rn(x, y);
+        w[pl] = *reinterpret_cast<const uint32_t*>(&h);
+        x -= __low2float(h); y -= __high2float(h);
+      }
     }
   }
+}
+
+template <bool F16>
+__device__ __forceinline__ void pm_store_planes_t(const PmPlanes& P, long long row, int c, float v) {
+  uint16_t* o = reinterpret_cast<uint16_t*>(P.ptr) + row * P.ld + c;
+  uint32_t w[3];
+  pm_split_pair_t<F16>(v, 0.f, P.nsplit, w);
+#pragma unroll
+  for (int pl = 0; pl < 3; ++pl)
+    if (pl < P.nsplit) o[(long long)pl * P.ps] = (uint16_t)w[pl];
 }
 __device__ __forceinline__ void pm_store_planes(const PmPlanes& P, long long row, int c, float v) {
   pm_store_planes_t<false>(P, row, c, v);
@@ -140,39 +162,13 @@ __device__ __forceinline__ void pm_store_planes(const PmPlanes& P, long long row
 // 4 consecutive channels, c % 4 == 0, ld % 4 == 0, ps % 4 == 0, 8-byte aligned base
 template <bool F16>
 __device__ __forceinline__ void pm_store_planes4_t(const PmPlanes& P, long long row, int c, float4 v) {
-  if constexpr (F16) {
-    __half* o = reinterpret_cast<__half*>(P.ptr) + row * P.ld + c;
-    v.x *= PM_F16_ACT_SCALE; v.y *= PM_F16_ACT_SCALE; v.z *= PM_F16_ACT_SCALE; v.w *= PM_F16_ACT_SCALE;
-    if (P.nsplit == 2) {
-      const float4 f = make_float4(pm_f16_head(v.x), pm_f16_head(v.y), pm_f16_head(v.z), pm_f16_head(v.w));
-      const __half2 a0 = __floats2half2_rn(f.x, f.y), a1 = __floats2half2_rn(f.z, f.w);                       // exact
-      const __half2 b0 = __floats2half2_rn(v.x - f.x, v.y - f.y), b1 = __floats2half2_rn(v.z - f.z, v.w - f.w);
-      uint2 w0, w1;
-      w0.x = *reinterpret_cast<const uint32_t*>(&a0); w0.y = *reinterpret_cast<const uint32_t*>(&a1);
-      w1.x = *reinterpret_cast<const uint32_t*>(&b0); w1.y = *reinterpret_cast<const uint32_t*>(&b1);
-      *reinterpret_cast<uint2*>(o) = w0;
-      *reinterpret_cast<uint2*>(o + P.ps) = w1;
-      return;
-    }
-    for (int pl = 0; pl < P.nsplit; ++pl) {
-      const __half2 lo = __floats2half2_rn(v.x, v.y), hi = __floats2half2_rn(v.z, v.w);
-      uint2 w;
-      w.x = *reinterpret_cast<const uint32_t*>(&lo);
-      w.y = *reinterpret_cast<const uint32_t*>(&hi);
-      *reinterpret_cast<uint2*>(o + (long long)pl * P.ps) = w;
-      v.x -= __low2float(lo); v.y -= __high2float(lo); v.z -= __low2float(hi); v.w -= __high2float(hi);
-    }
-  } else {
-    __nv_bfloat16* o = P.ptr + row * P.ld + c;
-    for (int pl = 0; pl < P.nsplit; ++pl) {
-      const __nv_bfloat162 lo = __floats2bfloat162_rn(v.x, v.y), hi = __floats2bfloat162_rn(v.z, v.w);
-      uint2 w;
-      w.x = *reinterpret_cast<const uint32_t*>(&lo);
-      w.y = *reinterpret_cast<const uint32_t*>(&hi);
-      *reinterpret_cast<uint2*>(o + (long long)pl * P.ps) = w;
-      v.x -= __low2float(lo); v.y -= __high2float(lo); v.z -= __low2float(hi); v.w -= __high2float(hi);
-    }
-  }
+  __nv_bfloat16* o = P.ptr + row * P.ld + c;
+  uint32_t lo[3], hi[3];
+  pm_split_pair_t<F16>(v.x, v.y, P.nsplit, lo);
+  pm_split_pair_t<F16>(v.z, v.w, P.nsplit, hi);
+#pragma unroll
+  for (int pl = 0; pl < 3; ++pl)
+    if (pl < P.nsplit) *reinterpret_cast<uint2*>(o + (long long)pl * P.ps) = make_uint2(lo[pl], hi[pl]);
 }
 __device__ __forceinline__ void pm_store_planes4(const PmPlanes& P, long long row, int c, float4 v) {
   pm_store_planes4_t<false>(P, row, c, v);

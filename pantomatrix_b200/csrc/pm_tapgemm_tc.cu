@@ -17,14 +17,17 @@
 //                              exits at once
 //   warpgroups 1-2   consumers, 232 registers per thread (setmaxnreg.inc) - consumer warpgroup g issues
 //                      wgmma.m64nBNk16 for tile rows 64 g .. 64 g + 63 out of the shared operand stage into three
-//                      BN / 2-register accumulators, then runs the epilogue: registers -> smem tile ->
-//                      bias / residual (both from smem) / activation -> coalesced fp32 store and/or split planes
+//                      BN / 2-register accumulators, then runs the epilogue: bias / residual (both from smem) /
+//                      activation on its own fragment values in registers -> fp32 and/or split-plane tiles in smem
+//                      in the TMA boxes' swizzled layout -> TMA stores by one thread.  Output views TMA cannot
+//                      describe take the per-element store loop: registers -> staging tile -> global
 // Contract and reference call sites: include/pm_emage.h (pm_tapgemm_tc).
 #include <cuda.h>
 #include <stdio.h>
 #include <stdlib.h>
 
 #include <cstring>
+#include <type_traits>
 #include "pm_common.cuh"
 #include "../../include/pm_emage.h"
 
@@ -56,6 +59,8 @@ struct TcParams {
   const float* bias;
   const float* residual; long long r_bs; int ldr;
   int res_tma;                      // residual tile loaded by TMA (map_r) into the ring; else read per element
+  int tma_out;                      // outputs written by TMA stores (map_o / map_p) from swizzled smem tiles; else
+                                    // the per-element store loop
   int act, act_cols; float slope;
   float* out_f32; long long o_bs; int ldo;
   __nv_bfloat16* out_bf16; long long ob_ps, ob_bs; int ldob; int out_nsplit;
@@ -118,6 +123,8 @@ template <int BN, bool F16, int NSPLIT>
 __global__ void __launch_bounds__(NUM_THREADS, 1) tapgemm_tc_kernel(const __grid_constant__ CUtensorMap map_a,
                                                                   const __grid_constant__ CUtensorMap map_w,
                                                                   const __grid_constant__ CUtensorMap map_r,
+                                                                  const __grid_constant__ CUtensorMap map_o,
+                                                                  const __grid_constant__ CUtensorMap map_p,
                                                                   const TcParams p) {
   constexpr int W_TILE_BYTES = BN * BK * 2;
   constexpr int NACC = BN / 2;                      // accumulator registers per thread (m64 x BN over 128 threads)
@@ -128,7 +135,9 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tapgemm_tc_kernel(const __grid
   // carve: [stages][nsplit A tiles][nsplit W tiles] (1024-aligned), then barriers, then the tile's BN bias values.
   // The epilogue reuses the ring: the staging tile at its start, the residual tile in its last RES_BYTES (launch()
   // checks that they do not overlap).
-  uint8_t* tiles = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  // 1024-aligned by pointer arithmetic on smem_raw itself: a pointer that went through an integer is generic to the
+  // compiler, and every epilogue access through it would be a generic ld / st instead of lds / sts
+  uint8_t* tiles = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   const int stage_bytes = p.nsplit * (A_TILE_BYTES + W_TILE_BYTES);
   const int ring_bytes = p.stages * stage_bytes > BM * ST * 4 ? p.stages * stage_bytes : BM * ST * 4;
   uint64_t* bars = reinterpret_cast<uint64_t*>(tiles + ring_bytes);
@@ -151,6 +160,8 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tapgemm_tc_kernel(const __grid
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_w) : "memory");
     if (p.res_tma) asm volatile("prefetch.tensormap [%0];" ::"l"(&map_r) : "memory");
+    if (p.tma_out && p.out_f32) asm volatile("prefetch.tensormap [%0];" ::"l"(&map_o) : "memory");
+    if (p.tma_out && p.out_nsplit) asm volatile("prefetch.tensormap [%0];" ::"l"(&map_p) : "memory");
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(smem_u32(&full_bar[s]), 1);
       mbar_init(smem_u32(&empty_bar[s]), 2);       // one arrival per consumer warpgroup
@@ -213,9 +224,13 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tapgemm_tc_kernel(const __grid
         if (++s == p.stages) { s = 0; ph ^= 1u; }
       }
       if (elect_one()) {
+        // the store loop reads one [NB][R][BN] box; the TMA-store epilogue reads BN / 32 128B-swizzled
+        // [NB][R][32] boxes (the layout of its output tile, conflict-free for the accumulator fragments)
         const uint32_t bar = smem_u32(epi_bar);
         mbar_expect_tx(bar, (uint32_t)RES_BYTES);
-        tma_load_3d(smem_u32(tiles + ring_bytes - RES_BYTES), &map_r, bar, n0, l0, b0);
+        const int nbox = p.tma_out ? BN / 32 : 1;
+        for (int j = 0; j < nbox; ++j)
+          tma_load_3d(smem_u32(tiles + ring_bytes - RES_BYTES + j * (RES_BYTES / nbox)), &map_r, bar, n0 + j * (BN / nbox), l0, b0);
       }
       __syncwarp();
     }
@@ -264,8 +279,95 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) tapgemm_tc_kernel(const __grid
     wgmma_fence_regs(acc1);
     wgmma_fence_regs(accc);
   }
-  // every MMA of both warpgroups has read its operands: the ring becomes the epilogue's staging tile
+  // every MMA of both warpgroups has read its operands: the ring becomes the epilogue's output / staging tile
   named_bar_sync(1, CONSUMER_THREADS);
+  if (p.tma_out) {
+    // ===== epilogue, TMA stores: each thread finishes its own fragment values in registers, writes them once into
+    // the output tiles in the TMA boxes' 128B-swizzled layout, and one thread stores the tiles.  TMA clips at the
+    // maps' bounds (ragged rows_out / cout / batch, clip tiles with R < 128).  Smem (ring start): fp32 tile
+    // [BN / 32][BM][32 floats], then out_nsplit plane tiles [BN / 64][BM][64 halves]; the residual tile is
+    // [BN / 32][BM][32 floats] in the ring's last RES_BYTES.  A 128B swizzle puts 16-byte chunk k of 128-byte row r
+    // at chunk k ^ (r % 8), so the 8 rows of a fragment access hit 8 different chunks.  With both outputs the fp32
+    // tile goes out first: the TMA engine reads it while the consumers split the planes.
+    const int wq = warp & 3, t4 = lane & 3, sw = lane >> 2;       // sw = r % 8 for both rows of the thread
+    const int r0 = wg * 64 + wq * 16 + sw;
+    const float act_slope = p.act == PM_ACT_NONE ? 1.f : (p.act == PM_ACT_RELU ? 0.f : p.slope);
+    const float* res_s = reinterpret_cast<const float*>(tiles + ring_bytes - RES_BYTES);
+    // float offset of (row r, column c) in a [BN / 32][BM][32] swizzled tile; c = 8 i + 2 t4 (even)
+    auto off32 = [&](int r, int i) { return (i >> 2) * (BM * 32) + r * 32 + (((2 * (i & 3) + (t4 >> 1)) ^ sw) << 2) + 2 * (t4 & 1); };
+    mbar_wait_fast(smem_u32(epi_bar), 0);                        // bias (and residual tile) landed
+    // (acc0 + acc1) + accc, x acc_scale, + bias, + residual, activation: the store loop's order, into acc0
+#pragma unroll
+    for (int i = 0; i < NACC / 4; ++i) {
+      const int c = 8 * i + 2 * t4, n = n0 + c;
+      const float2 bc = *reinterpret_cast<const float2*>(bias_s + c);   // both rows' columns
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int j = 4 * i + 2 * h;
+        float v0 = acc0[j] + acc1[j], v1 = acc0[j + 1] + acc1[j + 1];
+        v0 += accc[j];
+        v1 += accc[j + 1];
+        if constexpr (F16) { v0 = __fmul_rn(v0, p.acc_scale); v1 = __fmul_rn(v1, p.acc_scale); }   // not fused with + bias
+        if (p.bias) { v0 += bc.x; v1 += bc.y; }
+        if (p.residual) {
+          const float2 t = *reinterpret_cast<const float2*>(res_s + off32(r0 + 8 * h, i));
+          v0 += t.x; v1 += t.y;
+        }
+        // compare-select, NaN kept (see the store loop)
+        acc0[j] = v0 < 0.f ? (n < p.act_cols ? act_slope : 1.f) * v0 : v0;
+        acc0[j + 1] = v1 < 0.f ? (n + 1 < p.act_cols ? act_slope : 1.f) * v1 : v1;
+      }
+    }
+    float* of_s = reinterpret_cast<float*>(tiles);
+    uint8_t* pl_s = tiles + (p.out_f32 ? BM * BN * 4 : 0);
+    constexpr int PLANE_BYTES = BM * BN * 2;
+    if (p.out_f32) {
+#pragma unroll
+      for (int i = 0; i < NACC / 4; ++i)
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+          *reinterpret_cast<float2*>(of_s + off32(r0 + 8 * h, i)) = make_float2(acc0[4 * i + 2 * h], acc0[4 * i + 2 * h + 1]);
+      fence_proxy_async_smem();                                  // the tile's generic writes -> the TMA engine
+      named_bar_sync(1, CONSUMER_THREADS);
+      if (ct == 0) {
+        for (int j = 0; j < BN / 32 && n0 + 32 * j < p.cout; ++j)
+          tma_store_3d(&map_o, smem_u32(of_s + j * (BM * 32)), n0 + 32 * j, l0, b0);
+        bulk_commit();
+      }
+    }
+    // the plane count as a constant where it is the operand split (every engine call), else read at run time
+    auto planes = [&](auto ons) {
+      constexpr int ONS = decltype(ons)::value;
+#pragma unroll
+      for (int i = 0; i < NACC / 4; ++i)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          uint32_t w[3];
+          pm_split_pair_t<F16, ONS>(acc0[4 * i + 2 * h], acc0[4 * i + 2 * h + 1], p.out_nsplit, w);
+          // byte offset of (row r, column c) in a [BN / 64][BM][64 halves] swizzled plane tile
+          const int o = (i >> 3) * (BM * 128) + (r0 + 8 * h) * 128 + (((i & 7) ^ sw) << 4) + 4 * t4;
+#pragma unroll
+          for (int pl = 0; pl < 3; ++pl)
+            if (pl < (ONS ? ONS : p.out_nsplit)) *reinterpret_cast<uint32_t*>(pl_s + pl * PLANE_BYTES + o) = w[pl];
+        }
+    };
+    if (p.out_nsplit) {
+      if (p.out_nsplit == NSPLIT) planes(std::integral_constant<int, NSPLIT>{});
+      else planes(std::integral_constant<int, 0>{});
+      fence_proxy_async_smem();
+      named_bar_sync(1, CONSUMER_THREADS);
+      if (ct == 0) {
+        for (int pl = 0; pl < p.out_nsplit; ++pl)
+          for (int j = 0; j < BN / 64 && n0 + 64 * j < p.cout; ++j)
+            tma_store_4d(&map_p, smem_u32(pl_s + pl * PLANE_BYTES + j * (BM * 128)), n0 + 64 * j, l0, b0, pl);
+        bulk_commit();
+      }
+    }
+    if (warp == STAMP_WARP) PM_STAMP(5);                      // the stores issued
+    if (ct == 0) bulk_wait_read0();                            // the tiles must stay until the TMA engine has read them
+    if (warp == STAMP_WARP) PM_STAMP(6);                       // their shared-memory reads complete
+    return;
+  }
   {
     const int wq = warp & 3, t4 = lane & 3;
     const int r0 = wg * 64 + wq * 16 + (lane >> 2);
@@ -382,16 +484,33 @@ __global__ void __launch_bounds__(256) split_bf16_kernel(const float* __restrict
 }
 
 // ---------------------------------------------------------------------------------------------------
+// The operand ring of an instance: as many stages of nsplit A and W tiles as fit RING_KB, at most MAX_STAGES.
+constexpr int stage_bytes_of(int bn, int nsplit) { return nsplit * (A_TILE_BYTES + bn * BK * 2); }
+constexpr int stages_of(int bn, int nsplit) {
+  return RING_KB * 1024 / stage_bytes_of(bn, nsplit) < MAX_STAGES ? RING_KB * 1024 / stage_bytes_of(bn, nsplit) : MAX_STAGES;
+}
+constexpr int ring_bytes_of(int bn, int nsplit) { return stages_of(bn, nsplit) * stage_bytes_of(bn, nsplit); }
+// Whether the TMA-store epilogue's tiles fit the ring: fp32 tile and out_nsplit plane tiles from its start, the
+// residual tile at its end.
+constexpr bool tma_out_fits(int bn, int nsplit, bool f32, int out_nsplit, bool residual) {
+  return (f32 ? BM * bn * 4 : 0) + out_nsplit * BM * bn * 2 + (residual ? BM * bn * 4 : 0) <= ring_bytes_of(bn, nsplit);
+}
+
 template <int BN, bool F16, int NSPLIT>
-int launch(const CUtensorMap& ma, const CUtensorMap& mw, const CUtensorMap& mr, TcParams& p, dim3 grid, cudaStream_t st) {
-  constexpr int stage_bytes = NSPLIT * (A_TILE_BYTES + BN * BK * 2);
-  constexpr int stages = RING_KB * 1024 / stage_bytes < MAX_STAGES ? RING_KB * 1024 / stage_bytes : MAX_STAGES;
+int launch(const CUtensorMap& ma, const CUtensorMap& mw, const CUtensorMap& mr, const CUtensorMap& mo,
+           const CUtensorMap& mp, TcParams& p, dim3 grid, cudaStream_t st) {
+  constexpr int stage_bytes = stage_bytes_of(BN, NSPLIT);
+  constexpr int stages = stages_of(BN, NSPLIT);
   static_assert(stages >= 2, "the operand ring needs two stages");
-  // The epilogue's staging tile (ring start) and residual tile (ring end) must not overlap, and the residual must
+  // The store loop's staging tile (ring start) and residual tile (ring end) must not overlap, and the residual must
   // leave the slot below it to the last k-block.
   constexpr int staging = BM * (BN + 8) * 4, res_bytes = BM * BN * 4;
   static_assert(staging + res_bytes <= stages * stage_bytes && res_bytes <= (stages - 1) * stage_bytes,
                 "staging and residual tiles must fit the ring side by side");
+  // The TMA-store epilogue fits with the fp32 tile, two plane tiles and the residual (the fp16x3 engine's widest
+  // call); three planes beside fp32 and a residual at BN = 128 take the store loop (pm_tapgemm_tc checks).
+  static_assert(tma_out_fits(BN, NSPLIT, true, 2, true), "fp32, two plane and residual tiles must fit the ring");
+  static_assert(BN * 4 * BM % 1024 == 0 && stage_bytes % 1024 == 0, "128B-swizzled TMA boxes need 1024-byte alignment");
   p.stages = stages;
   p.res_slot0 = (stages * stage_bytes - res_bytes) / stage_bytes;
   p.rot = (p.res_slot0 - 1 - (p.taps * p.kblocks - 1) % stages + stages) % stages;
@@ -401,21 +520,20 @@ int launch(const CUtensorMap& ma, const CUtensorMap& mw, const CUtensorMap& mr, 
     cudaError_t e = cudaFuncSetAttribute(tapgemm_tc_kernel<BN, F16, NSPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
     if (e != cudaSuccess) { configured = 0; return (int)e; }
   }
-  tapgemm_tc_kernel<BN, F16, NSPLIT><<<grid, NUM_THREADS, smem, st>>>(ma, mw, mr, p);
+  tapgemm_tc_kernel<BN, F16, NSPLIT><<<grid, NUM_THREADS, smem, st>>>(ma, mw, mr, mo, mp, p);
   PM_LAUNCH_CHECK();
 }
 
 template <int BN>
-int launch_fmt(const CUtensorMap& ma, const CUtensorMap& mw, const CUtensorMap& mr, TcParams& p, dim3 grid, cudaStream_t st,
-               bool f16) {
+int launch_fmt(const CUtensorMap* m, TcParams& p, dim3 grid, cudaStream_t st, bool f16) {
   if (f16) {
-    if (p.nsplit == 1) return launch<BN, true, 1>(ma, mw, mr, p, grid, st);
-    if (p.nsplit == 2) return launch<BN, true, 2>(ma, mw, mr, p, grid, st);
-    return launch<BN, true, 3>(ma, mw, mr, p, grid, st);
+    if (p.nsplit == 1) return launch<BN, true, 1>(m[0], m[1], m[2], m[3], m[4], p, grid, st);
+    if (p.nsplit == 2) return launch<BN, true, 2>(m[0], m[1], m[2], m[3], m[4], p, grid, st);
+    return launch<BN, true, 3>(m[0], m[1], m[2], m[3], m[4], p, grid, st);
   }
-  if (p.nsplit == 1) return launch<BN, false, 1>(ma, mw, mr, p, grid, st);
-  if (p.nsplit == 2) return launch<BN, false, 2>(ma, mw, mr, p, grid, st);
-  return launch<BN, false, 3>(ma, mw, mr, p, grid, st);
+  if (p.nsplit == 1) return launch<BN, false, 1>(m[0], m[1], m[2], m[3], m[4], p, grid, st);
+  if (p.nsplit == 2) return launch<BN, false, 2>(m[0], m[1], m[2], m[3], m[4], p, grid, st);
+  return launch<BN, false, 3>(m[0], m[1], m[2], m[3], m[4], p, grid, st);
 }
 
 // N tile of a launch: a pure function of the shape and the SM count, so a captured graph keeps its choice.
@@ -448,6 +566,7 @@ extern "C" int pm_tapgemm_tc(const uint16_t* A, long long a_ps, long long a_bs, 
                              const void* prefetch, long long prefetch_bytes, void* stream) {
   PM_REQUIRE(A && W && (out_f32 || out_bf16));
   const int tile = (nsplit >> PM_TC_TILE_SHIFT) & 0xff;   // N tile override: 0 automatic, 1 = 64, 2 = 128 columns
+  const bool store_loop = (nsplit & PM_TC_STORE_LOOP) != 0;   // force the per-element store loop (tests, A/B runs)
   PM_TAKE_FMT(nsplit, f16);                 // operand planes: bf16 (default) or fp16
   PM_TAKE_FMT(out_nsplit, out_f16);
   PM_REQUIRE(!out_bf16 || out_f16 == f16);  // emitted planes use the operand format
@@ -490,7 +609,9 @@ extern "C" int pm_tapgemm_tc(const uint16_t* A, long long a_ps, long long a_bs, 
   p.prefetch = static_cast<const uint8_t*>(prefetch);
   p.prefetch_bytes = prefetch ? prefetch_bytes : 0;
   p.acc_scale = acc_scale;
-  CUtensorMap ma, mw;
+  CUtensorMap m[5];   // A, W, residual, fp32 output, output planes
+  std::memset(m, 0, sizeof(m));
+  CUtensorMap &ma = m[0], &mw = m[1], &mr = m[2], &mo = m[3], &mp = m[4];
   {
     const long long bs_el = batch > 1 ? a_bs : (long long)rows_in * lda;
     const long long ps_el = nsplit > 1 ? a_ps : bs_el * batch;
@@ -508,22 +629,48 @@ extern "C" int pm_tapgemm_tc(const uint16_t* A, long long a_ps, long long a_bs, 
   }
   // The residual tile by TMA where it can describe the view (16-byte base and strides); the box is the output tile,
   // zero-filled past cout / rows_out / batch.  Any other view (or one the driver declines to encode) is read per
-  // element in the epilogue.
-  CUtensorMap mr;
-  std::memset(&mr, 0, sizeof(mr));
-  p.res_tma = residual && (reinterpret_cast<uintptr_t>(residual) & 15) == 0 && (ldr & 3) == 0 && (batch == 1 || (r_bs & 3) == 0);
-  if (p.res_tma) {
+  // element in the store loop.
+  const bool res_ok = residual && (reinterpret_cast<uintptr_t>(residual) & 15) == 0 && (ldr & 3) == 0 && (batch == 1 || (r_bs & 3) == 0);
+  // The outputs by TMA stores where TMA can describe every output view (16-byte base and strides), the residual (if
+  // any) is TMA-loaded and the tiles fit the ring.  Boxes of 32 fp32 / 64 plane elements (one 128-byte swizzle row)
+  // x R rows x NB clips, clipped at cout / rows_out / batch; views at an offset (a window's rows, a column slice) are
+  // just another base.  Every other case, or a view the driver declines to encode, keeps the per-element store loop.
+  bool tma_out = !store_loop && (!residual || res_ok) && tma_out_fits(BNsel, nsplit, out_f32, p.out_nsplit, residual);
+  if (tma_out && out_f32) {
+    tma_out = (reinterpret_cast<uintptr_t>(out_f32) & 15) == 0 && (ldo & 3) == 0 && (batch == 1 || (o_bs & 3) == 0);
+    const long long bs_el = batch > 1 ? o_bs : (long long)rows_out * ldo;
+    cuuint64_t dims[3] = {(cuuint64_t)cout, (cuuint64_t)rows_out, (cuuint64_t)batch};
+    cuuint64_t strides[2] = {(cuuint64_t)ldo * 4, (cuuint64_t)bs_el * 4};
+    cuuint32_t box[3] = {32, (cuuint32_t)R, (cuuint32_t)NB};
+    tma_out = tma_out && encode_tiled(&mo, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, CU_TENSOR_MAP_SWIZZLE_128B, out_f32, 3, dims, strides, box);
+  }
+  if (tma_out && out_bf16) {
+    tma_out = (reinterpret_cast<uintptr_t>(out_bf16) & 15) == 0 && (ldob & 7) == 0 && (batch == 1 || (ob_bs & 7) == 0) &&
+              (out_nsplit == 1 || (ob_ps & 7) == 0);
+    const long long bs_el = batch > 1 ? ob_bs : (long long)rows_out * ldob;
+    const long long ps_el = out_nsplit > 1 ? ob_ps : bs_el * batch;
+    cuuint64_t dims[4] = {(cuuint64_t)cout, (cuuint64_t)rows_out, (cuuint64_t)batch, (cuuint64_t)out_nsplit};
+    cuuint64_t strides[3] = {(cuuint64_t)ldob * 2, (cuuint64_t)bs_el * 2, (cuuint64_t)ps_el * 2};
+    cuuint32_t box[4] = {64, (cuuint32_t)R, (cuuint32_t)NB, 1};
+    tma_out = tma_out && encode_map(&mp, out_bf16, 4, dims, strides, box, f16);
+  }
+  // the TMA-store epilogue reads the residual in its output tile's layout: BN / 32 swizzled 32-column boxes
+  p.res_tma = false;
+  for (int swz = tma_out; res_ok && !p.res_tma && swz >= 0; --swz) {
     const long long bs_el = batch > 1 ? r_bs : (long long)rows_out * ldr;
     cuuint64_t dims[3] = {(cuuint64_t)cout, (cuuint64_t)rows_out, (cuuint64_t)batch};
     cuuint64_t strides[2] = {(cuuint64_t)ldr * 4, (cuuint64_t)bs_el * 4};
-    cuuint32_t box[3] = {(cuuint32_t)BNsel, (cuuint32_t)R, (cuuint32_t)NB};
-    p.res_tma = encode_tiled(&mr, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, CU_TENSOR_MAP_SWIZZLE_NONE, residual, 3, dims, strides, box);
+    cuuint32_t box[3] = {swz ? 32u : (cuuint32_t)BNsel, (cuuint32_t)R, (cuuint32_t)NB};
+    p.res_tma = encode_tiled(&mr, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, swz ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE,
+                             residual, 3, dims, strides, box);
+    if (!p.res_tma) tma_out = false;
   }
+  p.tma_out = tma_out;
   dim3 grid(pm_cdiv(rows_out, R), pm_cdiv(cout, BNsel), pm_cdiv(batch, NB));
   PM_REQUIRE(grid.z <= 65535 && grid.y <= 65535);
   const cudaStream_t st = (cudaStream_t)stream;
-  if (BNsel == 128) return launch_fmt<128>(ma, mw, mr, p, grid, st, f16);
-  return launch_fmt<64>(ma, mw, mr, p, grid, st, f16);
+  if (BNsel == 128) return launch_fmt<128>(m, p, grid, st, f16);
+  return launch_fmt<64>(m, p, grid, st, f16);
 }
 
 #ifdef PM_TC_TIMING

@@ -22,6 +22,7 @@ launch_count = 0
 # match three bf16 planes (6 products) in accuracy while magnitudes stay below 65504 (include/pm_emage.h).
 FMT_F16 = 0x100
 TC_TILE_SHIFT = 16           # pm_tapgemm_tc: N tile override in bits 16-23 of nsplit (PM_TC_TILE_SHIFT)
+TC_STORE_LOOP = 1 << 24      # pm_tapgemm_tc: force the per-element store loop (PM_TC_STORE_LOOP)
 # fp16 activation planes hold F16_ACT_SCALE * x (csrc/pm_common.cuh PM_F16_ACT_SCALE: the tensor core flushes fp16
 # subnormal operands, the exact pre-scale keeps second planes normal down to |x| = 2^-9); PackedW.acc_scale undoes it.
 F16_ACT_SCALE = 64.0
@@ -497,11 +498,13 @@ class PackedW:
 
 
 def tapgemm_tc(a: Planes, w: PackedW, bias, *, rows_in=None, rows_out, pad=0, act=ACT_NONE, act_cols=0, slope=0.0,
-               residual=None, want_f32=True, out_nsplit=0, out=None, a_view=None, out_slack=0, prefetch=None, tile=0):
+               residual=None, want_f32=True, out_nsplit=0, out=None, a_view=None, out_slack=0, prefetch=None, tile=0,
+               store_loop=False):
     """Tensor-core tap-GEMM.  `prefetch`: a tensor (the next GEMM's packed weights) to pull into L2 meanwhile.
     `a_view` = (rows_in, cin, lda) overrides the logical view of the A planes
     (strided convs pass the (rows/s, s*C) view of the same memory).  `tile` forces the kernel's N tile (64 or 128
-    columns; 0 = chosen from the shape), for tests and A/B runs: results are bit-identical either way.
+    columns; 0 = chosen from the shape), for tests and A/B runs: results are bit-identical either way.  `store_loop`
+    forces the epilogue's per-element store loop instead of its TMA stores (tests, A/B runs; the same bits).
     Returns (fp32 out | None, Planes | None)."""
     t = a.t
     nsplit, batch = t.shape[0], t.shape[1]
@@ -527,7 +530,7 @@ def tapgemm_tc(a: Planes, w: PackedW, bias, *, rows_in=None, rows_out, pad=0, ac
         _chk(residual)
         assert residual.shape == (batch, rows_out, cout)
     _call("pm_tapgemm_tc", t.data_ptr(), t.stride(0), t.stride(1), lda, batch, rows_a, cin,
-          w.t.data_ptr(), w.t.stride(0), w.w_rows, w.ldw, w.taps, pad, nsplit | fmt | (tile // 64) << TC_TILE_SHIFT,
+          w.t.data_ptr(), w.t.stride(0), w.w_rows, w.ldw, w.taps, pad, nsplit | fmt | (tile // 64) << TC_TILE_SHIFT | (TC_STORE_LOOP if store_loop else 0),
           _ptr(bias), rows_out, cout, _ptr(residual), r_bs, ldr, act, act_cols, float(slope), float(w.acc_scale),
           _ptr(out_f), o_bs, ldo,
           None if out_p is None else out_p.t.data_ptr(), 0 if out_p is None else out_p.t.stride(0),

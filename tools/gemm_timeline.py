@@ -4,8 +4,9 @@
     PM_EMAGE_LIB=pantomatrix_b200/csrc/_build/variants/libpm_emage_timing.so python tools/gemm_timeline.py
 
 Stamps, one set per CTA (= per output tile), written by the first consumer warp (cycles of the CTA's SM clock, relative
-to kernel entry of that CTA): prologue done, first operand stage landed, all MMAs issued, accumulators complete, this
-warp's epilogue issued, all consumer warps done.  The launch uses the automatically chosen N tile.  The launch-to-launch
+to kernel entry of that CTA): prologue done, first operand stage landed, all MMAs issued, accumulators complete, then
+for the TMA-store epilogue the output tiles' stores issued and their shared-memory reads complete, for the
+per-element store loop this warp's share issued and all consumer warps done.  The launch uses the automatically chosen N tile.  The launch-to-launch
 period (CUDA events around a replayed graph of 20 launches) minus the in-kernel span is launch / drain / tail cost.
 The first line printed is the card record."""
 import ctypes
