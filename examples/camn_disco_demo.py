@@ -46,6 +46,8 @@ def main():
     ap.add_argument("--render", action="store_true")
     ap.add_argument("--video", action="store_true", help="write <npz base>.mp4 (needs --smplx)")
     ap.add_argument("--with-audio", action="store_true", help="put the WAV's sound in the --video file")
+    ap.add_argument("--gop", type=int, default=1,
+                    help="--video keyframe interval: an IDR frame every GOP frames, P frames between (1: all IDR)")
     args = ap.parse_args()
     if not args.trans_zero and args.smplx is None:
         ap.error("the npz needs a pelvis translation: pass --smplx SMPLX_NEUTRAL_2020.npz, or --trans-zero to write zeros")
@@ -55,6 +57,8 @@ def main():
         ap.error("--video needs --smplx SMPLX_NEUTRAL_2020.npz")
     if args.with_audio and not args.video:
         ap.error("--with-audio needs --video")
+    if args.gop < 1:
+        ap.error("--gop must be at least 1")
     device = torch.device("cuda")
     body_model = renderer = None
     if args.smplx is not None:
@@ -93,7 +97,7 @@ def main():
                 from pantomatrix_b200 import video
                 video.write_mp4(drawn, os.path.splitext(npz)[0] + ".mp4", fps=30,
                                 audio=read_track(os.path.join(args.audio_folder, name), device)
-                                if args.with_audio else None)
+                                if args.with_audio else None, gop=args.gop)
         frames += t
     print(f"generate total {frames / fps:.2f} seconds motion in {time.time() - t0:.2f} seconds, saved in {args.save_folder}")
 

@@ -375,9 +375,42 @@ int pm_png_crc(int n_frames, int h, int w, unsigned char* data, long long cap, c
  *   pm_memset_async(data, 0, n_frames * cap), pm_h264_encode, pm_h264_gather.
  * pm_h264_encode: one warp per (frame, row): the slice into scratch + (f h / 16 + row) slice_cap, its length prefix
  *   included, and its byte count into slice_bytes.
- * pm_h264_gather: one CTA per (frame, row): the slice copied to its offset in the frame's slot; nbytes[f] the sum. */
+ * pm_h264_gather: one CTA per (frame, row): the slice copied to its offset in the frame's slot; nbytes[f] the sum.
+ *
+ * pm_h264_encode_gop: the same with keyframe interval 1 <= gop <= clip_len; gop 1 is pm_h264_encode (recon unused).
+ * n_frames is a multiple of clip_len.  Any gop >= clip_len gives the bytes of gop = clip_len, so a caller with a
+ * larger gop passes clip_len.  Frame t of a clip is an IDR frame when t mod gop == 0, coded as above with idr_pic_id =
+ * (t div gop) mod 2, else a P frame against the reconstruction of frame t - 1:
+ *   SPS (video.sps(h, w, gop)): max_num_ref_frames 1 when gop > 1; the PPS is unchanged;
+ *   P picture: one P slice per row, nal_ref_idc 2, nal_unit_type 1: first_mb_in_slice, slice_type 5, pps id 0,
+ *     frame_num = (t mod gop) mod 16 (4 bits, wraps), num_ref_idx_active_override_flag 0,
+ *     ref_pic_list_modification_flag_l0 0, adaptive_ref_pic_marking_mode_flag 0, slice_qp_delta, and
+ *     disable_deblocking_filter_idc 1;
+ *   motion: always (0, 0).  The macroblock above lies in another slice, so the P_Skip vector and every predictor are
+ *     (0, 0); the prediction is the co-located 16x16 luma and 8x8 chroma of the reference, and a row reads only the
+ *     same row of the reference;
+ *   macroblock: the inter candidate is source - reference with the 4x4 transform of all 16 luma coefficients (no luma
+ *     DC Hadamard), the chroma DC / AC split as intra, and f = 2^qbits / 6 for every level.  P_Skip when every inter
+ *     level is 0 (the reconstruction is the reference).  Else P_L0_16x16 (mb_type 0, mvd (0, 0), coded_block_pattern
+ *     by Table 9-4's Inter column: luma bit b8 when a 4x4 block of 8x8 block b8 has a level, chroma 0 / 1 / 2 as intra;
+ *     mb_qp_delta 0 only when cbp > 0; luma residual_block(16) per 4x4 block of each set 8x8 bit) when the luma SAD
+ *     against the reference is <= the Intra16x16 candidate's SAD, else Intra16x16 as above with mb_type + 5.  I_PCM
+ *     (mb_type 30) in the same cases as above.  nC: a P_Skip neighbour counts 0, I_PCM 16.  mb_skip_run ue(v) before
+ *     every coded macroblock, and after the last one when the slice ends in skips;
+ *   bound: a slice has at most P = ceil((70 + 3201 w / 16 + 8) / 8) RBSP bytes (the longest slice header; at most 3201
+ *     bits per macroblock with its share of the skip runs), so slice_cap >= 4 + P + P / 2, and data's slots hold
+ *     (h / 16) times that (video.slot_bytes(h, w, gop)).
+ * One warp per (chain, row), a chain being one GOP of one clip: the warp codes the chain's frames in order and keeps
+ * the row's reconstruction (luma 16 x w, then Cb and Cr 8 x w / 2) in recon + (chain h / 16 + row) recon_stride,
+ * recon_stride >= 24 w, (n_frames / clip_len) ceil(clip_len / gop) (h / 16) rows of workspace.  Each GOP's IDR frame
+ * writes it before the P frames read it, so it needs no clearing.  Launch order: as pm_h264_encode.
+ * pm_h264_gather checks cap and slice_cap against the gop = 1 bound only; with gop > 1 the caller sizes both by the
+ * gop > 1 bound above (video.slice_bytes(w, gop), video.slot_bytes(h, w, gop)). */
 int pm_h264_encode(const unsigned char* frames, long long f_fs, int n_frames, int clip_len, int h, int w, int qp,
                    unsigned char* scratch, long long slice_cap, int* slice_bytes, void* stream);
+int pm_h264_encode_gop(const unsigned char* frames, long long f_fs, int n_frames, int clip_len, int h, int w, int qp,
+                       unsigned char* scratch, long long slice_cap, int* slice_bytes, int gop, unsigned char* recon,
+                       long long recon_stride, void* stream);
 int pm_h264_gather(int n_frames, int h, int w, const unsigned char* scratch, long long slice_cap,
                    const int* slice_bytes, unsigned char* data, long long cap, long long* nbytes, void* stream);
 

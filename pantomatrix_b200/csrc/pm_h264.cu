@@ -1,13 +1,18 @@
-// H.264 encoding of RGB8 frames (pantomatrix_b200/video.py): one IDR access unit per frame by the rule of
-// include/pm_emage.h and DESIGN.md section 12 (one I slice per macroblock row, Intra16x16 DC / Horizontal or I_PCM,
-// CAVLC, deblocking off).  Two launches per call after the caller's memset of the output slots:
+// H.264 encoding of RGB8 frames (pantomatrix_b200/video.py): one access unit per frame by the rule of
+// include/pm_emage.h and DESIGN.md section 12 (one slice per macroblock row, Intra16x16 DC / Horizontal or I_PCM,
+// CAVLC, deblocking off; with a keyframe interval gop > 1, P frames of P_Skip and zero-motion inter macroblocks
+// between the IDR frames).  Two launches per call after the caller's memset of the output slots:
 //   pm_h264_encode  one warp per (frame, macroblock row): the row's slice, emulation prevention applied, into its
-//                   scratch slot, and the slice's size;
+//                   scratch slot, and the slice's size; pm_h264_encode_gop: one warp per (GOP, row), walking the
+//                   GOP's frames in order;
 //   pm_h264_gather  one CTA per (frame, row): the slice's offset in the frame's sample, the copy, the frame's size.
 // A warp stages its bits in shared memory in stream byte order (pm_put_bits, as FLAC writes its slots), so whole
 // bytes leave the staging buffer as byte loads.
-// CPU restatement: oracle/h264_oracle.py.  Every byte depends only on the frame, qp and its index parity.
+// CPU restatement: oracle/h264_oracle.py, and tests/h264_gop_ref.py for P frames.  Every byte depends only on the
+// frame (its GOP's frames), qp, gop and the parity of its index (t div gop).
 #include <cub/block/block_reduce.cuh>
+
+#include <type_traits>
 
 #include "pm_common.cuh"
 #include "../../include/pm_emage.h"
@@ -16,7 +21,8 @@ namespace {
 
 constexpr int WARPS = 4;                  // warps (slices) per CTA of pm_h264_encode
 constexpr int MB_BITS_LIMIT = 3200;       // 128 + RawMbBits (A.3.1)
-constexpr int SLICE_HEADER_BITS = 62;     // NAL header byte and the longest slice header
+constexpr int SLICE_HEADER_BITS = 62;     // NAL header byte and the slice header, as the gop = 1 bound counts it
+constexpr int SLICE_HEADER_BITS_GOP = 70; // the longest slice header of either kind: IDR, last row, qp 0
 constexpr int STG_WORDS = 128;            // staging bits of one warp: header + one macroblock < 4096 bits
 constexpr int GATHER_THREADS = 256;
 
@@ -211,16 +217,32 @@ __device__ __forceinline__ int quant(int w, int mf, int f, int qbits) {
   return w < 0 ? -q : q;
 }
 
+// Table 9-4 (ChromaArrayType 1): codeNum of each coded_block_pattern of an Inter macroblock.
+__constant__ unsigned char INTER_CODE[48] = {0,  2,  3,  7,  4,  8,  17, 13, 5,  18, 9,  14, 10, 15, 16, 11,
+                                             1,  32, 33, 36, 34, 37, 44, 40, 35, 45, 38, 41, 39, 42, 43, 19,
+                                             6,  24, 25, 20, 26, 21, 46, 28, 27, 47, 22, 29, 23, 30, 31, 12};
+
+// The reference samples of a P frame's macroblock: the co-located samples of the previous reconstruction.
+struct WarpRef {
+  unsigned char ry[256], rc[2][64];
+  __device__ __forceinline__ int ref(int k, int i) const { return k < 0 ? ry[i] : rc[k][i]; }
+};
+struct WarpNoRef {
+  __device__ __forceinline__ int ref(int, int) const { return 0; }
+};
+
 // One warp's state.  Units of a macroblock_layer(), in syntax order: 0 header, 1 luma DC, 2..17 luma AC by
-// luma4x4BlkIdx, 18 / 19 chroma DC Cb / Cr, 20..27 chroma AC Cb 0..3, Cr 0..3; lev[u - 1] holds unit u's levels.
-struct Warp {
+// luma4x4BlkIdx, 18 / 19 chroma DC Cb / Cr, 20..27 chroma AC Cb 0..3, Cr 0..3; lev[u - 1] holds unit u's levels.  An
+// inter macroblock has no unit 1, and its luma units 2..17 hold all 16 levels of their block.
+template <bool GOP>
+struct Warp : std::conditional_t<GOP, WarpRef, WarpNoRef> {
   unsigned stg[STG_WORDS];
   int lev[27][16];
   int dcw[16], cdcw[2][4];                 // DC of each block's forward transform (raster)
   int dcy[16], dcc[2][4];                  // scaled DC (8.5.10, 8.5.11.1)
   int tc[24];                              // TotalCoeff of the AC blocks: luma raster 0..15, chroma 16 + 4 k + raster
   int ly[16], lc[2][8];                    // left neighbour: reconstructed right column
-  int ny[16], nc[2][8];                    // this macroblock's Intra16x16 right column
+  int ny[16], nc[2][8];                    // this macroblock's reconstructed right column
   int lnz[8];                              // left neighbour's right blocks' TotalCoeff: luma rows, Cb rows, Cr rows
   unsigned char y[256], cb[64], cr[64];    // source samples
 };
@@ -269,6 +291,8 @@ __device__ __forceinline__ int warp_sum(int v) {
   return v;
 }
 
+__device__ __forceinline__ int ue_bits(unsigned k) { return 2 * (32 - __clz(k + 1)) - 1; }
+
 struct Job {
   const unsigned char* px;   // frame 0, pixel (0, 0)
   long long fs;              // frame stride (bytes)
@@ -276,309 +300,438 @@ struct Job {
   unsigned char* scratch;
   long long slice_cap;
   int* slice_bytes;
+  int gop, chains_per_clip;  // GOP: frames per GOP, GOPs per clip
+  unsigned char* recon;      // GOP: one macroblock row's reconstruction per (chain, row), recon_stride apart
+  long long recon_stride;
 };
 
 __device__ __forceinline__ void rgb(const unsigned char* p, int& r, int& g, int& b) { r = p[0]; g = p[1]; b = p[2]; }
 
+// One warp per (chain, macroblock row).  A chain is one frame (GOP false: every frame IDR) or one GOP of one clip
+// (GOP true): the warp codes the row of each of the chain's frames in turn, the IDR frame first, and keeps the row's
+// reconstruction in J.recon for the next frame's P slice.
+template <bool GOP>
 __global__ void __launch_bounds__(32 * WARPS) h264_encode_kernel(Job J) {
-  __shared__ Warp WS[WARPS];
+  __shared__ Warp<GOP> WS[WARPS];
   const int lane = threadIdx.x & 31;
-  Warp& S = WS[threadIdx.x >> 5];
+  Warp<GOP>& S = WS[threadIdx.x >> 5];
   const int mbw = J.w >> 4, mbh = J.h >> 4;
   const long long slice = (long long)blockIdx.x * WARPS + (threadIdx.x >> 5);
-  if (slice >= (long long)J.n_frames * mbh) return;
-  const long long f = slice / mbh;
+  const long long chains = GOP ? (long long)(J.n_frames / J.clip_len) * J.chains_per_clip : J.n_frames;
+  if (slice >= chains * mbh) return;
+  const long long chain = slice / mbh;
   const int my = (int)(slice % mbh);
-  const unsigned char* fr = J.px + f * J.fs;
-  const int qp = J.qp, qpc = QPC[qp];
-  unsigned char* out = J.scratch + slice * J.slice_cap;
-  long long at = 4;                                      // the 4-byte length prefix goes first
-  int zrun = 0;
-
-  for (int i = lane; i < STG_WORDS; i += 32) S.stg[i] = 0;
-  __syncwarp();
-  int pend;                                              // bits in the staging buffer
-  {
-    Bits<true> b{S.stg, 0};
-    if (lane == 0) {
-      b.put(0x65, 8);                                    // nal_ref_idc 3, nal_unit_type 5 (IDR)
-      b.ue((unsigned)(my * mbw));                        // first_mb_in_slice
-      b.ue(7);                                           // slice_type I (every slice of the picture)
-      b.ue(0);                                           // pic_parameter_set_id
-      b.put(0, 4);                                       // frame_num
-      b.ue((unsigned)((f % J.clip_len) & 1));            // idr_pic_id
-      b.put(0, 2);                                       // no_output_of_prior_pics_flag, long_term_reference_flag
-      b.se(qp - 26);                                     // slice_qp_delta
-      b.ue(1);                                           // disable_deblocking_filter_idc
-    }
-    pend = __shfl_sync(0xffffffffu, b.pos, 0);
+  long long f0;                                          // the chain's first frame, at index t0 of its clip
+  int t0, t1;
+  if (GOP) {
+    t0 = (int)(chain % J.chains_per_clip) * J.gop;
+    t1 = min(t0 + J.gop, J.clip_len);
+    f0 = chain / J.chains_per_clip * J.clip_len + t0;
+  } else {
+    f0 = chain;
+    t0 = (int)(chain % J.clip_len);
+    t1 = t0 + 1;
   }
-
+  unsigned char* const rrow = GOP ? J.recon + slice * J.recon_stride : nullptr;   // Y 16 x w, Cb, Cr 8 x w / 2
+  const int qp = J.qp, qpc = QPC[qp];
   const int mf0 = MF[qp % 6][0], qbits = 15 + qp / 6, fq = (1 << qbits) / 3;
   const int cmf0 = MF[qpc % 6][0], cqbits = 15 + qpc / 6, cfq = (1 << cqbits) / 3;
 
-  for (int mx = 0; mx < mbw; ++mx) {
-    const bool have_left = mx > 0;
-    // ---- source samples (colour rule) ----
-    for (int p = lane; p < 256; p += 32) {
-      int r, g, bb;
-      rgb(fr + ((long long)(16 * my + (p >> 4)) * J.w + 16 * mx + (p & 15)) * 3, r, g, bb);
-      S.y[p] = (unsigned char)(((66 * r + 129 * g + 25 * bb + 128) >> 8) + 16);
-    }
-    for (int p = lane; p < 64; p += 32) {
-      const int yy = 16 * my + 2 * (p >> 3), xx = 16 * mx + 2 * (p & 7);
-      int rs = 0, gs = 0, bs = 0;
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        int r, g, bb;
-        rgb(fr + ((long long)(yy + (q >> 1)) * J.w + xx + (q & 1)) * 3, r, g, bb);
-        rs += r; gs += g; bs += bb;
-      }
-      S.cb[p] = (unsigned char)(((-38 * rs - 74 * gs + 112 * bs + 512) >> 10) + 128);
-      S.cr[p] = (unsigned char)(((112 * rs - 94 * gs - 18 * bs + 512) >> 10) + 128);
-    }
+  for (int t = t0; t < t1; ++t) {
+    const long long f = f0 + (t - t0);
+    const bool pf = GOP && t > t0;                       // a P frame: every frame of a GOP after its IDR frame
+    const unsigned char* fr = J.px + f * J.fs;
+    const long long row = GOP ? f * mbh + my : slice;    // this slice's index in scratch and slice_bytes
+    unsigned char* out = J.scratch + row * J.slice_cap;
+    long long at = 4;                                      // the 4-byte length prefix goes first
+    int zrun = 0;
+
+    for (int i = lane; i < STG_WORDS; i += 32) S.stg[i] = 0;
     __syncwarp();
-    // ---- prediction: DC, or Horizontal when its SAD is strictly lower ----
-    int dc = 128;
-    if (have_left) {
-      int s = 0;
-#pragma unroll
-      for (int r = 0; r < 16; ++r) s += S.ly[r];
-      dc = (s + 8) >> 4;
-    }
-    int sad_dc = 0, sad_h = 0;
-    for (int p = lane; p < 256; p += 32) {
-      sad_dc += abs((int)S.y[p] - dc);
-      if (have_left) sad_h += abs((int)S.y[p] - S.ly[p >> 4]);
-    }
-    sad_dc = warp_sum(sad_dc);
-    sad_h = warp_sum(sad_h);
-    const bool use_h = have_left && sad_h < sad_dc;
-    int cp[2][2];
-#pragma unroll
-    for (int k = 0; k < 2; ++k)
-#pragma unroll
-      for (int hy = 0; hy < 2; ++hy)
-        cp[k][hy] = have_left ? (S.lc[k][4 * hy] + S.lc[k][4 * hy + 1] + S.lc[k][4 * hy + 2] + S.lc[k][4 * hy + 3]
-                                 + 2) >> 2
-                              : 128;
-    // ---- forward transform and AC quantisation: lanes 0..15 luma blocks, 16..23 chroma blocks (raster) ----
-    if (lane < 24) {
-      const bool luma = lane < 16;
-      const int k = luma ? 0 : (lane - 16) >> 2, bi = luma ? lane : (lane - 16) & 3;
-      const int by = luma ? bi >> 2 : bi >> 1, bx = luma ? bi & 3 : bi & 1;
-      int x[16];
-#pragma unroll
-      for (int i = 0; i < 16; ++i) {
-        const int r = 4 * by + (i >> 2), c = 4 * bx + (i & 3);
-        if (luma) x[i] = (int)S.y[16 * r + c] - (use_h ? S.ly[r] : dc);
-        else x[i] = (int)(k ? S.cr : S.cb)[8 * r + c] - cp[k][by];
-      }
-      fdct(x);
-      const int unit = luma ? 2 + ((by >> 1) << 3) + ((bx >> 1) << 2) + ((by & 1) << 1) + (bx & 1)
-                            : 20 + 4 * k + bi;
-      const int q = luma ? qp : qpc;
-      const int qb = 15 + q / 6, fr3 = (1 << qb) / 3;
-      int total = 0;
-#pragma unroll
-      for (int s = 1; s < 16; ++s) {
-        const int rz = ZZ[s];
-        const int l = quant(x[rz], MF[q % 6][pos_class(rz)], fr3, qb);
-        S.lev[unit - 1][s - 1] = l;
-        total += l != 0;
-      }
-      S.tc[lane] = total;
-      if (luma) S.dcw[bi] = x[0];
-      else S.cdcw[k][bi] = x[0];
-    }
-    __syncwarp();
-    // ---- DC paths: lane 0 luma (4x4 Hadamard), lanes 1 / 2 chroma Cb / Cr (2x2 Hadamard) ----
-    bool cdc_nz = false;
-    if (lane == 0) {
-      int d[16];
-#pragma unroll
-      for (int i = 0; i < 16; ++i) d[i] = S.dcw[i];
-      // H d H with H = [[1,1,1,1],[1,1,-1,-1],[1,-1,-1,1],[1,-1,1,-1]]: columns, then rows (exact, so any order)
-#pragma unroll
-      for (int pass = 0; pass < 2; ++pass)
-#pragma unroll
-        for (int a = 0; a < 4; ++a) {
-          const int st = pass ? 1 : 4, o = pass ? 4 * a : a;
-          const int v0 = d[o], v1 = d[o + st], v2 = d[o + 2 * st], v3 = d[o + 3 * st];
-          d[o] = v0 + v1 + v2 + v3; d[o + st] = v0 + v1 - v2 - v3;
-          d[o + 2 * st] = v0 - v1 - v2 + v3; d[o + 3 * st] = v0 - v1 + v2 - v3;
-        }
-      int z[16];
-#pragma unroll
-      for (int i = 0; i < 16; ++i) {
-        const int q = ((abs(d[i]) >> 1) * mf0 + 2 * fq) >> (qbits + 1);
-        z[i] = d[i] < 0 ? -q : q;
-      }
-#pragma unroll
-      for (int s = 0; s < 16; ++s) S.lev[0][s] = z[ZZ[s]];
-      // 8.5.10: f = H z H, then scaled with LevelScale(qp % 6, 0, 0) = 16 v0
-#pragma unroll
-      for (int pass = 0; pass < 2; ++pass)
-#pragma unroll
-        for (int a = 0; a < 4; ++a) {
-          const int st = pass ? 1 : 4, o = pass ? 4 * a : a;
-          const int v0 = z[o], v1 = z[o + st], v2 = z[o + 2 * st], v3 = z[o + 3 * st];
-          z[o] = v0 + v1 + v2 + v3; z[o + st] = v0 + v1 - v2 - v3;
-          z[o + 2 * st] = v0 - v1 - v2 + v3; z[o + 3 * st] = v0 - v1 + v2 - v3;
-        }
-      const int ls = 16 * VS[qp % 6][0];
-#pragma unroll
-      for (int i = 0; i < 16; ++i)
-        S.dcy[i] = qp >= 36 ? (z[i] * ls) << (qp / 6 - 6) : (z[i] * ls + (1 << (5 - qp / 6))) >> (6 - qp / 6);
-    } else if (lane <= 2) {
-      const int k = lane - 1;
-      const int a = S.cdcw[k][0], b = S.cdcw[k][1], c = S.cdcw[k][2], e = S.cdcw[k][3];
-      const int d[4] = {a + b + c + e, a - b + c - e, a + b - c - e, a - b - c + e};
-      int z[4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        z[i] = quant(d[i], cmf0, 2 * cfq, cqbits + 1);
-        S.lev[17 + k][i] = z[i];
-        cdc_nz |= z[i] != 0;
-      }
-      const int g[4] = {z[0] + z[1] + z[2] + z[3], z[0] - z[1] + z[2] - z[3], z[0] + z[1] - z[2] - z[3],
-                        z[0] - z[1] - z[2] + z[3]};
-      const int ls = 16 * VS[qpc % 6][0];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) S.dcc[k][i] = ((g[i] * ls) << (qpc / 6)) >> 5;
-    }
-    const bool cbp_l = __ballot_sync(0xffffffffu, lane < 16 && S.tc[lane] > 0) != 0;
-    const bool ac_c = __ballot_sync(0xffffffffu, lane >= 16 && lane < 24 && S.tc[lane] > 0) != 0;
-    const bool dc_c = __ballot_sync(0xffffffffu, cdc_nz) != 0;
-    const int cbp_c = ac_c ? 2 : (dc_c ? 1 : 0);
-    __syncwarp();
-    // ---- reconstruction of the right column: luma blocks with bx = 3, chroma blocks with bx = 1 ----
-    if ((lane < 16 && (lane & 3) == 3) || (lane >= 16 && lane < 24 && (lane & 1) == 1)) {
-      const bool luma = lane < 16;
-      const int k = luma ? 0 : (lane - 16) >> 2, bi = luma ? lane : (lane - 16) & 3;
-      const int by = luma ? bi >> 2 : bi >> 1, bx = luma ? 3 : 1;
-      const int unit = luma ? 2 + ((by >> 1) << 3) + ((bx >> 1) << 2) + ((by & 1) << 1) + (bx & 1)
-                            : 20 + 4 * k + bi;
-      const int q = luma ? qp : qpc;
-      int d[16];
-      d[0] = luma ? S.dcy[bi] : S.dcc[k][bi];
-#pragma unroll
-      for (int s = 1; s < 16; ++s) {
-        const int rz = ZZ[s];
-        const int c = S.lev[unit - 1][s - 1], ls = 16 * VS[q % 6][pos_class(rz)];
-        d[rz] = q >= 24 ? (c * ls) << (q / 6 - 4) : (c * ls + (1 << (3 - q / 6))) >> (4 - q / 6);
-      }
-      idct(d);
-#pragma unroll
-      for (int r = 0; r < 4; ++r) {
-        const int row = 4 * by + r;
-        const int pred = luma ? (use_h ? S.ly[row] : dc) : cp[k][by];
-        const int v = min(255, max(0, pred + d[4 * r + 3]));
-        if (luma) S.ny[row] = v;
-        else S.nc[k][row] = v;
-      }
-    }
-    // ---- macroblock_layer() bits per unit, then the I_PCM decision ----
-    auto unit_bits = [&](auto& b) -> bool {
-      const int u = lane;
-      if (u == 0) {
-        b.ue((unsigned)(1 + (use_h ? 1 : 2) + 4 * cbp_c + (cbp_l ? 12 : 0)));
-        b.ue(0);                                         // intra_chroma_pred_mode: DC
-        b.se(0);                                         // mb_qp_delta
-        return true;
-      }
-      if (u == 1) return residual_block(b, S.lev[0], 16, have_left ? S.lnz[0] : 0);
-      if (u < 18) {
-        if (!cbp_l) return true;
-        const int blk = u - 2;
-        const int by = ((blk >> 3) << 1) | ((blk >> 1) & 1), bx = (((blk >> 2) & 1) << 1) | (blk & 1);
-        const bool ha = bx > 0 || have_left, hb = by > 0;
-        const int na = bx > 0 ? S.tc[4 * by + bx - 1] : (have_left ? S.lnz[by] : 0);
-        const int nb = hb ? S.tc[4 * (by - 1) + bx] : 0;
-        const int nc = ha && hb ? (na + nb + 1) >> 1 : (ha ? na : nb);
-        return residual_block(b, S.lev[u - 1], 15, nc);
-      }
-      if (u < 20) return cbp_c ? residual_block(b, S.lev[u - 1], 4, -1) : true;
-      if (u < 28) {
-        if (cbp_c != 2) return true;
-        const int k = (u - 20) >> 2, bi = (u - 20) & 3, by = bi >> 1, bx = bi & 1;
-        const bool ha = bx > 0 || have_left, hb = by > 0;
-        const int na = bx > 0 ? S.tc[16 + 4 * k + 2 * by] : (have_left ? S.lnz[4 + 2 * k + by] : 0);
-        const int nb = hb ? S.tc[16 + 4 * k + bx] : 0;
-        const int nc = ha && hb ? (na + nb + 1) >> 1 : (ha ? na : nb);
-        return residual_block(b, S.lev[u - 1], 15, nc);
-      }
-      return true;
-    };
-    Bits<false> cnt{nullptr, 0};
-    const bool ok = unit_bits(cnt);
-    int excl = cnt.pos;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const int v = __shfl_up_sync(0xffffffffu, excl, o);
-      if (lane >= o) excl += v;
-    }
-    const int mb_bits = __shfl_sync(0xffffffffu, excl, 31);
-    excl -= cnt.pos;
-    const bool pcm = __ballot_sync(0xffffffffu, !ok) != 0 || mb_bits > MB_BITS_LIMIT;
-    int end;
-    if (!pcm) {
-      Bits<true> b{S.stg, pend + excl};
-      unit_bits(b);
-      end = pend + mb_bits;
-    } else {
+    int pend;                                              // bits in the staging buffer
+    {
+      Bits<true> b{S.stg, 0};
       if (lane == 0) {
-        Bits<true> b{S.stg, pend};
-        b.ue(25);                                        // I_PCM, then pcm_alignment_zero_bits
+        if (pf) {
+          b.put(0x41, 8);                                  // nal_ref_idc 2, nal_unit_type 1 (non-IDR)
+          b.ue((unsigned)(my * mbw));                      // first_mb_in_slice
+          b.ue(5);                                         // slice_type P (every slice of the picture)
+          b.ue(0);                                         // pic_parameter_set_id
+          b.put((t - t0) & 15, 4);                         // frame_num = (t mod gop) mod 16
+          b.put(0, 3);                                     // num_ref_idx_active_override_flag,
+                                                           // ref_pic_list_modification_flag_l0,
+                                                           // adaptive_ref_pic_marking_mode_flag
+        } else {
+          b.put(0x65, 8);                                  // nal_ref_idc 3, nal_unit_type 5 (IDR)
+          b.ue((unsigned)(my * mbw));                      // first_mb_in_slice
+          b.ue(7);                                         // slice_type I (every slice of the picture)
+          b.ue(0);                                         // pic_parameter_set_id
+          b.put(0, 4);                                     // frame_num
+          b.ue((unsigned)((GOP ? t / J.gop : t) & 1));               // idr_pic_id
+          b.put(0, 2);                                     // no_output_of_prior_pics_flag, long_term_reference_flag
+        }
+        b.se(qp - 26);                                     // slice_qp_delta
+        b.ue(1);                                           // disable_deblocking_filter_idc
       }
-      const int at8 = (pend + 9 + 7) >> 3;
+      pend = __shfl_sync(0xffffffffu, b.pos, 0);
+    }
+    int run = 0;                                           // P_Skip macroblocks since the last coded one
+
+    for (int mx = 0; mx < mbw; ++mx) {
+      const bool have_left = mx > 0;
+      // ---- source samples (colour rule) ----
+      for (int p = lane; p < 256; p += 32) {
+        int r, g, bb;
+        rgb(fr + ((long long)(16 * my + (p >> 4)) * J.w + 16 * mx + (p & 15)) * 3, r, g, bb);
+        S.y[p] = (unsigned char)(((66 * r + 129 * g + 25 * bb + 128) >> 8) + 16);
+      }
+      for (int p = lane; p < 64; p += 32) {
+        const int yy = 16 * my + 2 * (p >> 3), xx = 16 * mx + 2 * (p & 7);
+        int rs = 0, gs = 0, bs = 0;
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          int r, g, bb;
+          rgb(fr + ((long long)(yy + (q >> 1)) * J.w + xx + (q & 1)) * 3, r, g, bb);
+          rs += r; gs += g; bs += bb;
+        }
+        S.cb[p] = (unsigned char)(((-38 * rs - 74 * gs + 112 * bs + 512) >> 10) + 128);
+        S.cr[p] = (unsigned char)(((112 * rs - 94 * gs - 18 * bs + 512) >> 10) + 128);
+      }
+      if constexpr (GOP) {
+        if (pf) {
+          for (int p = lane; p < 256; p += 32) S.ry[p] = rrow[(p >> 4) * J.w + 16 * mx + (p & 15)];
+          for (int p = lane; p < 128; p += 32) {
+            const int k = p >> 6, q = p & 63;
+            S.rc[k][q] = rrow[16 * J.w + k * 4 * J.w + (q >> 3) * (J.w >> 1) + 8 * mx + (q & 7)];
+          }
+        }
+      }
       __syncwarp();
-      for (int i = lane; i < 384; i += 32) {
-        const int j = at8 + i;
-        const unsigned v = i < 256 ? S.y[i] : (i < 320 ? S.cb[i - 256] : S.cr[i - 320]);
-        atomicOr(S.stg + (j >> 2), v << (8 * (j & 3)));
+      int dc = 128;
+      bool use_h = false;
+      // the chroma DC prediction of rows 4 hy .. 4 hy + 3 of component k
+      auto cpred = [&](int k, int hy) {
+        return have_left ? (S.lc[k][4 * hy] + S.lc[k][4 * hy + 1] + S.lc[k][4 * hy + 2] + S.lc[k][4 * hy + 3] + 2) >> 2
+                         : 128;
+      };
+      // ---- forward transform and AC quantisation: lanes 0..15 luma blocks, 16..23 chroma blocks (raster); then the
+      // DC paths: lane 0 luma (4x4 Hadamard, intra only), lanes 1 / 2 chroma Cb / Cr (2x2 Hadamard).  An inter
+      // macroblock transforms source - reference, quantises all 16 luma levels, and rounds with f = 2^qbits / 6. ----
+      auto transform = [&](bool inter) -> bool {
+        if (lane < 24) {
+          const bool luma = lane < 16;
+          const int k = luma ? 0 : (lane - 16) >> 2, bi = luma ? lane : (lane - 16) & 3;
+          const int by = luma ? bi >> 2 : bi >> 1, bx = luma ? bi & 3 : bi & 1;
+          int x[16];
+#pragma unroll
+          for (int i = 0; i < 16; ++i) {
+            const int r = 4 * by + (i >> 2), c = 4 * bx + (i & 3);
+            if (luma) x[i] = (int)S.y[16 * r + c] - (inter ? S.ref(-1, 16 * r + c) : (use_h ? S.ly[r] : dc));
+            else x[i] = (int)(k ? S.cr : S.cb)[8 * r + c] - (inter ? S.ref(k, 8 * r + c) : cpred(k, by));
+          }
+          fdct(x);
+          const int unit = luma ? 2 + ((by >> 1) << 3) + ((bx >> 1) << 2) + ((by & 1) << 1) + (bx & 1)
+                                : 20 + 4 * k + bi;
+          const int q = luma ? qp : qpc;
+          const int qb = 15 + q / 6, fr3 = (1 << qb) / (inter ? 6 : 3);
+          const bool all16 = inter && luma;
+          int total = 0;
+#pragma unroll
+          for (int s = 0; s < 16; ++s) {
+            if (s == 0 && !all16) continue;
+            const int rz = ZZ[s];
+            const int l = quant(x[rz], MF[q % 6][pos_class(rz)], fr3, qb);
+            S.lev[unit - 1][all16 ? s : s - 1] = l;
+            total += l != 0;
+          }
+          S.tc[lane] = total;
+          if (luma) S.dcw[bi] = x[0];
+          else S.cdcw[k][bi] = x[0];
+        }
+        __syncwarp();
+        bool cdc_nz = false;
+        if (lane == 0 && !inter) {
+          int d[16];
+#pragma unroll
+          for (int i = 0; i < 16; ++i) d[i] = S.dcw[i];
+          // H d H with H = [[1,1,1,1],[1,1,-1,-1],[1,-1,-1,1],[1,-1,1,-1]]: columns, then rows (exact, so any order)
+#pragma unroll
+          for (int pass = 0; pass < 2; ++pass)
+#pragma unroll
+            for (int a = 0; a < 4; ++a) {
+              const int st = pass ? 1 : 4, o = pass ? 4 * a : a;
+              const int v0 = d[o], v1 = d[o + st], v2 = d[o + 2 * st], v3 = d[o + 3 * st];
+              d[o] = v0 + v1 + v2 + v3; d[o + st] = v0 + v1 - v2 - v3;
+              d[o + 2 * st] = v0 - v1 - v2 + v3; d[o + 3 * st] = v0 - v1 + v2 - v3;
+            }
+          int z[16];
+#pragma unroll
+          for (int i = 0; i < 16; ++i) {
+            const int q = ((abs(d[i]) >> 1) * mf0 + 2 * fq) >> (qbits + 1);
+            z[i] = d[i] < 0 ? -q : q;
+          }
+#pragma unroll
+          for (int s = 0; s < 16; ++s) S.lev[0][s] = z[ZZ[s]];
+          // 8.5.10: f = H z H, then scaled with LevelScale(qp % 6, 0, 0) = 16 v0
+#pragma unroll
+          for (int pass = 0; pass < 2; ++pass)
+#pragma unroll
+            for (int a = 0; a < 4; ++a) {
+              const int st = pass ? 1 : 4, o = pass ? 4 * a : a;
+              const int v0 = z[o], v1 = z[o + st], v2 = z[o + 2 * st], v3 = z[o + 3 * st];
+              z[o] = v0 + v1 + v2 + v3; z[o + st] = v0 + v1 - v2 - v3;
+              z[o + 2 * st] = v0 - v1 - v2 + v3; z[o + 3 * st] = v0 - v1 + v2 - v3;
+            }
+          const int ls = 16 * VS[qp % 6][0];
+#pragma unroll
+          for (int i = 0; i < 16; ++i)
+            S.dcy[i] = qp >= 36 ? (z[i] * ls) << (qp / 6 - 6) : (z[i] * ls + (1 << (5 - qp / 6))) >> (6 - qp / 6);
+        } else if (lane >= 1 && lane <= 2) {
+          const int k = lane - 1;
+          const int a = S.cdcw[k][0], b = S.cdcw[k][1], c = S.cdcw[k][2], e = S.cdcw[k][3];
+          const int d[4] = {a + b + c + e, a - b + c - e, a + b - c - e, a - b - c + e};
+          const int cf = inter ? (1 << cqbits) / 6 : cfq;
+          int z[4];
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            z[i] = quant(d[i], cmf0, 2 * cf, cqbits + 1);
+            S.lev[17 + k][i] = z[i];
+            cdc_nz |= z[i] != 0;
+          }
+          const int g[4] = {z[0] + z[1] + z[2] + z[3], z[0] - z[1] + z[2] - z[3], z[0] + z[1] - z[2] - z[3],
+                            z[0] - z[1] - z[2] + z[3]};
+          const int ls = 16 * VS[qpc % 6][0];
+#pragma unroll
+          for (int i = 0; i < 4; ++i) S.dcc[k][i] = ((g[i] * ls) << (qpc / 6)) >> 5;
+        }
+        return cdc_nz;
+      };
+      // ---- P frames: the zero-motion inter candidate; P_Skip when all its levels are zero ----
+      bool cdc_nz = false;
+      if (pf) {
+        cdc_nz = transform(true);
+        if (!__ballot_sync(0xffffffffu, (lane < 24 && S.tc[lane] > 0) || cdc_nz)) {
+          ++run;
+          // the reconstruction is the reference, already in J.recon; the next macroblock's left neighbour
+          if (lane < 16) {
+            const int k = lane >> 3, r = lane & 7;
+            S.ly[lane] = S.ref(-1, 16 * lane + 15);
+            S.lc[k][r] = S.ref(k, 8 * r + 7);
+          }
+          if (lane < 8) S.lnz[lane] = 0;
+          __syncwarp();
+          continue;
+        }
       }
-      end = 8 * (at8 + 384);
-    }
-    __syncwarp();
-    // ---- whole bytes out, the partial byte stays ----
-    at = flush_bytes(S.stg, end >> 3, out, at, zrun, lane);
-    const unsigned keep = (end & 7) ? stg_byte(S.stg, end >> 3) : 0u;
-    __syncwarp();
-    for (int i = lane; i <= (end >> 5) && i < STG_WORDS; i += 32) S.stg[i] = 0;
-    __syncwarp();
-    if (lane == 0) S.stg[0] = keep;
-    pend = end & 7;
-    // ---- the left neighbour of the next macroblock ----
-    if (lane < 16) {
-      const int k = lane >> 3, r = lane & 7;
-      S.ly[lane] = pcm ? S.y[16 * lane + 15] : S.ny[lane];
-      S.lc[k][r] = pcm ? (k ? S.cr : S.cb)[8 * r + 7] : S.nc[k][r];
-    }
-    if (lane < 8) {
-      int v;
-      if (pcm) v = 16;
-      else if (lane < 4) v = S.tc[4 * lane + 3];
-      else {
-        const int k = (lane - 4) >> 1, by = (lane - 4) & 1;
-        v = S.tc[16 + 4 * k + 2 * by + 1];
+      // ---- Intra16x16 prediction: DC, or Horizontal when its SAD is strictly lower ----
+      if (have_left) {
+        int s = 0;
+#pragma unroll
+        for (int r = 0; r < 16; ++r) s += S.ly[r];
+        dc = (s + 8) >> 4;
       }
-      S.lnz[lane] = v;
+      int sad_dc = 0, sad_h = 0, sad_p = 0;
+      for (int p = lane; p < 256; p += 32) {
+        sad_dc += abs((int)S.y[p] - dc);
+        if (have_left) sad_h += abs((int)S.y[p] - S.ly[p >> 4]);
+        if (pf) sad_p += abs((int)S.y[p] - S.ref(-1, p));
+      }
+      sad_dc = warp_sum(sad_dc);
+      sad_h = warp_sum(sad_h);
+      use_h = have_left && sad_h < sad_dc;
+      // inter when the zero-motion residual's luma SAD is at most the Intra16x16 candidate's
+      const bool inter = pf && warp_sum(sad_p) <= (use_h ? sad_h : sad_dc);
+      if (!inter) cdc_nz = transform(false);
+      const bool cbp_l = __ballot_sync(0xffffffffu, lane < 16 && S.tc[lane] > 0) != 0;
+      const bool ac_c = __ballot_sync(0xffffffffu, lane >= 16 && lane < 24 && S.tc[lane] > 0) != 0;
+      const bool dc_c = __ballot_sync(0xffffffffu, cdc_nz) != 0;
+      const int cbp_c = ac_c ? 2 : (dc_c ? 1 : 0);
+      // an inter macroblock's CodedBlockPatternLuma: bit b8 when a 4x4 block of 8x8 block b8 has a level
+      int cbp8 = 0;
+      if (inter)
+        cbp8 = (int)__reduce_or_sync(0xffffffffu, lane < 16 && S.tc[lane] > 0
+                                                      ? 1u << (((lane >> 3) << 1) | ((lane & 3) >> 1)) : 0u);
+      __syncwarp();
+      // ---- reconstruction: GOP every block into J.recon, else the right column (luma bx = 3, chroma bx = 1) ----
+      if (GOP ? lane < 24 : ((lane < 16 && (lane & 3) == 3) || (lane >= 16 && lane < 24 && (lane & 1) == 1))) {
+        const bool luma = lane < 16;
+        const int k = luma ? 0 : (lane - 16) >> 2, bi = luma ? lane : (lane - 16) & 3;
+        const int by = luma ? bi >> 2 : bi >> 1, bx = GOP ? (luma ? bi & 3 : bi & 1) : (luma ? 3 : 1);
+        const int unit = luma ? 2 + ((by >> 1) << 3) + ((bx >> 1) << 2) + ((by & 1) << 1) + (bx & 1)
+                              : 20 + 4 * k + bi;
+        const int q = luma ? qp : qpc;
+        const bool all16 = inter && luma;
+        int d[16];
+        d[0] = luma ? S.dcy[bi] : S.dcc[k][bi];
+#pragma unroll
+        for (int s = 0; s < 16; ++s) {
+          if (s == 0 && !all16) continue;
+          const int rz = ZZ[s];
+          const int c = S.lev[unit - 1][all16 ? s : s - 1], ls = 16 * VS[q % 6][pos_class(rz)];
+          d[rz] = q >= 24 ? (c * ls) << (q / 6 - 4) : (c * ls + (1 << (3 - q / 6))) >> (4 - q / 6);
+        }
+        idct(d);
+        const bool right = bx == (luma ? 3 : 1);
+        if constexpr (GOP) {
+#pragma unroll
+          for (int r = 0; r < 4; ++r)
+#pragma unroll
+            for (int c = 0; c < 4; ++c) {
+              const int row = 4 * by + r, col = 4 * bx + c;
+              const int pred = inter ? (luma ? S.ref(-1, 16 * row + col) : S.ref(k, 8 * row + col))
+                                     : (luma ? (use_h ? S.ly[row] : dc) : cpred(k, by));
+              const int v = min(255, max(0, pred + d[4 * r + c]));
+              if (luma) rrow[row * J.w + 16 * mx + col] = (unsigned char)v;
+              else rrow[16 * J.w + k * 4 * J.w + row * (J.w >> 1) + 8 * mx + col] = (unsigned char)v;
+              if (right && c == 3) {
+                if (luma) S.ny[row] = v;
+                else S.nc[k][row] = v;
+              }
+            }
+        } else {
+#pragma unroll
+          for (int r = 0; r < 4; ++r) {
+            const int row = 4 * by + r;
+            const int pred = luma ? (use_h ? S.ly[row] : dc) : cpred(k, by);
+            const int v = min(255, max(0, pred + d[4 * r + 3]));
+            if (luma) S.ny[row] = v;
+            else S.nc[k][row] = v;
+          }
+        }
+      }
+      // ---- macroblock_layer() bits per unit, then the I_PCM decision ----
+      auto unit_bits = [&](auto& b) -> bool {
+        const int u = lane;
+        if (u == 0) {
+          if (inter) {
+            b.ue(0);                                       // mb_type P_L0_16x16
+            b.se(0);                                       // mvd_l0 (0, 0): the predictor is (0, 0)
+            b.se(0);
+            b.ue(INTER_CODE[cbp8 | cbp_c << 4]);           // coded_block_pattern
+            if (cbp8 | cbp_c) b.se(0);                     // mb_qp_delta
+          } else {
+            b.ue((unsigned)((pf ? 5 : 0) + 1 + (use_h ? 1 : 2) + 4 * cbp_c + (cbp_l ? 12 : 0)));
+            b.ue(0);                                       // intra_chroma_pred_mode: DC
+            b.se(0);                                       // mb_qp_delta
+          }
+          return true;
+        }
+        if (u == 1) return inter || residual_block(b, S.lev[0], 16, have_left ? S.lnz[0] : 0);
+        if (u < 18) {
+          const int blk = u - 2;
+          if (inter ? !((cbp8 >> (blk >> 2)) & 1) : !cbp_l) return true;
+          const int by = ((blk >> 3) << 1) | ((blk >> 1) & 1), bx = (((blk >> 2) & 1) << 1) | (blk & 1);
+          const bool ha = bx > 0 || have_left, hb = by > 0;
+          const int na = bx > 0 ? S.tc[4 * by + bx - 1] : (have_left ? S.lnz[by] : 0);
+          const int nb = hb ? S.tc[4 * (by - 1) + bx] : 0;
+          const int nc = ha && hb ? (na + nb + 1) >> 1 : (ha ? na : nb);
+          return residual_block(b, S.lev[u - 1], inter ? 16 : 15, nc);
+        }
+        if (u < 20) return cbp_c ? residual_block(b, S.lev[u - 1], 4, -1) : true;
+        if (u < 28) {
+          if (cbp_c != 2) return true;
+          const int k = (u - 20) >> 2, bi = (u - 20) & 3, by = bi >> 1, bx = bi & 1;
+          const bool ha = bx > 0 || have_left, hb = by > 0;
+          const int na = bx > 0 ? S.tc[16 + 4 * k + 2 * by] : (have_left ? S.lnz[4 + 2 * k + by] : 0);
+          const int nb = hb ? S.tc[16 + 4 * k + bx] : 0;
+          const int nc = ha && hb ? (na + nb + 1) >> 1 : (ha ? na : nb);
+          return residual_block(b, S.lev[u - 1], 15, nc);
+        }
+        return true;
+      };
+      if (pf) {                                            // mb_skip_run before every coded macroblock
+        if (lane == 0) {
+          Bits<true> b{S.stg, pend};
+          b.ue((unsigned)run);
+        }
+        pend += ue_bits((unsigned)run);
+        run = 0;
+      }
+      Bits<false> cnt{nullptr, 0};
+      const bool ok = unit_bits(cnt);
+      int excl = cnt.pos;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const int v = __shfl_up_sync(0xffffffffu, excl, o);
+        if (lane >= o) excl += v;
+      }
+      const int mb_bits = __shfl_sync(0xffffffffu, excl, 31);
+      excl -= cnt.pos;
+      const bool pcm = __ballot_sync(0xffffffffu, !ok) != 0 || mb_bits > MB_BITS_LIMIT;
+      int end;
+      if (!pcm) {
+        Bits<true> b{S.stg, pend + excl};
+        unit_bits(b);
+        end = pend + mb_bits;
+      } else {
+        if (lane == 0) {
+          Bits<true> b{S.stg, pend};
+          b.ue(pf ? 30 : 25);                              // I_PCM, then pcm_alignment_zero_bits
+        }
+        const int at8 = (pend + 9 + 7) >> 3;
+        __syncwarp();
+        for (int i = lane; i < 384; i += 32) {
+          const int j = at8 + i;
+          const unsigned v = i < 256 ? S.y[i] : (i < 320 ? S.cb[i - 256] : S.cr[i - 320]);
+          atomicOr(S.stg + (j >> 2), v << (8 * (j & 3)));
+        }
+        end = 8 * (at8 + 384);
+      }
+      __syncwarp();
+      if constexpr (GOP) {
+        if (pcm) {                                         // the reconstruction is the source
+          for (int i = lane; i < 384; i += 32) {
+            if (i < 256) rrow[(i >> 4) * J.w + 16 * mx + (i & 15)] = S.y[i];
+            else {
+              const int k = (i - 256) >> 6, q = (i - 256) & 63;
+              rrow[16 * J.w + k * 4 * J.w + (q >> 3) * (J.w >> 1) + 8 * mx + (q & 7)] = (k ? S.cr : S.cb)[q];
+            }
+          }
+        }
+      }
+      // ---- whole bytes out, the partial byte stays ----
+      at = flush_bytes(S.stg, end >> 3, out, at, zrun, lane);
+      const unsigned keep = (end & 7) ? stg_byte(S.stg, end >> 3) : 0u;
+      __syncwarp();
+      for (int i = lane; i <= (end >> 5) && i < STG_WORDS; i += 32) S.stg[i] = 0;
+      __syncwarp();
+      if (lane == 0) S.stg[0] = keep;
+      pend = end & 7;
+      // ---- the left neighbour of the next macroblock ----
+      if (lane < 16) {
+        const int k = lane >> 3, r = lane & 7;
+        S.ly[lane] = pcm ? S.y[16 * lane + 15] : S.ny[lane];
+        S.lc[k][r] = pcm ? (k ? S.cr : S.cb)[8 * r + 7] : S.nc[k][r];
+      }
+      if (lane < 8) {
+        int v;
+        if (pcm) v = 16;
+        else if (lane < 4) v = S.tc[4 * lane + 3];
+        else {
+          const int k = (lane - 4) >> 1, by = (lane - 4) & 1;
+          v = S.tc[16 + 4 * k + 2 * by + 1];
+        }
+        S.lnz[lane] = v;
+      }
+      __syncwarp();
     }
+    // ---- a trailing mb_skip_run, rbsp_slice_trailing_bits, the last bytes, the length prefix ----
+    if (lane == 0) {
+      Bits<true> b{S.stg, pend};
+      if (run) b.ue((unsigned)run);
+      b.put(1, 1);
+    }
+    if (run) pend += ue_bits((unsigned)run);
     __syncwarp();
-  }
-  // ---- rbsp_slice_trailing_bits, the last bytes, the length prefix ----
-  if (lane == 0) {
-    Bits<true> b{S.stg, pend};
-    b.put(1, 1);
-  }
-  __syncwarp();
-  at = flush_bytes(S.stg, (pend + 1 + 7) >> 3, out, at, zrun, lane);
-  if (lane == 0) {
-    const long long len = at - 4;
-    out[0] = (unsigned char)(len >> 24); out[1] = (unsigned char)(len >> 16);
-    out[2] = (unsigned char)(len >> 8); out[3] = (unsigned char)len;
-    J.slice_bytes[slice] = (int)at;
+    at = flush_bytes(S.stg, (pend + 1 + 7) >> 3, out, at, zrun, lane);
+    if (lane == 0) {
+      const long long len = at - 4;
+      out[0] = (unsigned char)(len >> 24); out[1] = (unsigned char)(len >> 16);
+      out[2] = (unsigned char)(len >> 8); out[3] = (unsigned char)len;
+      J.slice_bytes[row] = (int)at;
+    }
+    if (!GOP) break;                                     // one frame per warp
+    __syncwarp();
   }
 }
 
@@ -612,6 +765,13 @@ long long slice_bound(int w) {
   return 4 + p + p / 2;
 }
 
+// gop > 1: the longest slice header of either kind, and at most 3201 bits per macroblock with its share of the
+// mb_skip_run codes (include/pm_emage.h).
+long long slice_bound_gop(int w) {
+  const long long p = (SLICE_HEADER_BITS_GOP + (long long)(MB_BITS_LIMIT + 1) * (w / 16) + 8 + 7) / 8;
+  return 4 + p + p / 2;
+}
+
 bool shape_ok(int frames, int h, int w) {
   if (frames < 0 || h < 16 || w < 16 || h % 16 || w % 16) return false;
   const long long mbh = h / 16, mbw = w / 16;
@@ -627,8 +787,27 @@ extern "C" int pm_h264_encode(const unsigned char* frames, long long f_fs, int n
   const long long slices = (long long)n_frames * (h / 16);
   if (slices == 0) return PM_OK;
   PM_REQUIRE(slices / WARPS < 0x7fffffffLL);
-  h264_encode_kernel<<<(unsigned)((slices + WARPS - 1) / WARPS), 32 * WARPS, 0, (cudaStream_t)stream>>>(
-      Job{frames, f_fs, n_frames, clip_len, h, w, qp, scratch, slice_cap, slice_bytes});
+  h264_encode_kernel<false><<<(unsigned)((slices + WARPS - 1) / WARPS), 32 * WARPS, 0, (cudaStream_t)stream>>>(
+      Job{frames, f_fs, n_frames, clip_len, h, w, qp, scratch, slice_cap, slice_bytes, 1, 1, nullptr, 0});
+  PM_LAUNCH_CHECK();
+}
+
+extern "C" int pm_h264_encode_gop(const unsigned char* frames, long long f_fs, int n_frames, int clip_len, int h,
+                                  int w, int qp, unsigned char* scratch, long long slice_cap, int* slice_bytes,
+                                  int gop, unsigned char* recon, long long recon_stride, void* stream) {
+  PM_REQUIRE(gop >= 1);
+  if (gop == 1) return pm_h264_encode(frames, f_fs, n_frames, clip_len, h, w, qp, scratch, slice_cap, slice_bytes,
+                                      stream);
+  PM_REQUIRE(shape_ok(n_frames, h, w) && frames && scratch && slice_bytes && recon && f_fs >= 3LL * w * h
+             && clip_len >= 1 && n_frames % clip_len == 0 && gop <= clip_len && qp >= 0 && qp <= 51
+             && slice_cap >= slice_bound_gop(w) && recon_stride >= 24LL * w);
+  const int chains_per_clip = (int)(((long long)clip_len + gop - 1) / gop);
+  const long long slices = (long long)(n_frames / clip_len) * chains_per_clip * (h / 16);
+  if (slices == 0) return PM_OK;
+  PM_REQUIRE(slices / WARPS < 0x7fffffffLL);
+  h264_encode_kernel<true><<<(unsigned)((slices + WARPS - 1) / WARPS), 32 * WARPS, 0, (cudaStream_t)stream>>>(
+      Job{frames, f_fs, n_frames, clip_len, h, w, qp, scratch, slice_cap, slice_bytes, gop, chains_per_clip, recon,
+          recon_stride});
   PM_LAUNCH_CHECK();
 }
 

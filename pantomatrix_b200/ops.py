@@ -712,19 +712,29 @@ def png_encode(frames, data, nbytes, row_bits, row_adler):
 # ------------------------------------------------------------------------------------------------------
 
 
-def h264_encode(frames, clip_len, qp, data, nbytes, scratch, sizes):
+def h264_encode(frames, clip_len, qp, data, nbytes, scratch, sizes, gop=1, recon=None):
     """The H.264 samples of frames (N, H, W, 3) uint8, each frame dense, any stride apart, frame i at index i % clip_len
     of its clip, into the slots of data (N, cap) uint8 with their sizes in nbytes (N,) int64 (include/pm_emage.h
-    pm_h264_*).  scratch (N, H / 16, slice_cap) uint8 and sizes (N, H / 16) int32: workspace, one slice per row.  The
-    slots are cleared first by a memset (a memset node under graph capture), then two launches."""
+    pm_h264_*).  scratch (N, H / 16, slice_cap) uint8 and sizes (N, H / 16) int32: workspace, one slice per row.
+    gop: frames per group of pictures, 1 <= gop <= clip_len; gop > 1 needs recon (GOPs, H / 16, >= 24 W) uint8, one macroblock row's
+    reconstruction per (GOP, row), written by each GOP's IDR frame before its P frames read it.  The slots are cleared
+    first by a memset (a memset node under graph capture), then two launches."""
     _chk(frames, torch.uint8), _chk(data, torch.uint8), _chk(nbytes, torch.int64)
     _chk(scratch, torch.uint8), _chk(sizes, torch.int32)
     n, h, w, _ = frames.shape
     assert data.is_contiguous() and nbytes.is_contiguous() and scratch.is_contiguous() and sizes.is_contiguous()
     cap, fs, slice_cap = data.shape[1], frames.stride(0) if n > 1 else 3 * h * w, scratch.shape[2]
     _lib.call("pm_memset_async", data.data_ptr(), 0, data.numel(), _stream())
-    _call("pm_h264_encode", frames.data_ptr(), fs, n, clip_len, h, w, qp, scratch.data_ptr(), slice_cap,
-          sizes.data_ptr(), _stream())
+    if gop == 1:
+        _call("pm_h264_encode", frames.data_ptr(), fs, n, clip_len, h, w, qp, scratch.data_ptr(), slice_cap,
+              sizes.data_ptr(), _stream())
+    else:
+        _chk(recon, torch.uint8)
+        chains = n // clip_len * -(-clip_len // gop)
+        assert 1 < gop <= clip_len and n % clip_len == 0 and recon.is_contiguous()
+        assert recon.shape[0] >= chains and recon.shape[1] == h // 16 and recon.shape[2] >= 24 * w
+        _call("pm_h264_encode_gop", frames.data_ptr(), fs, n, clip_len, h, w, qp, scratch.data_ptr(), slice_cap,
+              sizes.data_ptr(), gop, recon.data_ptr(), recon.stride(1), _stream())
     _call("pm_h264_gather", n, h, w, scratch.data_ptr(), slice_cap, sizes.data_ptr(), data.data_ptr(), cap,
           nbytes.data_ptr(), _stream())
 

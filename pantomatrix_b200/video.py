@@ -5,7 +5,10 @@ one fixed rule (DESIGN.md section 12, include/pm_emage.h pm_h264_*): BT.601 limi
 slice per macroblock row with deblocking off, every macroblock Intra16x16 (DC or Horizontal luma, DC chroma) or I_PCM
 when it would pass 3200 bits or need a level escape Baseline lacks, CAVLC, and each slice as one length-prefixed NAL
 unit.  A frame's bytes depend only on the frame, qp and the parity of its index in its clip: the same frame gives the
-same sample alone or in any batch at the same index parity.
+same sample alone or in any batch at the same index parity.  With a keyframe interval gop > 1 (encode(..., gop=30)),
+every gop-th frame is an IDR frame and the frames between are P frames of P_Skip, zero-motion inter, Intra16x16 or
+I_PCM macroblocks, each coded against the frame before it; a GOP's bytes depend only on its frames, qp, gop and the
+parity of its index in the clip.
 
     data, nbytes = video.encode(renderer.render_sequence(poses, expression, trans))   # (B*T, cap) uint8, (B*T,) int64
     video.write_mp4(frames[0], "out/clip.mp4", fps=30)                                 # one silent clip
@@ -24,29 +27,36 @@ from . import flac, ops, slots
 
 MB_BITS_LIMIT = 3200                      # 128 + RawMbBits: the most bits one macroblock_layer() may take (A.3.1)
 MAX_FS, MAX_DIM_MBS = 36864, 543          # level 5.1: MaxFS, and the most macroblocks in a row or column
-SLICE_HEADER_BITS = 62                    # NAL header byte and the longest slice header this encoder writes
+SLICE_HEADER_BITS = 62                    # NAL header byte and the slice header, as the gop = 1 bound counts it
+SLICE_HEADER_BITS_GOP = 70                # the longest slice header of either kind: IDR, last row, qp 0
+RECON_ROW_BYTES = 24                      # reconstruction bytes per pixel column of a row: 16 Y + 4 Cb + 4 Cr
 
 
-def _rbsp_bytes(w: int) -> int:
-    """The most RBSP bytes of one slice: header, w / 16 macroblocks of at most 3200 bits, stop bit and alignment."""
-    return (SLICE_HEADER_BITS + MB_BITS_LIMIT * (w // 16) + 8 + 7) // 8
+def _rbsp_bytes(w: int, gop: int = 1) -> int:
+    """The most RBSP bytes of one slice: header, w / 16 macroblocks, stop bit and alignment.  gop 1: at most 3200
+    bits per macroblock.  gop > 1: at most 3201, a macroblock_layer() of at most 3200 bits after its 1-bit ue(0)
+    mb_skip_run; a run of r >= 1 skipped macroblocks takes at most 2 log2(r + 1) + 1 <= 3 r bits, and I_PCM 9 + 7 +
+    3072."""
+    if gop == 1:
+        return (SLICE_HEADER_BITS + MB_BITS_LIMIT * (w // 16) + 8 + 7) // 8
+    return (SLICE_HEADER_BITS_GOP + (MB_BITS_LIMIT + 1) * (w // 16) + 8 + 7) // 8
 
 
-def slice_bytes(w: int) -> int:
+def slice_bytes(w: int, gop: int = 1) -> int:
     """The most bytes of one length-prefixed slice: 4-byte length, the RBSP, at most one emulation prevention byte per
     two RBSP bytes (each needs two zero bytes before it)."""
-    p = _rbsp_bytes(w)
+    p = _rbsp_bytes(w, _gop(gop))
     return 4 + p + p // 2
 
 
-def max_bytes(h: int, w: int) -> int:
-    """The size bound of one (h, w) frame's sample: h / 16 slices of at most slice_bytes(w)."""
-    return (h // 16) * slice_bytes(w)
+def max_bytes(h: int, w: int, gop=1) -> int:
+    """The size bound of one (h, w) frame's sample: h / 16 slices of at most slice_bytes(w, gop)."""
+    return (h // 16) * slice_bytes(w, gop)
 
 
-def slot_bytes(h: int, w: int) -> int:
+def slot_bytes(h: int, w: int, gop=1) -> int:
     """Bytes of one output slot: max_bytes rounded up to a multiple of 4."""
-    return (max_bytes(h, w) + 3) & ~3
+    return (max_bytes(h, w, gop) + 3) & ~3
 
 
 def check_size(h: int, w: int) -> None:
@@ -60,6 +70,12 @@ def _qp(qp) -> int:
     if isinstance(qp, bool) or not isinstance(qp, int) or not 0 <= qp <= 51:
         raise ValueError(f"qp must be an int in 0..51, got {qp!r}")
     return qp
+
+
+def _gop(gop) -> int:
+    if isinstance(gop, bool) or not isinstance(gop, int) or gop < 1:
+        raise ValueError(f"gop must be an int >= 1, got {gop!r}")
+    return gop
 
 
 def _fps(fps) -> Fraction:
@@ -98,14 +114,16 @@ class _Bits:
         return bytes(out)
 
 
-def sps(h: int, w: int) -> bytes:
-    """Sequence parameter set NAL unit: Constrained Baseline, level 5.1, pic_order_cnt_type 2, no reference frames,
-    and a VUI holding only the video signal type (limited range, SMPTE 170M primaries, transfer and matrix)."""
+def sps(h: int, w: int, gop=1) -> bytes:
+    """Sequence parameter set NAL unit: Constrained Baseline, level 5.1, pic_order_cnt_type 2, no reference frames
+    (one when gop > 1: each P frame references the frame before it), and a VUI holding only the video signal type
+    (limited range, SMPTE 170M primaries, transfer and matrix)."""
     check_size(h, w)
+    gop = _gop(gop)
     b = _Bits()
     b.u(0x67, 8)                          # nal_ref_idc 3, nal_unit_type 7
     b.u(66, 8), b.u(0b11000000, 8), b.u(51, 8)   # profile_idc, constraint_set0/1, level_idc
-    b.ue(0), b.ue(0), b.ue(2), b.ue(0)    # sps id, log2_max_frame_num_minus4, poc type, max_num_ref_frames
+    b.ue(0), b.ue(0), b.ue(2), b.ue(int(gop > 1))   # sps id, log2_max_frame_num_minus4, poc type, max_num_ref_frames
     b.u(0, 1)                             # gaps_in_frame_num_value_allowed_flag
     b.ue(w // 16 - 1), b.ue(h // 16 - 1)
     b.u(1, 1), b.u(1, 1), b.u(0, 1)       # frame_mbs_only, direct_8x8_inference, frame_cropping
@@ -130,26 +148,36 @@ def pps() -> bytes:
 # ---- encoding on the GPU ----
 
 @torch.no_grad()
-def encode(frames, qp=20, out=None):
+def encode(frames, qp=20, out=None, gop=1):
     """H.264 samples of frames (N, H, W, 3) or (B, T, H, W, 3) uint8 CUDA, each frame dense (a MeshRenderer result is
-    read in place), H and W multiples of 16.  A frame's index in its clip (t, or n for (N, ...) input) sets its
-    idr_pic_id (index mod 2).  Returns (data, nbytes): data (N, cap) uint8 holds sample i (its slices, each prefixed
-    by its 4-byte big-endian length) in data[i, :nbytes[i]] (zeros after it), nbytes (N,) int64, both on the frames'
-    device.  out: an optional (data, nbytes) pair to fill, data (N, cap) uint8 contiguous with cap >= slot_bytes(H, W)
-    and a multiple of 4, nbytes (N,) int64 contiguous.  No host synchronisation; with out given the call can be
-    captured in a CUDA graph.  Raises ValueError on a CPU tensor, a wrong dtype or shape, H or W not a multiple of 16,
-    a frame past level 5.1, frames that are not dense, qp outside 0..51 or an out too small."""
-    qp = _qp(qp)
+    read in place), H and W multiples of 16.  gop: frames per group of pictures.  Frame t of a clip (t, or n for
+    (N, ...) input) is an IDR frame with idr_pic_id (t div gop) mod 2 when t mod gop == 0, else a P frame coded
+    against frame t - 1 (P_Skip, zero-motion inter, Intra16x16 or I_PCM macroblocks); gop 1 makes every frame IDR,
+    and any gop >= T codes each clip as one GOP (the bytes of gop = T).  A GOP's bytes depend only on its frames, qp,
+    gop and the parity of t div gop.  Returns (data, nbytes): data (N, cap) uint8 holds sample i (its slices, each
+    prefixed by its 4-byte big-endian length) in data[i, :nbytes[i]] (zeros after it), nbytes (N,) int64, both on the
+    frames' device.  out: an optional (data, nbytes) pair to fill, data (N, cap) uint8 contiguous with
+    cap >= slot_bytes(H, W, gop) and a multiple of 4, nbytes (N,) int64 contiguous.  No host synchronisation; with
+    out given the call can be captured in a CUDA graph.  Raises ValueError on a CPU tensor, a wrong dtype or shape,
+    H or W not a multiple of 16, a frame past level 5.1, frames that are not dense, qp outside 0..51, gop not an int
+    >= 1 or an out too small (cap >= slot_bytes(H, W, gop))."""
+    qp, gop = _qp(qp), _gop(gop)
     frames, clip_len = slots.frames(frames)
     n, h, w, _ = frames.shape
     check_size(h, w)
     dev = frames.device
-    data, nbytes = slots.output(n, max_bytes(h, w), slot_bytes(h, w), dev, out)
+    data, nbytes = slots.output(n, max_bytes(h, w, gop), slot_bytes(h, w, gop), dev, out)
     if n == 0:
         return data, nbytes
-    scratch = torch.empty(n, h // 16, slice_bytes(w), dtype=torch.uint8, device=dev)
+    scratch = torch.empty(n, h // 16, slice_bytes(w, gop), dtype=torch.uint8, device=dev)
     sizes = torch.empty(n, h // 16, dtype=torch.int32, device=dev)
-    ops.h264_encode(frames, clip_len, qp, data, nbytes, scratch, sizes)
+    # a gop past the clip length gives the gop = T bytes (the same idr_pic_id and frame_num); the kernel takes at most T
+    kgop = min(gop, clip_len)
+    recon = None
+    if kgop > 1:                          # one macroblock row's reconstruction per (GOP, row), updated frame by frame
+        chains = n // clip_len * -(-clip_len // kgop)
+        recon = torch.empty(chains, h // 16, RECON_ROW_BYTES * w, dtype=torch.uint8, device=dev)
+    ops.h264_encode(frames, clip_len, qp, data, nbytes, scratch, sizes, gop=kgop, recon=recon)
     return data, nbytes
 
 
@@ -178,15 +206,17 @@ def _chunks(sizes, starts):
 
 
 def _trak(track_id, duration, volume, size, timescale, media_dur, handler, media_header, entry, stts, sample_sizes,
-          chunks):
+          chunks, sync=None):
     """One track: tkhd (its duration in movie ticks, volume, size (w, h)), then mdia: mdhd (timescale and duration),
     hdlr (handler: type and name), and minf holding the media header box, dinf with its dref, and stbl: stsd with the
-    sample entry, the stts payload, the stsc and stco payloads of _chunks (chunks), stsz of the samples' sizes."""
+    sample entry, the stts payload, stss of the sync sample numbers (sync; none when sync is None), the stsc and stco
+    payloads of _chunks (chunks), stsz of the samples' sizes."""
     n = len(sample_sizes)
     stsc, stco = chunks
     stbl = _box(b"stbl",
                 _full(b"stsd", 0, 0, struct.pack(">I", 1), entry),
                 _full(b"stts", 0, 0, stts),
+                *([] if sync is None else [_full(b"stss", 0, 0, struct.pack(f">I{len(sync)}I", len(sync), *sync))]),
                 _full(b"stsc", 0, 0, stsc),
                 _full(b"stsz", 0, 0, struct.pack(">II", 0, n), struct.pack(f">{n}I", *sample_sizes)),
                 _full(b"stco", 0, 0, stco))
@@ -202,16 +232,18 @@ def _trak(track_id, duration, volume, size, timescale, media_dur, handler, media
     return _box(b"trak", tkhd, mdia)
 
 
-def mp4_bytes(samples, h: int, w: int, fps=30, audio=None) -> bytes:
+def mp4_bytes(samples, h: int, w: int, fps=30, audio=None, gop=1) -> bytes:
     """An MP4 file of one H.264 video track: samples (a list of bytes-like, each a sample as encode() writes it), h x w
-    frames at a constant fps.  ftyp, then moov (avc1 with its avcC holding the SPS and PPS, stts, stsc, stsz, stco, no
-    stss: every sample is a sync sample), then mdat, so the file plays while it downloads.
+    frames at a constant fps, encoded with keyframe interval gop.  ftyp, then moov (avc1 with its avcC holding the SPS
+    (sps(h, w, gop)) and PPS, stts, stsc, stsz, stco; with gop 1 no stss, as every sample is a sync sample, else an
+    stss listing the IDR samples 1, 1 + gop, ...), then mdat, so the file plays while it downloads.
     audio: None (a silent file), or (frames, info), a FLAC track: its frames (bytes-like, as flac.encode writes them)
     and their 34-byte STREAMINFO (flac.streaminfo).  The file then has a second track, and mdat holds one-second
     chunks: each second's video samples, then the audio frames that start in that second.
     Raises ValueError on no samples, fps <= 0 or a file that would pass 2^32 bytes."""
     check_size(h, w)
     rate = _fps(fps)
+    gop = _gop(gop)
     samples = [bytes(s) for s in samples]
     if not samples:
         raise ValueError("mp4_bytes needs at least one sample")
@@ -246,12 +278,14 @@ def mp4_bytes(samples, h: int, w: int, fps=30, audio=None) -> bytes:
         plan = [(t, idx) for s in sorted(second) for t, idx in enumerate(second[s]) if idx]
     movie = max(movie_dur, audio_dur)
     data = (samples, sound)
-    s, p = sps(h, w), pps()
+    s, p = sps(h, w, gop), pps()
     avcc = _box(b"avcC", bytes([1, 66, 0xC0, 51, 0xFF, 0xE1]), struct.pack(">H", len(s)), s,
                 bytes([1]), struct.pack(">H", len(p)), p)
     avc1 = _box(b"avc1", bytes(6), struct.pack(">H", 1), bytes(16), struct.pack(">HH", w, h),
                 struct.pack(">II", 0x480000, 0x480000), bytes(4), struct.pack(">H", 1), bytes(32),
                 struct.pack(">Hh", 0x18, -1), avcc)
+
+    sync = None if gop == 1 else list(range(1, n + 1, gop))
 
     def moov(offset):
         starts, at = ([], []), offset
@@ -263,7 +297,7 @@ def mp4_bytes(samples, h: int, w: int, fps=30, audio=None) -> bytes:
                      bytes(10), _MATRIX, bytes(24), struct.pack(">I", 2 if audio is None else 3))
         traks = [_trak(1, movie_dur, 0, (w, h), timescale, media_dur, (b"vide", b"VideoHandler\0"),
                        _full(b"vmhd", 0, 1, bytes(8)), avc1, struct.pack(">III", 1, n, delta),
-                       [len(x) for x in samples], tables[0])]
+                       [len(x) for x in samples], tables[0], sync)]
         if audio is not None:
             traks.append(_trak(2, audio_dur, 0x100, (0, 0), srate, pcm_n, (b"soun", b"SoundHandler\0"),
                                _full(b"smhd", 0, 0, bytes(4)), fla, sound_stts, [len(x) for x in sound], tables[1]))
@@ -278,17 +312,18 @@ def mp4_bytes(samples, h: int, w: int, fps=30, audio=None) -> bytes:
     return ftyp + moov(head) + struct.pack(">I", 8 + total - head) + b"mdat" + body
 
 
-def write_mp4(frames, path, fps=30, qp=20, audio=None):
-    """Encode one clip (T, H, W, 3) uint8 CUDA frames and write it to path as an MP4 file.  audio: None (one silent
-    video track), or (pcm, rate): pcm (n, C) CUDA int16 or int32 (24-bit) samples at rate Hz, coded as a FLAC track
-    (flac.encode) and trimmed to the video's duration: the first min(n, floor(T rate / fps)) samples.  That matches
-    ffmpeg's -shortest when the audio is the longer stream; shorter audio is kept whole, and the video plays on past
-    its end in silence.  Both streams are encoded on the current stream; the sizes are read once (one
-    synchronisation), only the encoded bytes (and the samples, for the MD5) are copied to pinned host memory, and
-    the copies are waited for once.  Returns path."""
+def write_mp4(frames, path, fps=30, qp=20, audio=None, gop=1):
+    """Encode one clip (T, H, W, 3) uint8 CUDA frames with keyframe interval gop (encode) and write it to path as an
+    MP4 file.  audio: None (one silent video track), or (pcm, rate): pcm (n, C) CUDA int16 or int32 (24-bit) samples
+    at rate Hz, coded as a FLAC track (flac.encode) and trimmed to the video's duration: the first
+    min(n, floor(T rate / fps)) samples.  That matches ffmpeg's -shortest when the audio is the longer stream; shorter
+    audio is kept whole, and the video plays on past its end in silence.  Both streams are encoded on the current
+    stream; the sizes are read once (one synchronisation), only the encoded bytes (and the samples, for the MD5) are
+    copied to pinned host memory, and the copies are waited for once.  Returns path."""
     if torch.is_tensor(frames) and frames.dim() != 4:
         raise ValueError(f"write_mp4 takes one clip (T, H, W, 3), got {tuple(frames.shape)}")
     frame_rate = _fps(fps)
+    gop = _gop(gop)
     if audio is not None:
         pcm, rate = audio
         flac._rate(rate)
@@ -298,7 +333,7 @@ def write_mp4(frames, path, fps=30, qp=20, audio=None):
         if keep < 1:
             raise ValueError(f"write_mp4: {frames.shape[0]} frames at {fps} fps hold no sample at {rate} Hz")
         pcm = pcm[:keep]
-    data, nbytes = encode(frames, qp=qp)
+    data, nbytes = encode(frames, qp=qp, gop=gop)
     h, w = frames.shape[1:3]
     if audio is None:
         (pieces,) = slots.to_host((data, nbytes.tolist()))
@@ -313,7 +348,7 @@ def write_mp4(frames, path, fps=30, qp=20, audio=None):
         host_pcm.copy_(pcm, non_blocking=True)          # done by the time to_host's one synchronisation returns
         pieces, sound = slots.to_host((data, sizes), (adata, sound_sizes))
         track = (sound, flac.streaminfo(host_pcm, rate, sound_sizes))
-    blob = mp4_bytes(pieces, h, w, fps, audio=track)
+    blob = mp4_bytes(pieces, h, w, fps, audio=track, gop=gop)
     with open(path, "wb") as f:
         f.write(blob)
     return path

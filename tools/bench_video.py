@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """H.264 encoding of rendered frames on one GPU (pantomatrix_b200/video.py), beside PNG encoding of the same frames.
 
-    python tools/bench_video.py OUT.json [--reps 5] [--stage-reps 3] [--psnr-frames 30]
+    python tools/bench_video.py OUT.json [--reps 5] [--stage-reps 3] [--psnr-frames 30] [--no-mb-types] [--gop-only]
+                                         [--baseline-lib PARENT/pantomatrix_b200/libpm_emage.so]
 
 Inputs: the frames tools/bench_png.py uses: render_sequence of EMAGE generate() output (synthetic weights, full-size
 synthetic surface model), 1 x 300 and 8 x 300 frames of 960 x 720, and render_body(upsample=2) of CaMN forward()
@@ -13,7 +14,17 @@ Reported per input, from CUDA events after a warm-up call (medians over --reps):
   qp 16, 20, 26 and 32, the luma decoded by OpenCV's FFmpeg from a write_mp4 file of the first --psnr-frames frames;
 and, for one 300-frame EMAGE clip, the demos' output stage on the host clock: render + encode + copy + write mp4
 (video.write_mp4) against render + png.write_frames, alternating the two, into a temporary directory removed after.
+GOP arms (keyframe interval gop 1, 30 and T, the clip length), per input: the video.encode call at qp 20 (median ms,
+the three gops alternating), bytes per frame (min, mean, max), and luma PSNR of the first --psnr-frames frames decoded
+by OpenCV's FFmpeg from a write_mp4 file; for the 1 x 300 EMAGE clip also the share of P_Skip / inter / intra / I_PCM
+macroblocks over one whole GOP at gop 30 (frames 0..29: the IDR frame and 29 P frames), counted by the CPU
+restatement (tests/h264_gop_ref.py), whose bytes equal the GPU's; and the output stage (render + write_mp4) at gop 1
+against gop 30, alternating.  --gop-only runs only the GOP arms and that output stage.
+--baseline-lib: the libpm_emage.so of another build (for instance the parent commit's, built from a checkout of it):
+pm_h264_encode of that library, pm_h264_encode of this tree and pm_h264_encode_gop(gop = 1) of this tree on the
+EMAGE 1 x 300 and 8 x 300 frames, alternating, medians over 2 * --reps, and whether all three wrote the same slices.
 The card's name, power limit and max SM clock are read in the same run.  Nothing is written except OUT."""
+import ctypes
 import argparse
 import json
 import os
@@ -36,6 +47,9 @@ from pantomatrix_b200.body_model import SmplxBodyModel  # noqa: E402
 from pantomatrix_b200.pipeline import generate  # noqa: E402
 from pantomatrix_b200.render import MeshRenderer  # noqa: E402
 from synthetic_models import build_lstm_product, build_product, smplx_surface_arrays  # noqa: E402
+
+sys.path.insert(0, os.path.join(ROOT, "tests"))
+import h264_gop_ref  # noqa: E402
 
 QP = 20
 
@@ -116,6 +130,107 @@ def quality(frames, count, tmp):
     return out
 
 
+def luma_psnr(frames, path, count):
+    """Mean and min luma PSNR (dB) of the first count frames of an MP4 file against the colour rule's Y."""
+    import cv2
+    ys = source_y(frames[:count]).cpu().numpy().astype(np.float64)
+    h, w = frames.shape[1:3]
+    cap = cv2.VideoCapture(path, cv2.CAP_FFMPEG)
+    cap.set(cv2.CAP_PROP_CONVERT_RGB, 0)
+    psnr = []
+    for i in range(count):
+        ok, fr = cap.read()
+        assert ok, i
+        y = np.asarray(fr).reshape(-1)[:h * w].reshape(h, w).astype(np.float64)
+        mse = ((y - ys[i]) ** 2).mean()
+        psnr.append(99.0 if mse == 0 else 10 * np.log10(255.0 ** 2 / mse))
+    cap.release()
+    return float(np.mean(psnr)), float(np.min(psnr))
+
+
+def baseline(frames, lib_path, reps):
+    """pm_h264_encode of the library at lib_path against this tree's pm_h264_encode and pm_h264_encode_gop(gop = 1),
+    alternating: median ms of each, and whether the three wrote the same slices and sizes."""
+    clip_len = frames.shape[1]
+    frames = frames.reshape(-1, *frames.shape[-3:])
+    n, h, w, _ = frames.shape
+    sc = video.slice_bytes(w)
+    base = ctypes.CDLL(lib_path)
+    base.pm_h264_encode.argtypes, base.pm_h264_encode.restype = _lib.SIGNATURES["pm_h264_encode"], ctypes.c_int
+    bufs = {k: (torch.zeros(n, h // 16, sc, dtype=torch.uint8, device="cuda"),
+                torch.zeros(n, h // 16, dtype=torch.int32, device="cuda"))
+            for k in ("baseline", "encode", "encode_gop1")}
+    args = lambda k: (frames.data_ptr(), 3 * h * w, n, clip_len, h, w, QP, bufs[k][0].data_ptr(), sc,
+                      bufs[k][1].data_ptr())
+    st = ops._stream()
+
+    def run_base():
+        assert base.pm_h264_encode(*args("baseline"), st) == 0
+
+    calls = {"baseline": run_base,
+             "encode": lambda: _lib.call("pm_h264_encode", *args("encode"), st),
+             "encode_gop1": lambda: _lib.call("pm_h264_encode_gop", *args("encode_gop1"), 1, None, 0, st)}
+    for fn in calls.values():
+        fn()
+    torch.cuda.synchronize()
+    ms = {k: [] for k in calls}
+    for _ in range(2 * reps):
+        for k, fn in calls.items():
+            ms[k].append(event_ms(fn))
+    same = all(torch.equal(bufs[k][i], bufs["baseline"][i]) for k in calls for i in (0, 1))
+    return {"lib": lib_path, "identical": same,
+            **{k: {"ms_median": statistics.median(v), "ms_all": v} for k, v in ms.items()}}
+
+
+def gop_arms(frames, reps, psnr_frames, mb_types, tmp):
+    """encode time, bytes per frame and luma PSNR at gop 1, 30 and T, the gops alternating in the timed loop; with
+    mb_types, the macroblock shares over the first whole GOP at gop 30."""
+    t = frames.shape[1] if frames.dim() == 5 else frames.shape[0]
+    gops = (1, 30, t)
+    ms = {g: [] for g in gops}
+    for g in gops:
+        video.encode(frames, qp=QP, gop=g)                    # warm-up
+    torch.cuda.synchronize()
+    for _ in range(reps):
+        for g in gops:
+            ms[g].append(event_ms(lambda: video.encode(frames, qp=QP, gop=g)))
+    out = {}
+    clip = frames[0] if frames.dim() == 5 else frames
+    for g in gops:
+        sizes = video.encode(frames, qp=QP, gop=g)[1].cpu().numpy()
+        path = video.write_mp4(clip, os.path.join(tmp, f"g{g}.mp4"), fps=30, qp=QP, gop=g)
+        psnr_mean, psnr_min = luma_psnr(clip, path, psnr_frames)
+        out[f"gop{g}"] = {"encode_ms_median": statistics.median(ms[g]), "encode_ms_all": ms[g],
+                          "bytes_per_frame_mean": float(sizes.mean()), "bytes_per_frame_min": int(sizes.min()),
+                          "bytes_per_frame_max": int(sizes.max()), "file_bytes_clip0": os.path.getsize(path),
+                          "luma_psnr_db_mean": psnr_mean, "luma_psnr_db_min": psnr_min}
+        if mb_types and g == 30 < t:
+            enc = h264_gop_ref.encode_clip(list(clip[:g].cpu().numpy()), QP, g)
+            types = np.concatenate([e[2].reshape(-1) for e in enc])
+            out[f"gop{g}"]["mb_share_first_gop"] = {k: float((types == k).mean())
+                                                    for k in ("SKIP", "P", "DC", "H", "PCM")}
+    return out
+
+
+def output_stage_gop(r, pred, reps):
+    """Render + video.write_mp4 of one 300-frame EMAGE clip at gop 1 against gop 30, alternating, host clock."""
+    poses, expr, trans = (pred[k][:1] for k in ("motion_axis_angle", "expression", "trans"))
+    res, size = {1: [], 30: []}, {}
+    for _ in range(reps):
+        for g in res:
+            d = tempfile.mkdtemp()
+            try:
+                torch.cuda.synchronize()
+                t0 = time.perf_counter()
+                frames = r.render_sequence(poses, expr, trans)[0]
+                video.write_mp4(frames, os.path.join(d, "clip.mp4"), fps=30, qp=QP, gop=g)
+                res[g].append(time.perf_counter() - t0)
+                size[g] = os.path.getsize(os.path.join(d, "clip.mp4"))
+            finally:
+                shutil.rmtree(d)
+    return {f"gop{g}": {"s_median": statistics.median(v), "s_all": v, "file_bytes": size[g]} for g, v in res.items()}
+
+
 def output_stage(r, pred, reps):
     """One 300-frame EMAGE clip from poses to files, alternating the two arms, host clock around work that ends in
     files: render + video.write_mp4 against render + png.write_frames."""
@@ -148,29 +263,25 @@ def output_stage(r, pred, reps):
     return out
 
 
-def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("out")
-    ap.add_argument("--reps", type=int, default=5)
-    ap.add_argument("--stage-reps", type=int, default=3)
-    ap.add_argument("--psnr-frames", type=int, default=30)
-    args = ap.parse_args()
-    assert torch.cuda.is_available(), "the video benchmark measures the GPU: no CUDA device found"
-    torch.cuda.set_device(0)
-    model, vqm = build_product(seed=0, device="cuda")
-    _, pred = generate(model, vqm, torch.from_numpy(synth_audio(8, 160000, 5)).cuda())
-    r = MeshRenderer(SmplxBodyModel(smplx_surface_arrays(), "cuda"))
-    res = {"card": card()}
+def run(args, r, pred, res, tmp):
+    """Every arm main() asks for, into res; tmp: a scratch directory for the MP4 files, removed by main()."""
     for clips in (1, 8):
         frames = r.render_sequence(*(pred[k][:clips] for k in ("motion_axis_angle", "expression", "trans")))
+        res[f"gop_emage_sequence_{clips}x300"] = gop_arms(frames, args.reps, args.psnr_frames,
+                                                          clips == 1 and not args.no_mb_types, tmp)
+        print("gop emage", clips, json.dumps(res[f"gop_emage_sequence_{clips}x300"]), flush=True)
+        if args.baseline_lib:
+            res[f"baseline_emage_sequence_{clips}x300"] = baseline(frames, args.baseline_lib, args.reps)
+            print("baseline", clips, json.dumps(res[f"baseline_emage_sequence_{clips}x300"])[:700], flush=True)
+        if args.gop_only:
+            del frames
+            continue
         res[f"emage_sequence_{clips}x300"] = arm(frames, args.reps)
         print("emage", clips, json.dumps(res[f"emage_sequence_{clips}x300"])[:700], flush=True)
         if clips == 1:
-            tmp = tempfile.mkdtemp()
-            try:
-                res["emage_quality"] = quality(frames[0], args.psnr_frames, tmp)
-            finally:
-                shutil.rmtree(tmp)
+            qtmp = os.path.join(tmp, "quality")
+            os.makedirs(qtmp)
+            res["emage_quality"] = quality(frames[0], args.psnr_frames, qtmp)
             print("quality", json.dumps(res["emage_quality"]), flush=True)
         del frames
     camn = build_lstm_product("camn", device="cuda")
@@ -178,11 +289,41 @@ def main():
                  torch.zeros(1, 1, dtype=torch.long, device="cuda"))["motion_axis_angle"]
     poses = poses.reshape(1, poses.shape[1], 165)
     frames = r.render_body(poses, torch.zeros(1, poses.shape[1], 3, device="cuda"), upsample=2)
-    res["camn_body_1x10s"] = arm(frames, args.reps)
-    print("camn", json.dumps(res["camn_body_1x10s"])[:700], flush=True)
+    res["gop_camn_body_1x10s"] = gop_arms(frames, args.reps, args.psnr_frames, False, tmp)
+    print("gop camn", json.dumps(res["gop_camn_body_1x10s"]), flush=True)
+    if not args.gop_only:
+        res["camn_body_1x10s"] = arm(frames, args.reps)
+        print("camn", json.dumps(res["camn_body_1x10s"])[:700], flush=True)
     del frames
-    res["output_stage_1x300"] = output_stage(r, pred, args.stage_reps)
-    print("output stage", json.dumps(res["output_stage_1x300"]), flush=True)
+    res["output_stage_gop_1x300"] = output_stage_gop(r, pred, args.stage_reps)
+    print("output stage gop", json.dumps(res["output_stage_gop_1x300"]), flush=True)
+    if not args.gop_only:
+        res["output_stage_1x300"] = output_stage(r, pred, args.stage_reps)
+        print("output stage", json.dumps(res["output_stage_1x300"]), flush=True)
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("out")
+    ap.add_argument("--reps", type=int, default=5)
+    ap.add_argument("--stage-reps", type=int, default=3)
+    ap.add_argument("--psnr-frames", type=int, default=30)
+    ap.add_argument("--no-mb-types", action="store_true", help="skip the macroblock shares (CPU restatement)")
+    ap.add_argument("--baseline-lib", default=None,
+                    help="libpm_emage.so of another build to time pm_h264_encode against")
+    ap.add_argument("--gop-only", action="store_true", help="only the GOP arms and the gop output stage")
+    args = ap.parse_args()
+    assert torch.cuda.is_available(), "the video benchmark measures the GPU: no CUDA device found"
+    torch.cuda.set_device(0)
+    model, vqm = build_product(seed=0, device="cuda")
+    _, pred = generate(model, vqm, torch.from_numpy(synth_audio(8, 160000, 5)).cuda())
+    r = MeshRenderer(SmplxBodyModel(smplx_surface_arrays(), "cuda"))
+    res = {"card": card()}
+    tmp = tempfile.mkdtemp()
+    try:
+        run(args, r, pred, res, tmp)
+    finally:
+        shutil.rmtree(tmp, ignore_errors=True)
     res["card_after"] = card()
     with open(args.out, "w") as f:
         json.dump(res, f, indent=1)
