@@ -58,6 +58,8 @@ def main():
     ap.add_argument("--with-audio", action="store_true", help="put the WAV's sound in the --video file")
     ap.add_argument("--gop", type=int, default=1,
                     help="--video keyframe interval: an IDR frame every GOP frames, P frames between (1: all IDR)")
+    ap.add_argument("--search", type=int, default=0,
+                    help="--video motion search range in pixels, 0..32, for the P frames (0: zero motion)")
     args = ap.parse_args()
     if not args.synthetic and not args.checkpoint:
         ap.error("give --checkpoint DIR or --synthetic")
@@ -69,6 +71,8 @@ def main():
         ap.error("--with-audio needs --video")
     if args.gop < 1:
         ap.error("--gop must be at least 1")
+    if not 0 <= args.search <= 32:
+        ap.error("--search must be in 0..32")
     os.makedirs(args.save_folder, exist_ok=True)
     device = torch.device("cuda")                      # no CPU fallback by design
     model, motion_vq = load_models(args, device)
@@ -97,7 +101,8 @@ def main():
                 from pantomatrix_b200 import video
                 video.write_mp4(drawn, os.path.splitext(npz)[0] + ".mp4", fps=30,
                                 audio=read_track(os.path.join(args.audio_folder, name), device)
-                                if args.with_audio else None, gop=args.gop)
+                                if args.with_audio else None, gop=args.gop,
+                                search=args.search)
         frames += t
     print(f"generate total {frames / fps:.2f} seconds motion in {time.time() - t0:.2f} seconds")
 

@@ -411,6 +411,38 @@ int pm_h264_encode(const unsigned char* frames, long long f_fs, int n_frames, in
 int pm_h264_encode_gop(const unsigned char* frames, long long f_fs, int n_frames, int clip_len, int h, int w, int qp,
                        unsigned char* scratch, long long slice_cap, int* slice_bytes, int gop, unsigned char* recon,
                        long long recon_stride, void* stream);
+/* pm_h264_encode_me: pm_h264_encode_gop (gop 2 .. clip_len) with motion search range 1 <= search <= 32 whole pixels.
+ * Everything but the inter macroblocks' vectors is the rule above (GOP structure, headers, SPS, PPS, intra, I_PCM,
+ * nC, skip runs, cbp mapping):
+ *   reference: the whole reconstruction of frame t - 1 (luma h x w, chroma h / 2 x w / 2), read at clipped
+ *     coordinates outside it (8.4.2.2);
+ *   integer search: every (dx, dy), |dx|, |dy| <= search, whose 16x16 luma block lies inside the frame; vectors in
+ *     quarter-pel units; J(mv) = SAD_Y(mv) + LAMBDA[qp] (b(mvx) + b(mvy)), b(v) the bits of se(v), SAD_Y against the
+ *     motion-compensated luma, measured against a zero predictor (every macroblock's search is independent); lowest
+ *     J, ties to the smaller |mvx| + |mvy|, then smaller mvy, then smaller mvx;
+ *   sub-pel: the 8 neighbours at +-2 of the integer winner, then the 8 at +-1 of the half-pel winner, in raster order,
+ *     each replacing the centre only when its J is strictly lower.  Luma by 8.4.2.2.1 (6-tap, j from unrounded
+ *     intermediates, quarter positions rounded averages), chroma by 8.4.2.2.2 (the luma vector in eighth chroma
+ *     samples, bilinear);
+ *   LAMBDA[qp] = floor(sqrt(0.85 2^((qp - 12) / 3)) + 0.5) in float64: 0 0 0 0 0 0 0 1 1 1 1 1 1 1 1 1 1 2 2 2 2 3 3 3
+ *     4 4 5 5 6 7 7 8 9 10 12 13 15 17 19 21 23 26 30 33 37 42 47 53 59 66 74 83;
+ *   macroblock: P_Skip when every level of the zero-motion inter candidate is 0 (vector (0, 0), 8.4.1.1), else the
+ *     inter candidate at the searched vector (source - MC prediction, transform and quantisation as above) is
+ *     P_L0_16x16 when its luma SAD <= the Intra16x16 candidate's, else Intra16x16; a non-zero vector with no level is
+ *     P_L0_16x16 with cbp 0; I_PCM as above;
+ *   mvd = mv - mvp, se(v) x then y; mvp (8.4.1.3, B and C never available) is the left macroblock's vector when it is
+ *     P_L0_16x16, else (0, 0);
+ *   bound: as gop > 1 above (the mvd counts toward the 3200 bits).
+ * Workspaces: recon, two whole-frame reconstructions (Y, Cb, Cr planes, 3 h w / 2 bytes each) per chain,
+ * recon_stride >= 3 h w apart; mv, mv_len >= chains (h / 16) (w / 16) int16 (x, y) pairs, 4-byte aligned; chains =
+ * (n_frames / clip_len) ceil(clip_len / gop).  Neither needs clearing.  Launches, on one stream with no host
+ * synchronisation: the code kernel for frame 0 of every chain (IDR, into buffer 0), then for k = 1 .. gop - 1 the
+ * search kernel (one CTA per macroblock of every chain's frame k, the vectors into mv) and the code kernel (one warp
+ * per (chain, row), frame k against buffer (k - 1) mod 2, into buffer k mod 2).  Launch order around it and slot
+ * sizes: as pm_h264_encode_gop. */
+int pm_h264_encode_me(const unsigned char* frames, long long f_fs, int n_frames, int clip_len, int h, int w, int qp,
+                      unsigned char* scratch, long long slice_cap, int* slice_bytes, int gop, unsigned char* recon,
+                      long long recon_stride, int search, short* mv, long long mv_len, void* stream);
 int pm_h264_gather(int n_frames, int h, int w, const unsigned char* scratch, long long slice_cap,
                    const int* slice_bytes, unsigned char* data, long long cap, long long* nbytes, void* stream);
 

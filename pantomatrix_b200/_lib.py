@@ -60,6 +60,7 @@ SIGNATURES = {
     "pm_png_crc": [_i, _i, _i, _p, _ll, _p, _p],
     "pm_h264_encode": [_p, _ll, _i, _i, _i, _i, _i, _p, _ll, _p, _p],
     "pm_h264_encode_gop": [_p, _ll, _i, _i, _i, _i, _i, _p, _ll, _p, _i, _p, _ll, _p],
+    "pm_h264_encode_me": [_p, _ll, _i, _i, _i, _i, _i, _p, _ll, _p, _i, _p, _ll, _i, _p, _ll, _p],
     "pm_h264_gather": [_i, _i, _i, _p, _ll, _p, _p, _ll, _p, _p],
     "pm_flac_analyse": [_p, _ll, _i, _i, _i, _i, _p, _p],
     "pm_flac_emit": [_p, _ll, _i, _i, _i, _i, _i, _p, _p, _ll, _p, _p],

@@ -1,15 +1,17 @@
 // H.264 encoding of RGB8 frames (pantomatrix_b200/video.py): one access unit per frame by the rule of
 // include/pm_emage.h and DESIGN.md section 12 (one slice per macroblock row, Intra16x16 DC / Horizontal or I_PCM,
 // CAVLC, deblocking off; with a keyframe interval gop > 1, P frames of P_Skip and zero-motion inter macroblocks
-// between the IDR frames).  Two launches per call after the caller's memset of the output slots:
+// between the IDR frames, or with a motion search range, quarter-pel vectors against the whole previous frame).  Two
+// launches per call after the caller's memset of the output slots (pm_h264_encode_me: 2 gop - 1 encode launches,
+// h264_search_kernel before each P frame's):
 //   pm_h264_encode  one warp per (frame, macroblock row): the row's slice, emulation prevention applied, into its
 //                   scratch slot, and the slice's size; pm_h264_encode_gop: one warp per (GOP, row), walking the
 //                   GOP's frames in order;
 //   pm_h264_gather  one CTA per (frame, row): the slice's offset in the frame's sample, the copy, the frame's size.
 // A warp stages its bits in shared memory in stream byte order (pm_put_bits, as FLAC writes its slots), so whole
 // bytes leave the staging buffer as byte loads.
-// CPU restatement: oracle/h264_oracle.py, and tests/h264_gop_ref.py for P frames.  Every byte depends only on the
-// frame (its GOP's frames), qp, gop and the parity of its index (t div gop).
+// CPU restatement: oracle/h264_oracle.py, tests/h264_gop_ref.py for P frames, tests/h264_me_ref.py for motion.  Every
+// byte depends only on the frame (its GOP's frames), qp, gop, search and the parity of its index (t div gop).
 #include <cub/block/block_reduce.cuh>
 
 #include <type_traits>
@@ -301,17 +303,69 @@ struct Job {
   long long slice_cap;
   int* slice_bytes;
   int gop, chains_per_clip;  // GOP: frames per GOP, GOPs per clip
-  unsigned char* recon;      // GOP: one macroblock row's reconstruction per (chain, row), recon_stride apart
-  long long recon_stride;
+  unsigned char* recon;      // GOP: one macroblock row's reconstruction per (chain, row), recon_stride apart; ME: two
+  long long recon_stride;    // whole-frame reconstructions per chain (frame k in buffer k & 1), recon_stride apart
+  int k, search;             // ME: the frame of each chain this launch codes (or searches), the search range
+  short2* mv;                // ME: frame k's vector per (chain, macroblock), quarter-pel
 };
+
+// The kernel's three instances: every frame IDR; GOPs with zero motion, a warp walking its GOP's frames; GOPs with
+// motion search, one launch per frame of the GOPs (h264_search_kernel before each P frame's).
+enum Mode { INTRA, GOP_ZERO, GOP_ME };
+
+__constant__ unsigned char LAMBDA[52] = {0,  0,  0,  0,  0,  0,  0,  1,  1,  1,  1,  1,  1,  1,  1,  1,  1,  2,
+                                         2,  2,  2,  3,  3,  3,  4,  4,  5,  5,  6,  7,  7,  8,  9,  10, 12, 13,
+                                         15, 17, 19, 21, 23, 26, 30, 33, 37, 42, 47, 53, 59, 66, 74, 83};
+
+__device__ __forceinline__ int se_bits(int v) { return ue_bits(v > 0 ? 2 * v - 1 : -2 * v); }
+
+__device__ __forceinline__ int clip255(int v) { return min(255, max(0, v)); }
+
+// 8.4.2.2.1: the luma prediction sample at quarter-pel phase (fx, fy) of the integer sample G = at(0, 0); at(dx, dy)
+// reads the reference at an offset from G (clipped to the frame by the caller).  b, h, m, s: the half-pel samples
+// right of G, below G, below G's right neighbour and right of G's lower neighbour; j from unrounded intermediates;
+// the quarter-pel samples are rounded averages of the two nearest.
+template <class At>
+__device__ __forceinline__ int luma_pred(const At& at, int fx, int fy) {
+  auto tap = [](int a, int b, int c, int d, int e, int f) { return a - 5 * b + 20 * c + 20 * d - 5 * e + f; };
+  auto row1 = [&](int r) { return tap(at(-2, r), at(-1, r), at(0, r), at(1, r), at(2, r), at(3, r)); };
+  auto col1 = [&](int c) { return tap(at(c, -2), at(c, -1), at(c, 0), at(c, 1), at(c, 2), at(c, 3)); };
+  auto half = [](int v) { return clip255((v + 16) >> 5); };
+  if (fy == 0) {
+    if (fx == 0) return at(0, 0);
+    const int b = half(row1(0));
+    return fx == 2 ? b : (b + at(fx >> 1, 0) + 1) >> 1;                      // a, b, c
+  }
+  if (fx == 0) {
+    const int h = half(col1(0));
+    return fy == 2 ? h : (h + at(0, fy >> 1) + 1) >> 1;                      // d, h, n
+  }
+  if (fx == 2 || fy == 2) {
+    const int j = clip255((tap(row1(-2), row1(-1), row1(0), row1(1), row1(2), row1(3)) + 512) >> 10);
+    if (fx == 2 && fy == 2) return j;
+    const int o = fx == 2 ? half(row1(fy >> 1)) : half(col1(fx >> 1));      // f / q: b / s; i / k: h / m
+    return (j + o + 1) >> 1;
+  }
+  return (half(row1(fy >> 1)) + half(col1(fx >> 1)) + 1) >> 1;              // e, g, p, r
+}
+
+// 8.4.2.2.2: the chroma prediction sample at eighth-pel phase (fx, fy) between A = at(0, 0), B, C, D.
+template <class At>
+__device__ __forceinline__ int chroma_pred(const At& at, int fx, int fy) {
+  return ((8 - fx) * (8 - fy) * at(0, 0) + fx * (8 - fy) * at(1, 0) + (8 - fx) * fy * at(0, 1) + fx * fy * at(1, 1)
+          + 32) >> 6;
+}
 
 __device__ __forceinline__ void rgb(const unsigned char* p, int& r, int& g, int& b) { r = p[0]; g = p[1]; b = p[2]; }
 
-// One warp per (chain, macroblock row).  A chain is one frame (GOP false: every frame IDR) or one GOP of one clip
-// (GOP true): the warp codes the row of each of the chain's frames in turn, the IDR frame first, and keeps the row's
-// reconstruction in J.recon for the next frame's P slice.
-template <bool GOP>
+// One warp per (chain, macroblock row).  A chain is one frame (INTRA: every frame IDR) or one GOP of one clip.
+// GOP_ZERO: the warp codes the row of each of the chain's frames in turn, the IDR frame first, and keeps the row's
+// reconstruction in J.recon for the next frame's P slice.  GOP_ME: the warp codes the row of the chain's frame J.k
+// only, against the whole reconstruction of frame k - 1, with the vectors h264_search_kernel chose, and writes frame
+// k's reconstruction to the other buffer; kernel boundaries order the frames.
+template <Mode MODE>
 __global__ void __launch_bounds__(32 * WARPS) h264_encode_kernel(Job J) {
+  constexpr bool GOP = MODE != INTRA, ME = MODE == GOP_ME;
   __shared__ Warp<GOP> WS[WARPS];
   const int lane = threadIdx.x & 31;
   Warp<GOP>& S = WS[threadIdx.x >> 5];
@@ -332,12 +386,29 @@ __global__ void __launch_bounds__(32 * WARPS) h264_encode_kernel(Job J) {
     t0 = (int)(chain % J.clip_len);
     t1 = t0 + 1;
   }
-  unsigned char* const rrow = GOP ? J.recon + slice * J.recon_stride : nullptr;   // Y 16 x w, Cb, Cr 8 x w / 2
+  if (ME && t0 + J.k >= t1) return;                     // a last GOP shorter than gop
+  // GOP_ZERO: the row's reconstruction (Y 16 x w, Cb, Cr 8 x w / 2), read and updated in place.  GOP_ME: frame k's
+  // reconstruction (Y h x w, Cb, Cr h / 2 x w / 2) is written to rrow, frame k - 1's read from rref.
+  const long long fsz = 3LL * J.h * J.w / 2;
+  unsigned char* const rrow = ME ? J.recon + chain * J.recon_stride + (J.k & 1) * fsz
+                                 : (GOP ? J.recon + slice * J.recon_stride : nullptr);
+  const unsigned char* const rref = ME ? J.recon + chain * J.recon_stride + ((J.k + 1) & 1) * fsz : rrow;
+  // offsets in rrow / rref of luma (row, col) and chroma k (row, col) of macroblock mx of the row
+  auto yo = [&](int row, int mx, int col) -> long long {
+    if constexpr (ME) return (long long)(16 * my + row) * J.w + 16 * mx + col;
+    else return row * J.w + 16 * mx + col;
+  };
+  auto co = [&](int k, int row, int mx, int col) -> long long {
+    if constexpr (ME)
+      return (long long)J.h * J.w + k * ((long long)J.h * J.w >> 2) + (long long)(8 * my + row) * (J.w >> 1) + 8 * mx
+             + col;
+    else return 16 * J.w + k * 4 * J.w + row * (J.w >> 1) + 8 * mx + col;
+  };
   const int qp = J.qp, qpc = QPC[qp];
   const int mf0 = MF[qp % 6][0], qbits = 15 + qp / 6, fq = (1 << qbits) / 3;
   const int cmf0 = MF[qpc % 6][0], cqbits = 15 + qpc / 6, cfq = (1 << cqbits) / 3;
 
-  for (int t = t0; t < t1; ++t) {
+  for (int t = ME ? t0 + J.k : t0; t < t1; ++t) {
     const long long f = f0 + (t - t0);
     const bool pf = GOP && t > t0;                       // a P frame: every frame of a GOP after its IDR frame
     const unsigned char* fr = J.px + f * J.fs;
@@ -376,6 +447,7 @@ __global__ void __launch_bounds__(32 * WARPS) h264_encode_kernel(Job J) {
       pend = __shfl_sync(0xffffffffu, b.pos, 0);
     }
     int run = 0;                                           // P_Skip macroblocks since the last coded one
+    short2 lmv = make_short2(0, 0);                        // ME: the vector predictor, the left P_L0_16x16's vector
 
     for (int mx = 0; mx < mbw; ++mx) {
       const bool have_left = mx > 0;
@@ -399,10 +471,13 @@ __global__ void __launch_bounds__(32 * WARPS) h264_encode_kernel(Job J) {
       }
       if constexpr (GOP) {
         if (pf) {
-          for (int p = lane; p < 256; p += 32) S.ry[p] = rrow[(p >> 4) * J.w + 16 * mx + (p & 15)];
+          // (the GOP_ZERO instance keeps its own address arithmetic: sharing yo / co costs it spills)
+          for (int p = lane; p < 256; p += 32)
+            S.ry[p] = ME ? rref[yo(p >> 4, mx, p & 15)] : rrow[(p >> 4) * J.w + 16 * mx + (p & 15)];
           for (int p = lane; p < 128; p += 32) {
             const int k = p >> 6, q = p & 63;
-            S.rc[k][q] = rrow[16 * J.w + k * 4 * J.w + (q >> 3) * (J.w >> 1) + 8 * mx + (q & 7)];
+            S.rc[k][q] = ME ? rref[co(k, q >> 3, mx, q & 7)]
+                            : rrow[16 * J.w + k * 4 * J.w + (q >> 3) * (J.w >> 1) + 8 * mx + (q & 7)];
           }
         }
       }
@@ -508,11 +583,20 @@ __global__ void __launch_bounds__(32 * WARPS) h264_encode_kernel(Job J) {
       };
       // ---- P frames: the zero-motion inter candidate; P_Skip when all its levels are zero ----
       bool cdc_nz = false;
+      short2 mv = make_short2(0, 0);
       if (pf) {
         cdc_nz = transform(true);
         if (!__ballot_sync(0xffffffffu, (lane < 24 && S.tc[lane] > 0) || cdc_nz)) {
           ++run;
-          // the reconstruction is the reference, already in J.recon; the next macroblock's left neighbour
+          if constexpr (ME) {                              // the reconstruction is the reference
+            for (int p = lane; p < 256; p += 32) rrow[yo(p >> 4, mx, p & 15)] = S.ry[p];
+            for (int p = lane; p < 128; p += 32) {
+              const int k = p >> 6, q = p & 63;
+              rrow[co(k, q >> 3, mx, q & 7)] = S.rc[k][q];
+            }
+            lmv = make_short2(0, 0);
+          }
+          // GOP_ZERO: the reconstruction is the reference, already in J.recon; the next macroblock's left neighbour
           if (lane < 16) {
             const int k = lane >> 3, r = lane & 7;
             S.ly[lane] = S.ref(-1, 16 * lane + 15);
@@ -521,6 +605,30 @@ __global__ void __launch_bounds__(32 * WARPS) h264_encode_kernel(Job J) {
           if (lane < 8) S.lnz[lane] = 0;
           __syncwarp();
           continue;
+        }
+        if constexpr (ME) {                                // the inter candidate at the searched vector
+          mv = J.mv[(chain * mbh + my) * mbw + mx];
+          if (mv.x | mv.y) {
+            __syncwarp();
+            const int w = J.w, h = J.h;
+            for (int p = lane; p < 256; p += 32) {
+              const int xi = 16 * mx + (p & 15) + (mv.x >> 2), yi = 16 * my + (p >> 4) + (mv.y >> 2);
+              S.ry[p] = (unsigned char)luma_pred([&](int dx, int dy) {
+                return (int)rref[(long long)min(h - 1, max(0, yi + dy)) * w + min(w - 1, max(0, xi + dx))];
+              }, mv.x & 3, mv.y & 3);
+            }
+            for (int p = lane; p < 128; p += 32) {
+              const int k = p >> 6, q = p & 63;
+              const int xi = 8 * mx + (q & 7) + (mv.x >> 3), yi = 8 * my + (q >> 3) + (mv.y >> 3);
+              const unsigned char* pl = rref + (long long)h * w + k * ((long long)h * w >> 2);
+              S.rc[k][q] = (unsigned char)chroma_pred([&](int dx, int dy) {
+                return (int)pl[(long long)min((h >> 1) - 1, max(0, yi + dy)) * (w >> 1)
+                               + min((w >> 1) - 1, max(0, xi + dx))];
+              }, mv.x & 7, mv.y & 7);
+            }
+            __syncwarp();
+            cdc_nz = transform(true);
+          }
         }
       }
       // ---- Intra16x16 prediction: DC, or Horizontal when its SAD is strictly lower ----
@@ -581,8 +689,13 @@ __global__ void __launch_bounds__(32 * WARPS) h264_encode_kernel(Job J) {
               const int pred = inter ? (luma ? S.ref(-1, 16 * row + col) : S.ref(k, 8 * row + col))
                                      : (luma ? (use_h ? S.ly[row] : dc) : cpred(k, by));
               const int v = min(255, max(0, pred + d[4 * r + c]));
-              if (luma) rrow[row * J.w + 16 * mx + col] = (unsigned char)v;
-              else rrow[16 * J.w + k * 4 * J.w + row * (J.w >> 1) + 8 * mx + col] = (unsigned char)v;
+              if constexpr (ME) {
+                if (luma) rrow[yo(row, mx, col)] = (unsigned char)v;
+                else rrow[co(k, row, mx, col)] = (unsigned char)v;
+              } else {
+                if (luma) rrow[row * J.w + 16 * mx + col] = (unsigned char)v;
+                else rrow[16 * J.w + k * 4 * J.w + row * (J.w >> 1) + 8 * mx + col] = (unsigned char)v;
+              }
               if (right && c == 3) {
                 if (luma) S.ny[row] = v;
                 else S.nc[k][row] = v;
@@ -605,8 +718,8 @@ __global__ void __launch_bounds__(32 * WARPS) h264_encode_kernel(Job J) {
         if (u == 0) {
           if (inter) {
             b.ue(0);                                       // mb_type P_L0_16x16
-            b.se(0);                                       // mvd_l0 (0, 0): the predictor is (0, 0)
-            b.se(0);
+            b.se(ME ? mv.x - lmv.x : 0);                   // mvd_l0; GOP_ZERO: (0, 0), the predictor is (0, 0)
+            b.se(ME ? mv.y - lmv.y : 0);
             b.ue(INTER_CODE[cbp8 | cbp_c << 4]);           // coded_block_pattern
             if (cbp8 | cbp_c) b.se(0);                     // mb_qp_delta
           } else {
@@ -681,10 +794,13 @@ __global__ void __launch_bounds__(32 * WARPS) h264_encode_kernel(Job J) {
       if constexpr (GOP) {
         if (pcm) {                                         // the reconstruction is the source
           for (int i = lane; i < 384; i += 32) {
-            if (i < 256) rrow[(i >> 4) * J.w + 16 * mx + (i & 15)] = S.y[i];
-            else {
-              const int k = (i - 256) >> 6, q = (i - 256) & 63;
-              rrow[16 * J.w + k * 4 * J.w + (q >> 3) * (J.w >> 1) + 8 * mx + (q & 7)] = (k ? S.cr : S.cb)[q];
+            const int k = (i - 256) >> 6, q = (i - 256) & 63;
+            if constexpr (ME) {
+              if (i < 256) rrow[yo(i >> 4, mx, i & 15)] = S.y[i];
+              else rrow[co(k, q >> 3, mx, q & 7)] = (k ? S.cr : S.cb)[q];
+            } else {
+              if (i < 256) rrow[(i >> 4) * J.w + 16 * mx + (i & 15)] = S.y[i];
+              else rrow[16 * J.w + k * 4 * J.w + (q >> 3) * (J.w >> 1) + 8 * mx + (q & 7)] = (k ? S.cr : S.cb)[q];
             }
           }
         }
@@ -698,6 +814,7 @@ __global__ void __launch_bounds__(32 * WARPS) h264_encode_kernel(Job J) {
       if (lane == 0) S.stg[0] = keep;
       pend = end & 7;
       // ---- the left neighbour of the next macroblock ----
+      if constexpr (ME) lmv = inter && !pcm ? mv : make_short2(0, 0);
       if (lane < 16) {
         const int k = lane >> 3, r = lane & 7;
         S.ly[lane] = pcm ? S.y[16 * lane + 15] : S.ny[lane];
@@ -730,9 +847,107 @@ __global__ void __launch_bounds__(32 * WARPS) h264_encode_kernel(Job J) {
       out[2] = (unsigned char)(len >> 8); out[3] = (unsigned char)len;
       J.slice_bytes[row] = (int)at;
     }
-    if (!GOP) break;                                     // one frame per warp
+    if (!GOP || ME) break;                               // one frame per warp
     __syncwarp();
   }
+}
+
+// One CTA per (chain, macroblock) of frame J.k of every chain (k >= 1): the vector of the P_L0_16x16 candidate by the
+// rule of include/pm_emage.h, into J.mv.  The reference window the search and the 6-tap filter read, clipped to the
+// frame, is staged in shared memory.  Integer search: one thread per candidate, SADs four samples at a time; the
+// argmin under the tie rule is a block-wide minimum of (J, |dx| + |dy|, dy, dx) keys.  Sub-pel refinement: one warp
+// per neighbour, 8 neighbours per step.
+constexpr int SEARCH_THREADS = 256;
+constexpr int MAX_SEARCH = 32;
+constexpr int WIN_PITCH = (16 + 2 * MAX_SEARCH + 6 + 3) & ~3;   // window row bytes (16 + 2 search + 6 used)
+
+__global__ void __launch_bounds__(SEARCH_THREADS) h264_search_kernel(Job J) {
+  __shared__ unsigned win[(16 + 2 * MAX_SEARCH + 6) * WIN_PITCH / 4];
+  __shared__ unsigned src[64];
+  __shared__ unsigned long long red[SEARCH_THREADS / 32];
+  __shared__ int jn[8];
+  const unsigned char* wb = reinterpret_cast<const unsigned char*>(win);
+  const unsigned char* sb = reinterpret_cast<const unsigned char*>(src);
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int mbw = J.w >> 4, mbh = J.h >> 4;
+  const long long chain = blockIdx.x / ((long long)mbw * mbh);
+  const int my = (int)(blockIdx.x / mbw % mbh), mx = (int)(blockIdx.x % mbw);
+  const int t0 = (int)(chain % J.chains_per_clip) * J.gop;
+  if (t0 + J.k >= min(t0 + J.gop, J.clip_len)) return;
+  const unsigned char* fr = J.px + (chain / J.chains_per_clip * J.clip_len + t0 + J.k) * J.fs;
+  const unsigned char* ref = J.recon + chain * J.recon_stride + ((J.k + 1) & 1) * (3LL * J.h * J.w / 2);
+  const int s = J.search, wn = 16 + 2 * s + 6, ox = 16 * mx - s - 3, oy = 16 * my - s - 3;
+  {
+    const unsigned char* p = fr + ((long long)(16 * my + (tid >> 4)) * J.w + 16 * mx + (tid & 15)) * 3;
+    reinterpret_cast<unsigned char*>(src)[tid] =
+        (unsigned char)(((66 * p[0] + 129 * p[1] + 25 * p[2] + 128) >> 8) + 16);
+  }
+  for (int i = tid; i < wn * wn; i += SEARCH_THREADS) {
+    const int r = i / wn, c = i - r * wn;
+    reinterpret_cast<unsigned char*>(win)[r * WIN_PITCH + c] =
+        ref[(long long)min(J.h - 1, max(0, oy + r)) * J.w + min(J.w - 1, max(0, ox + c))];
+  }
+  __syncthreads();
+  const int lam = LAMBDA[J.qp];
+  // ---- integer search: every (dx, dy), |dx|, |dy| <= s, whose block lies inside the frame ----
+  const int dx0 = max(-s, -16 * mx), dx1 = min(s, J.w - 16 - 16 * mx);
+  const int dy0 = max(-s, -16 * my), dy1 = min(s, J.h - 16 - 16 * my);
+  const int nx = dx1 - dx0 + 1, n = nx * (dy1 - dy0 + 1);
+  unsigned long long best = ~0ull;
+  for (int c = tid; c < n; c += SEARCH_THREADS) {
+    const int dx = dx0 + c % nx, dy = dy0 + c / nx;
+    const int x = 3 + s + dx, sh = 8 * (x & 3);
+    const unsigned* row = win + ((3 + s + dy) * WIN_PITCH + (x & ~3)) / 4;
+    unsigned sad = 0;
+#pragma unroll 4
+    for (int r = 0; r < 16; ++r, row += WIN_PITCH / 4) {
+      unsigned a = row[0];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const unsigned b = row[i + 1];
+        sad = __vsadu4(__funnelshift_r(a, b, sh), src[4 * r + i]) + sad;
+        a = b;
+      }
+    }
+    const unsigned cost = sad + lam * (se_bits(4 * dx) + se_bits(4 * dy));
+    const unsigned long long key = (unsigned long long)cost << 24 | (unsigned)(abs(dx) + abs(dy)) << 16
+                                   | (unsigned)(dy + MAX_SEARCH) << 8 | (unsigned)(dx + MAX_SEARCH);
+    best = min(best, key);
+  }
+#pragma unroll
+  for (int o = 16; o; o >>= 1) best = min(best, __shfl_xor_sync(0xffffffffu, best, o));
+  if (lane == 0) red[warp] = best;
+  __syncthreads();
+#pragma unroll
+  for (int i = 0; i < SEARCH_THREADS / 32; ++i) best = min(best, red[i]);
+  int mvx = 4 * ((int)(best & 0xff) - MAX_SEARCH), mvy = 4 * ((int)(best >> 8 & 0xff) - MAX_SEARCH);
+  int cost = (int)(best >> 24);
+  // ---- sub-pel refinement: the 8 neighbours at +-2, then at +-1, in raster order; strictly lower J replaces ----
+  for (int step = 2; step >= 1; step >>= 1) {
+    if (warp < 8) {
+      const int nb = warp < 4 ? warp : warp + 1;                  // raster index around the centre (4)
+      const int cx = mvx + (nb % 3 - 1) * step, cy = mvy + (nb / 3 - 1) * step;
+      int sad = 0;
+      for (int p = lane; p < 256; p += 32) {
+        const unsigned char* g = wb + (3 + s + (p >> 4) + (cy >> 2)) * WIN_PITCH + 3 + s + (p & 15) + (cx >> 2);
+        sad += abs((int)sb[p] - luma_pred([&](int dx, int dy) { return (int)g[dy * WIN_PITCH + dx]; }, cx & 3, cy & 3));
+      }
+      sad = warp_sum(sad);
+      if (lane == 0) jn[warp] = sad + lam * (se_bits(cx) + se_bits(cy));
+    }
+    __syncthreads();
+    int bi = -1;
+#pragma unroll
+    for (int i = 0; i < 8; ++i)
+      if (jn[i] < cost) { cost = jn[i]; bi = i; }
+    if (bi >= 0) {
+      const int nb = bi < 4 ? bi : bi + 1;
+      mvx += (nb % 3 - 1) * step;
+      mvy += (nb / 3 - 1) * step;
+    }
+    __syncthreads();
+  }
+  if (tid == 0) J.mv[blockIdx.x] = make_short2((short)mvx, (short)mvy);
 }
 
 __global__ void __launch_bounds__(GATHER_THREADS) h264_gather_kernel(int mbh, const unsigned char* __restrict__ scratch,
@@ -787,7 +1002,7 @@ extern "C" int pm_h264_encode(const unsigned char* frames, long long f_fs, int n
   const long long slices = (long long)n_frames * (h / 16);
   if (slices == 0) return PM_OK;
   PM_REQUIRE(slices / WARPS < 0x7fffffffLL);
-  h264_encode_kernel<false><<<(unsigned)((slices + WARPS - 1) / WARPS), 32 * WARPS, 0, (cudaStream_t)stream>>>(
+  h264_encode_kernel<INTRA><<<(unsigned)((slices + WARPS - 1) / WARPS), 32 * WARPS, 0, (cudaStream_t)stream>>>(
       Job{frames, f_fs, n_frames, clip_len, h, w, qp, scratch, slice_cap, slice_bytes, 1, 1, nullptr, 0});
   PM_LAUNCH_CHECK();
 }
@@ -805,9 +1020,32 @@ extern "C" int pm_h264_encode_gop(const unsigned char* frames, long long f_fs, i
   const long long slices = (long long)(n_frames / clip_len) * chains_per_clip * (h / 16);
   if (slices == 0) return PM_OK;
   PM_REQUIRE(slices / WARPS < 0x7fffffffLL);
-  h264_encode_kernel<true><<<(unsigned)((slices + WARPS - 1) / WARPS), 32 * WARPS, 0, (cudaStream_t)stream>>>(
+  h264_encode_kernel<GOP_ZERO><<<(unsigned)((slices + WARPS - 1) / WARPS), 32 * WARPS, 0, (cudaStream_t)stream>>>(
       Job{frames, f_fs, n_frames, clip_len, h, w, qp, scratch, slice_cap, slice_bytes, gop, chains_per_clip, recon,
           recon_stride});
+  PM_LAUNCH_CHECK();
+}
+
+extern "C" int pm_h264_encode_me(const unsigned char* frames, long long f_fs, int n_frames, int clip_len, int h,
+                                 int w, int qp, unsigned char* scratch, long long slice_cap, int* slice_bytes, int gop,
+                                 unsigned char* recon, long long recon_stride, int search, short* mv,
+                                 long long mv_len, void* stream) {
+  PM_REQUIRE(shape_ok(n_frames, h, w) && frames && scratch && slice_bytes && recon && mv && f_fs >= 3LL * w * h
+             && clip_len >= 1 && n_frames % clip_len == 0 && gop >= 2 && gop <= clip_len && qp >= 0 && qp <= 51
+             && search >= 1 && search <= MAX_SEARCH && slice_cap >= slice_bound_gop(w) && recon_stride >= 3LL * h * w);
+  const int chains_per_clip = (int)(((long long)clip_len + gop - 1) / gop);
+  const long long chains = (long long)(n_frames / clip_len) * chains_per_clip, slices = chains * (h / 16);
+  if (slices == 0) return PM_OK;
+  const long long mbs = slices * (w / 16);
+  PM_REQUIRE(mv_len >= mbs && reinterpret_cast<unsigned long long>(mv) % 4 == 0 && slices / WARPS < 0x7fffffffLL
+             && mbs < 0x7fffffffLL);
+  Job j{frames, f_fs, n_frames, clip_len, h, w, qp, scratch, slice_cap, slice_bytes, gop, chains_per_clip, recon,
+        recon_stride, 0, search, reinterpret_cast<short2*>(mv)};
+  const cudaStream_t st = (cudaStream_t)stream;
+  for (j.k = 0; j.k < gop; ++j.k) {
+    if (j.k) h264_search_kernel<<<(unsigned)mbs, SEARCH_THREADS, 0, st>>>(j);
+    h264_encode_kernel<GOP_ME><<<(unsigned)((slices + WARPS - 1) / WARPS), 32 * WARPS, 0, st>>>(j);
+  }
   PM_LAUNCH_CHECK();
 }
 

@@ -712,13 +712,15 @@ def png_encode(frames, data, nbytes, row_bits, row_adler):
 # ------------------------------------------------------------------------------------------------------
 
 
-def h264_encode(frames, clip_len, qp, data, nbytes, scratch, sizes, gop=1, recon=None):
+def h264_encode(frames, clip_len, qp, data, nbytes, scratch, sizes, gop=1, recon=None, search=0, mv=None):
     """The H.264 samples of frames (N, H, W, 3) uint8, each frame dense, any stride apart, frame i at index i % clip_len
     of its clip, into the slots of data (N, cap) uint8 with their sizes in nbytes (N,) int64 (include/pm_emage.h
     pm_h264_*).  scratch (N, H / 16, slice_cap) uint8 and sizes (N, H / 16) int32: workspace, one slice per row.
     gop: frames per group of pictures, 1 <= gop <= clip_len; gop > 1 needs recon (GOPs, H / 16, >= 24 W) uint8, one macroblock row's
-    reconstruction per (GOP, row), written by each GOP's IDR frame before its P frames read it.  The slots are cleared
-    first by a memset (a memset node under graph capture), then two launches."""
+    reconstruction per (GOP, row), written by each GOP's IDR frame before its P frames read it.  search: the motion
+    search range in whole pixels, 0..32; search > 0 with gop > 1 runs pm_h264_encode_me and needs recon (GOPs, >= 3 H W)
+    uint8, two whole-frame reconstructions per GOP, and mv (GOPs, H / 16, W / 16, 2) int16, the searched vectors.  The
+    slots are cleared first by a memset (a memset node under graph capture), then the launches."""
     _chk(frames, torch.uint8), _chk(data, torch.uint8), _chk(nbytes, torch.int64)
     _chk(scratch, torch.uint8), _chk(sizes, torch.int32)
     n, h, w, _ = frames.shape
@@ -728,6 +730,15 @@ def h264_encode(frames, clip_len, qp, data, nbytes, scratch, sizes, gop=1, recon
     if gop == 1:
         _call("pm_h264_encode", frames.data_ptr(), fs, n, clip_len, h, w, qp, scratch.data_ptr(), slice_cap,
               sizes.data_ptr(), _stream())
+    elif search > 0:
+        _chk(recon, torch.uint8), _chk(mv, torch.int16)
+        chains = n // clip_len * -(-clip_len // gop)
+        assert 1 < gop <= clip_len and 0 < search <= 32 and n % clip_len == 0
+        assert recon.is_contiguous() and recon.shape[0] >= chains and recon.shape[1] >= 3 * h * w
+        assert mv.is_contiguous() and mv.shape[0] >= chains and mv.shape[1:] == (h // 16, w // 16, 2)
+        _call("pm_h264_encode_me", frames.data_ptr(), fs, n, clip_len, h, w, qp, scratch.data_ptr(), slice_cap,
+              sizes.data_ptr(), gop, recon.data_ptr(), recon.stride(0), search, mv.data_ptr(), mv.numel() // 2,
+              _stream())
     else:
         _chk(recon, torch.uint8)
         chains = n // clip_len * -(-clip_len // gop)

@@ -3,6 +3,7 @@
 
     python tools/bench_video.py OUT.json [--reps 5] [--stage-reps 3] [--psnr-frames 30] [--no-mb-types] [--gop-only]
                                          [--baseline-lib PARENT/pantomatrix_b200/libpm_emage.so]
+                                         [--me-only [--me-mb-frames 4]]
 
 Inputs: the frames tools/bench_png.py uses: render_sequence of EMAGE generate() output (synthetic weights, full-size
 synthetic surface model), 1 x 300 and 8 x 300 frames of 960 x 720, and render_body(upsample=2) of CaMN forward()
@@ -23,6 +24,12 @@ against gop 30, alternating.  --gop-only runs only the GOP arms and that output 
 --baseline-lib: the libpm_emage.so of another build (for instance the parent commit's, built from a checkout of it):
 pm_h264_encode of that library, pm_h264_encode of this tree and pm_h264_encode_gop(gop = 1) of this tree on the
 EMAGE 1 x 300 and 8 x 300 frames, alternating, medians over 2 * --reps, and whether all three wrote the same slices.
+Motion search arms (--me-only runs only these): gop 30 and T with search 0, 16 and 32, per input, the six arms
+alternating in the timed loop: the video.encode call (median ms), bytes per frame (min, mean, max), luma PSNR of the
+first --psnr-frames frames, and the time of one call's search and code kernels from torch.profiler; for the 1 x 300
+EMAGE clip also the macroblock shares over the first --me-mb-frames frames of the first GOP at gop 30, with P split
+into zero and non-zero vectors, counted by the CPU restatement (tests/h264_me_ref.py; the whole 30-frame GOP takes it
+too long at 960 x 720); and the output stage (render + write_mp4) at gop 30 with search 0 against search 16.
 The card's name, power limit and max SM clock are read in the same run.  Nothing is written except OUT."""
 import ctypes
 import argparse
@@ -50,6 +57,7 @@ from synthetic_models import build_lstm_product, build_product, smplx_surface_ar
 
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 import h264_gop_ref  # noqa: E402
+import h264_me_ref  # noqa: E402
 
 QP = 20
 
@@ -231,6 +239,104 @@ def output_stage_gop(r, pred, reps):
     return {f"gop{g}": {"s_median": statistics.median(v), "s_all": v, "file_bytes": size[g]} for g, v in res.items()}
 
 
+def kernel_split(frames, gop, search):
+    """Summed CUDA time (ms) of each kernel kind in one video.encode call, from torch.profiler."""
+    from torch.profiler import ProfilerActivity, profile
+    video.encode(frames, qp=QP, gop=gop, search=search)
+    torch.cuda.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        video.encode(frames, qp=QP, gop=gop, search=search)
+        torch.cuda.synchronize()
+    out = {}
+    for e in prof.key_averages():
+        kind = next((k for k in ("search", "encode_kernel", "gather") if k in e.key), None)
+        if kind:
+            out[kind] = out.get(kind, 0.0) + e.device_time_total / 1e3
+    return out
+
+
+def me_arms(frames, reps, psnr_frames, mb_frames, tmp):
+    """gop 30 and T with search 0, 16 and 32, alternating in the timed loop: encode ms, bytes per frame, luma PSNR,
+    the search / code kernel split; with mb_frames, the macroblock shares of the first mb_frames frames at gop 30."""
+    t = frames.shape[1] if frames.dim() == 5 else frames.shape[0]
+    arms = [(g, s) for g in (30, t) for s in (0, 16, 32)]
+    ms = {a: [] for a in arms}
+    for g, s in arms:
+        video.encode(frames, qp=QP, gop=g, search=s)          # warm-up
+    torch.cuda.synchronize()
+    for _ in range(reps):
+        for g, s in arms:
+            ms[(g, s)].append(event_ms(lambda: video.encode(frames, qp=QP, gop=g, search=s)))
+    out = {}
+    clip = frames[0] if frames.dim() == 5 else frames
+    for g, s in arms:
+        sizes = video.encode(frames, qp=QP, gop=g, search=s)[1].cpu().numpy()
+        path = video.write_mp4(clip, os.path.join(tmp, f"g{g}s{s}.mp4"), fps=30, qp=QP, gop=g, search=s)
+        psnr_mean, psnr_min = luma_psnr(clip, path, psnr_frames)
+        a = out[f"gop{g}_search{s}"] = {
+            "encode_ms_median": statistics.median(ms[(g, s)]), "encode_ms_all": ms[(g, s)],
+            "bytes_per_frame_mean": float(sizes.mean()), "bytes_per_frame_min": int(sizes.min()),
+            "bytes_per_frame_max": int(sizes.max()), "file_bytes_clip0": os.path.getsize(path),
+            "luma_psnr_db_mean": psnr_mean, "luma_psnr_db_min": psnr_min,
+            "kernel_ms": kernel_split(frames, g, s)}
+        if mb_frames and g == 30:
+            enc = h264_me_ref.encode_clip(list(clip[:mb_frames].cpu().numpy()), QP, g, s)
+            types = np.concatenate([e[2].reshape(-1) for e in enc])
+            moved = np.concatenate([(e[3] if e[3] is not None else np.zeros(e[2].shape + (2,), int)).any(-1)
+                                    .reshape(-1) for e in enc])
+            share = {k: float((types == k).mean()) for k in ("SKIP", "DC", "H", "PCM")}
+            share["P_zero"] = float(((types == "P") & ~moved).mean())
+            share["P_nonzero"] = float(((types == "P") & moved).mean())
+            a["mb_share_first_frames"] = {"frames": mb_frames, **share}
+            assert [e[0] for e in enc] == [bytes(x) for x in _first_samples(clip[:mb_frames], g, s)]
+        print("  arm", g, s, json.dumps({k: v for k, v in a.items() if k != "encode_ms_all"}), flush=True)
+    return out
+
+
+def _first_samples(clip, gop, search):
+    data, nbytes = video.encode(clip, qp=QP, gop=gop, search=search)
+    return [data[i, :k].cpu().numpy().tobytes() for i, k in enumerate(nbytes.tolist())]
+
+
+def output_stage_me(r, pred, reps):
+    """Render + video.write_mp4 of one 300-frame EMAGE clip at gop 30, search 0 against search 16, alternating."""
+    poses, expr, trans = (pred[k][:1] for k in ("motion_axis_angle", "expression", "trans"))
+    res, size = {0: [], 16: []}, {}
+    for _ in range(reps):
+        for s in res:
+            d = tempfile.mkdtemp()
+            try:
+                torch.cuda.synchronize()
+                t0 = time.perf_counter()
+                frames = r.render_sequence(poses, expr, trans)[0]
+                video.write_mp4(frames, os.path.join(d, "clip.mp4"), fps=30, qp=QP, gop=30, search=s)
+                res[s].append(time.perf_counter() - t0)
+                size[s] = os.path.getsize(os.path.join(d, "clip.mp4"))
+            finally:
+                shutil.rmtree(d)
+    return {f"search{s}": {"s_median": statistics.median(v), "s_all": v, "file_bytes": size[s]}
+            for s, v in res.items()}
+
+
+def run_me(args, r, pred, res, tmp):
+    for clips in (1, 8):
+        frames = r.render_sequence(*(pred[k][:clips] for k in ("motion_axis_angle", "expression", "trans")))
+        print("me emage", clips, flush=True)
+        res[f"me_emage_sequence_{clips}x300"] = me_arms(frames, args.reps, args.psnr_frames,
+                                                        args.me_mb_frames if clips == 1 else 0, tmp)
+        del frames
+    camn = build_lstm_product("camn", device="cuda")
+    poses = camn(torch.from_numpy(synth_audio(1, 160000, 5)).cuda(),
+                 torch.zeros(1, 1, dtype=torch.long, device="cuda"))["motion_axis_angle"]
+    poses = poses.reshape(1, poses.shape[1], 165)
+    frames = r.render_body(poses, torch.zeros(1, poses.shape[1], 3, device="cuda"), upsample=2)
+    print("me camn", flush=True)
+    res["me_camn_body_1x10s"] = me_arms(frames, args.reps, args.psnr_frames, 0, tmp)
+    del frames
+    res["output_stage_me_1x300"] = output_stage_me(r, pred, args.stage_reps)
+    print("output stage me", json.dumps(res["output_stage_me_1x300"]), flush=True)
+
+
 def output_stage(r, pred, reps):
     """One 300-frame EMAGE clip from poses to files, alternating the two arms, host clock around work that ends in
     files: render + video.write_mp4 against render + png.write_frames."""
@@ -312,6 +418,8 @@ def main():
     ap.add_argument("--baseline-lib", default=None,
                     help="libpm_emage.so of another build to time pm_h264_encode against")
     ap.add_argument("--gop-only", action="store_true", help="only the GOP arms and the gop output stage")
+    ap.add_argument("--me-only", action="store_true", help="only the motion search arms and their output stage")
+    ap.add_argument("--me-mb-frames", type=int, default=4, help="frames the restatement counts macroblocks over")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "the video benchmark measures the GPU: no CUDA device found"
     torch.cuda.set_device(0)
@@ -321,7 +429,7 @@ def main():
     res = {"card": card()}
     tmp = tempfile.mkdtemp()
     try:
-        run(args, r, pred, res, tmp)
+        (run_me if args.me_only else run)(args, r, pred, res, tmp)
     finally:
         shutil.rmtree(tmp, ignore_errors=True)
     res["card_after"] = card()
