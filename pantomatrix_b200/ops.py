@@ -89,8 +89,10 @@ def tapgemm(a, w, bias, *, rows_out=None, stride=1, pad=0, act=ACT_NONE, slope=0
     if residual is not None:
         _chk(residual)
         assert residual.shape == out.shape
-    # a Linear (taps == 1, no padding) over contiguous batches is one tall matrix: better tile use
-    if (taps == 1 and pad == 0 and stride == 1 and batch > 1 and a.stride(0) == rows_in * a.stride(1)
+    # a Linear (taps == 1, no padding) over contiguous batches is one tall matrix: better tile use.  Only when every
+    # input row has its output row: with rows_out < rows_in, clip b's rows would start at b * rows_out of the tall A.
+    if (taps == 1 and pad == 0 and stride == 1 and batch > 1 and rows_out == rows_in
+            and a.stride(0) == rows_in * a.stride(1)
             and out.stride(0) == rows_out * out.stride(1)
             and (residual is None or residual.stride(0) == rows_out * residual.stride(1))):
         a = a.reshape(1, batch * rows_in, cin) if a.is_contiguous() else a.as_strided(

@@ -13,6 +13,7 @@ from body_cases import (JOINT_GATE, ROTATION_GATE, VELOCITY_GATE, VERTEX_GATE, f
                         random_tree, small_arrays)
 from helpers import check_tapgemm, use_precision
 from oracle.smplx_oracle import SmplxRestatement, forward_poses
+from simt_bounds import tapgemm_f32, within
 from pantomatrix_b200 import _lib
 from pantomatrix_b200.body_model import ALL_JOINTS, MOTION_REP_JOINTS, SmplxBodyModel
 from synthetic_models import SMPLX_PARENTS, smplx_arrays
@@ -82,12 +83,10 @@ def test_fk_joints_against_float64():
 
 
 def _fp32_gemm_bound_check(feat, lin, got):
-    """fp32 SIMT blend GEMM: |err| <= (K + 2) 2^-24 (|A| |W| + |bias|) + 2^-24 |result|, every element."""
-    a = feat[:, :886].double()
-    w = lin.w[0].double()
-    want = a @ w.t() + lin.b.double()
-    bound = 888 * 2.0 ** -24 * (a.abs() @ w.abs().t() + lin.b.double().abs()) + 2.0 ** -24 * want.abs()
-    assert bool(((got.double() - want).abs() <= bound).all())
+    """fp32 SIMT blend GEMM: |err| <= (K + 2) 2^-24 (|A| |W| + |bias|) + 2^-24 |result|, every element
+    (simt_bounds.tapgemm_f32)."""
+    want, bound = tapgemm_f32(feat[:, :886].unsqueeze(0), lin.w, lin.b)
+    assert within(got.unsqueeze(0), want, bound)
 
 
 @pytest.mark.parametrize("precision", ["fp16x3", "bf16x6", "fp32"])
