@@ -564,8 +564,10 @@ def lstm_bidir(xproj, whh, barrier, hidden):
 def rot6d_to_aa(rot6d, slot, n_sel):
     """rot6d (..., n_sel*6) -> axis-angle (..., 165); slot: int32[55] device tensor (position among the selected
     joints or -1)."""
-    _chk(rot6d)
+    _chk(rot6d), _chk(slot, torch.int32)
     assert rot6d.is_contiguous() and rot6d.shape[-1] == n_sel * 6
+    if slot.shape != (55,) or slot.device != rot6d.device:
+        raise _lib.PmError(f"slot must be a dense int32 [55] tensor on {rot6d.device}, got {tuple(slot.shape)} on {slot.device}")
     rows = rot6d.numel() // (n_sel * 6)
     out = torch.empty(*rot6d.shape[:-1], 165, device=rot6d.device, dtype=torch.float32)
     _call("pm_rot6d_to_aa_f32", rot6d.data_ptr(), rows, n_sel, slot.data_ptr(), out.data_ptr(), _stream())
@@ -619,7 +621,12 @@ def motion_rep(poses, joints, dt, two_dt, out):
     """rep15d (batch, t, 825) of get_motion_rep_tensor from poses (batch, t, 165) and joints (batch, t, 55, 3)."""
     _chk(poses), _chk(joints), _chk(out)
     assert joints.is_contiguous() and out.is_contiguous()
+    if poses.dim() != 3 or poses.shape[-1] != 165:
+        raise _lib.PmError(f"poses must be a (batch, t, 165) view, got {tuple(poses.shape)}")
     batch, t, _ = poses.shape
+    if joints.numel() != batch * t * 165 or tuple(out.shape) != (batch, t, 825):
+        raise _lib.PmError(f"joints must hold (batch, t, 55, 3) and out be (batch, t, 825) for poses {tuple(poses.shape)}, "
+                           f"got {tuple(joints.shape)} and {tuple(out.shape)}")
     pb, pt = _clip_frame_strides(poses)
     _call("pm_motion_rep_f32", poses.data_ptr(), pb, pt, joints.data_ptr(), batch, t, float(dt), float(two_dt),
           out.data_ptr(), _stream())
@@ -777,9 +784,28 @@ def softmax2_mix(sel, c1, c2, out=None):
     """out[..., :] = softmax(sel[..., 0:2])[0] * c1 + [1] * c2 (out may be a column slice of a wider tensor)."""
     _chk(sel), _chk(c1), _chk(c2)
     assert sel.is_contiguous() and c1.is_contiguous() and c2.is_contiguous() and sel.shape[-1] == 2
+    assert c2.shape == c1.shape and sel.shape[:-1] == c1.shape[:-1]
     ch = c1.shape[-1]
     rows = c1.numel() // ch
     if out is None:
         out = torch.empty_like(c1)
-    _call("pm_softmax2_mix_f32", sel.data_ptr(), c1.data_ptr(), c2.data_ptr(), out.data_ptr(), rows, ch, out.stride(-2), _stream())
+    _chk(out)
+    if out.shape != c1.shape:
+        raise _lib.PmError(f"out must be {tuple(c1.shape)}, got {tuple(out.shape)}")
+    _call("pm_softmax2_mix_f32", sel.data_ptr(), c1.data_ptr(), c2.data_ptr(), out.data_ptr(), rows, ch, _row_stride(out),
+          _stream())
     return out
+
+
+def _row_stride(x):
+    """The one row stride of a (..., ch) view whose rows lie evenly spaced, as in a (rows, ld) matrix - the layout a
+    kernel taking a single leading dimension can address.  Raises PmError for any other view, e.g. a [:, :T] slice of
+    a (B, T', ch) buffer with T' > T, whose clips lie T' rows apart."""
+    lead = [(n, st) for n, st in zip(x.shape[:-1], x.stride()[:-1]) if n != 1]
+    ld = lead[-1][1] if lead else x.shape[-1]
+    step = ld
+    for n, st in reversed(lead):
+        if st != step:
+            raise _lib.PmError(f"rows of a {tuple(x.shape)} view with strides {x.stride()} are not evenly spaced")
+        step *= n
+    return ld

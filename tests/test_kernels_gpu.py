@@ -431,28 +431,17 @@ def test_gather_rows(ops):
 
 
 def test_pose_compose_matches_oracle(ops):
-    from oracle import emage_oracle as O
-    from helpers import geodesic_deg
+    import pose_bounds as pb
     bs, t = 3, 50
     parts = dict(face=_rand(bs, t, 106, seed=39), upper=_rand(bs, t, 78, seed=40), hands=_rand(bs, t, 180, seed=41),
                  lower=_rand(bs, t, 61, seed=42))
     expr, aa, m4 = ops.pose_compose(parts["face"], parts["upper"], parts["hands"], parts["lower"], bs, t, "cuda")
-    c = {k: v.cpu() for k, v in parts.items()}
-    jaw = O.rot6d_to_axis_angle(c["face"][:, :, :6])
-    up = O.rot6d_to_axis_angle(c["upper"].reshape(bs, t, -1, 6)).reshape(bs, t, -1)
-    ha = O.rot6d_to_axis_angle(c["hands"].reshape(bs, t, -1, 6)).reshape(bs, t, -1)
-    lo = O.rot6d_to_axis_angle(c["lower"][:, :, :54].reshape(bs, t, -1, 6)).reshape(bs, t, -1)
-    want = (O._scatter_joints(up, O.UPPER_JOINTS, bs, t) + O._scatter_joints(ha, O.HANDS_JOINTS, bs, t)
-            + O._scatter_joints(lo, O.LOWER_JOINTS, bs, t))
-    want[:, :, 66:69] = jaw
-    assert torch.equal(expr.cpu(), c["face"][:, :, 6:])
-    assert torch.equal(m4.cpu()[:, :, 330:], c["lower"][:, :, 54:])
-    geo = geodesic_deg(aa.cpu().reshape(bs, t, 55, 3), want.reshape(bs, t, 55, 3))
-    assert geo.max() < 0.02, geo.max()
-    far = (want.reshape(bs, t, 55, 3).norm(dim=-1) < 3.0).unsqueeze(-1).expand(bs, t, 55, 3).reshape(bs, t, 165)
-    assert (aa.cpu() - want)[far].abs().max() < 1e-3           # the pose gate; fp32 quaternion route loses ~2e-4
-    want6 = O.axis_angle_to_rot6d(want.reshape(bs, t, 55, 3)).reshape(bs, t, 330)
-    assert (m4.cpu()[:, :, :330] - want6).abs().max() < 1e-3
+    # every element within its float64 bound (tests/pose_bounds.py), the near-pi joints included
+    want, bound, decided = pb.pose_compose(parts["face"], parts["upper"], parts["hands"], parts["lower"])
+    assert pb.within(aa, pb.pick_signs(aa, want, decided), bound)
+    (w4, b4), want_expr = pb.pose_compose_rest(parts["face"], parts["lower"], aa)
+    assert pb.within(m4, w4, b4)
+    assert torch.equal(expr, want_expr) and torch.equal(m4[:, :, 330:], parts["lower"][:, :, 54:])
     # the reference's zero branches (M.py:143-146,174-178): eyes and missing parts are identity rotations
     expr0, aa0, m40 = ops.pose_compose(None, parts["upper"], None, None, bs, t, "cuda")
     assert expr0.abs().max() == 0 and aa0[:, :, 66:75].abs().max() == 0
