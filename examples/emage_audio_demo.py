@@ -60,6 +60,8 @@ def main():
                     help="--video keyframe interval: an IDR frame every GOP frames, P frames between (1: all IDR)")
     ap.add_argument("--search", type=int, default=0,
                     help="--video motion search range in pixels, 0..32, for the P frames (0: zero motion)")
+    ap.add_argument("--intra4x4", action="store_true",
+                    help="--video: also code intra macroblocks as Intra 4x4 (nine prediction modes per 4x4 block)")
     args = ap.parse_args()
     if not args.synthetic and not args.checkpoint:
         ap.error("give --checkpoint DIR or --synthetic")
@@ -102,7 +104,7 @@ def main():
                 video.write_mp4(drawn, os.path.splitext(npz)[0] + ".mp4", fps=30,
                                 audio=read_track(os.path.join(args.audio_folder, name), device)
                                 if args.with_audio else None, gop=args.gop,
-                                search=args.search)
+                                search=args.search, intra4x4=args.intra4x4)
         frames += t
     print(f"generate total {frames / fps:.2f} seconds motion in {time.time() - t0:.2f} seconds")
 

@@ -35,6 +35,7 @@ extern "C" {
 
 #define PM_ABI_VERSION 6
 #define PM_FMT_F16 0x100
+#define PM_H264_I4X4 0x100   /* pm_h264_encode / _gop / _me: bit 8 of `qp` adds Intra 4x4 (I_NxN) macroblocks */
 #define PM_TC_TILE_SHIFT 16   /* pm_tapgemm_tc: N tile override in bits 16-23 of `nsplit` */
 #define PM_TC_STORE_LOOP (1 << 24)   /* pm_tapgemm_tc: bit 24 of `nsplit` forces the per-element store loop */
 int pm_abi_version(void);
@@ -443,6 +444,32 @@ int pm_h264_encode_gop(const unsigned char* frames, long long f_fs, int n_frames
 int pm_h264_encode_me(const unsigned char* frames, long long f_fs, int n_frames, int clip_len, int h, int w, int qp,
                       unsigned char* scratch, long long slice_cap, int* slice_bytes, int gop, unsigned char* recon,
                       long long recon_stride, int search, short* mv, long long mv_len, void* stream);
+/* Intra 4x4: qp | PM_H264_I4X4 (bit 8) in pm_h264_encode, pm_h264_encode_gop (forwarded at gop 1) and
+ * pm_h264_encode_me; every other bit above the quantiser is refused.  Without the bit every byte is the rule above.
+ * With it, in I and P slices, every coded macroblock also has an I_NxN candidate:
+ *   availability (6.4.11.4): the macroblock above is another slice and the one to the right is not coded, so blocks of
+ *     the top block row have no above samples, above-right samples come only from blocks of the same macroblock
+ *     coded before (luma4x4BlkIdx order; missing ones are p[3, -1] when the above samples exist, 8.3.1.2), and the
+ *     left (and, in block rows 1..3, above-left) samples of block column 0 come from the left macroblock's
+ *     reconstruction, whatever its type (constrained_intra_pred_flag stays 0);
+ *   mode per 4x4 block, in luma4x4BlkIdx order: the candidates are the modes 8.3.1.2 defines from the available
+ *     samples; J = SAD(source, prediction) + LAMBDA[qp] b, b = 1 when the mode equals predIntra4x4PredMode, else 4;
+ *     lowest J, ties to the lower mode.  predIntra4x4PredMode (8.3.1.1) is 2 for every top-row block and every block
+ *     of the frame's column 0, and a left neighbour outside an I_NxN macroblock counts as mode 2;
+ *   residual: the 4x4 transform of all 16 coefficients, quantised with f = 2^qbits / 3, reconstructed by 8.5.12 with
+ *     the DC scaled like every other position; each block is reconstructed before the next is predicted;
+ *   choice: J4 = the sum of the 16 blocks' J, J16 = the Intra16x16 candidate's SAD (DC or Horizontal as above); the
+ *     macroblock is I_NxN when J4 + 6 LAMBDA[qp] < J16.  In P slices the intra cost is min(J16, J4 + 6 LAMBDA[qp]),
+ *     and the inter candidate (zero-motion or searched) wins when its luma SAD is <= that cost; the P_Skip test and
+ *     the vectors do not change;
+ *   syntax: mb_type I_NxN (ue(0) in I slices, ue(5) in P slices), 16 x (prev_intra4x4_pred_mode_flag, or 0 and
+ *     rem_intra4x4_pred_mode), intra_chroma_pred_mode 0 (chroma DC, coded as for Intra16x16), coded_block_pattern by
+ *     Table 9-4's Intra column (luma bit b8 when a 4x4 block of 8x8 block b8 has a level), mb_qp_delta 0 only when
+ *     cbp > 0, residual_block(16) per 4x4 block of each set 8x8 bit; nC by 9.2.1 (P_Skip 0, a clear cbp bit 0,
+ *     I_PCM 16, an Intra16x16 AC block its TotalCoeff);
+ *   I_PCM replaces an I_NxN macroblock in the same cases as above (over 3200 bits, a level_prefix above 15), so the
+ *     slice bounds, slot sizes, SPS, PPS and MP4 boxes are unchanged.
+ * The launches are as without the bit (other kernel instances, the same workspaces). */
 int pm_h264_gather(int n_frames, int h, int w, const unsigned char* scratch, long long slice_cap,
                    const int* slice_bytes, unsigned char* data, long long cap, long long* nbytes, void* stream);
 

@@ -1,7 +1,8 @@
 // H.264 encoding of RGB8 frames (pantomatrix_b200/video.py): one access unit per frame by the rule of
 // include/pm_emage.h and DESIGN.md section 12 (one slice per macroblock row, Intra16x16 DC / Horizontal or I_PCM,
 // CAVLC, deblocking off; with a keyframe interval gop > 1, P frames of P_Skip and zero-motion inter macroblocks
-// between the IDR frames, or with a motion search range, quarter-pel vectors against the whole previous frame).  Two
+// between the IDR frames, or with a motion search range, quarter-pel vectors against the whole previous frame; with
+// PM_H264_I4X4 in qp, Intra 4x4 (I_NxN) macroblocks beside Intra16x16 in I and P slices).  Two
 // launches per call after the caller's memset of the output slots (pm_h264_encode_me: 2 gop - 1 encode launches,
 // h264_search_kernel before each P frame's):
 //   pm_h264_encode  one warp per (frame, macroblock row): the row's slice, emulation prevention applied, into its
@@ -10,8 +11,9 @@
 //   pm_h264_gather  one CTA per (frame, row): the slice's offset in the frame's sample, the copy, the frame's size.
 // A warp stages its bits in shared memory in stream byte order (pm_put_bits, as FLAC writes its slots), so whole
 // bytes leave the staging buffer as byte loads.
-// CPU restatement: oracle/h264_oracle.py, tests/h264_gop_ref.py for P frames, tests/h264_me_ref.py for motion.  Every
-// byte depends only on the frame (its GOP's frames), qp, gop, search and the parity of its index (t div gop).
+// CPU restatement: oracle/h264_oracle.py, tests/h264_gop_ref.py for P frames, tests/h264_me_ref.py for motion,
+// tests/h264_i4_ref.py for Intra 4x4.  Every byte depends only on the frame (its GOP's frames), qp, gop, search, the
+// Intra 4x4 switch and the parity of its index (t div gop).
 #include <cub/block/block_reduce.cuh>
 
 #include <type_traits>
@@ -248,6 +250,16 @@ struct Warp : std::conditional_t<GOP, WarpRef, WarpNoRef> {
   int lnz[8];                              // left neighbour's right blocks' TotalCoeff: luma rows, Cb rows, Cr rows
   unsigned char y[256], cb[64], cr[64];    // source samples
 };
+// The I4 instances' warp state: the I_NxN candidate beside the others.
+template <bool GOP>
+struct WarpI4 : Warp<GOP> {
+  int lev4[16][16];                        // each block's 16 levels (luma4x4BlkIdx, scan order)
+  int tc4[16];                             // each block's TotalCoeff (raster)
+  int j4[18];                              // J of each (block of the step, mode)
+  unsigned char rec4[256];                 // the candidate's luma reconstruction
+  unsigned char m4[16], pm4[16];           // each block's mode and predIntra4x4PredMode (raster)
+  unsigned char lm4[4];                    // the left macroblock's right blocks' modes; 2 when it is not I_NxN
+};
 
 __device__ __forceinline__ unsigned stg_byte(const unsigned* stg, int i) {
   return reinterpret_cast<const unsigned char*>(stg)[i];
@@ -317,6 +329,35 @@ __constant__ unsigned char LAMBDA[52] = {0,  0,  0,  0,  0,  0,  0,  1,  1,  1, 
                                          2,  2,  2,  3,  3,  3,  4,  4,  5,  5,  6,  7,  7,  8,  9,  10, 12, 13,
                                          15, 17, 19, 21, 23, 26, 30, 33, 37, 42, 47, 53, 59, 66, 74, 83};
 
+// Table 9-4 (ChromaArrayType 1): codeNum of each coded_block_pattern of an Intra_4x4 macroblock.
+__constant__ unsigned char INTRA_CODE[48] = {3,  29, 30, 17, 31, 18, 37, 8,  32, 38, 19, 9,  20, 10, 11, 2,
+                                             16, 33, 34, 21, 35, 22, 39, 4,  36, 40, 23, 5,  24, 6,  7,  1,
+                                             41, 42, 43, 25, 44, 26, 46, 12, 45, 47, 27, 13, 28, 14, 15, 0};
+
+// ---- Intra 4x4 (8.3.1.2) ----
+// A block's neighbours as one edge E[0..12]: p[-1, 3..0], p[-1, -1], p[0..7, -1].  Each sample of modes 0, 1, 3..8 is
+// kind << 4 | c: kind 0 E[c], 1 (E[c] + E[c + 1] + 1) >> 1, 2 (E[c - 1] + 2 E[c] + E[c + 1] + 2) >> 2 with the
+// indices clamped to 0..12 (which gives Diagonal_Down_Left's (3, 3) and Horizontal_Up's zHU = 5); raster order.
+__constant__ unsigned char PRED4[9][16] = {
+    {0x05, 0x06, 0x07, 0x08, 0x05, 0x06, 0x07, 0x08, 0x05, 0x06, 0x07, 0x08, 0x05, 0x06, 0x07, 0x08},
+    {0x03, 0x03, 0x03, 0x03, 0x02, 0x02, 0x02, 0x02, 0x01, 0x01, 0x01, 0x01, 0x00, 0x00, 0x00, 0x00},
+    {0},
+    {0x26, 0x27, 0x28, 0x29, 0x27, 0x28, 0x29, 0x2a, 0x28, 0x29, 0x2a, 0x2b, 0x29, 0x2a, 0x2b, 0x2c},
+    {0x24, 0x25, 0x26, 0x27, 0x23, 0x24, 0x25, 0x26, 0x22, 0x23, 0x24, 0x25, 0x21, 0x22, 0x23, 0x24},
+    {0x14, 0x15, 0x16, 0x17, 0x24, 0x25, 0x26, 0x27, 0x23, 0x14, 0x15, 0x16, 0x22, 0x24, 0x25, 0x26},
+    {0x13, 0x24, 0x25, 0x26, 0x12, 0x23, 0x13, 0x24, 0x11, 0x22, 0x12, 0x23, 0x10, 0x21, 0x11, 0x22},
+    {0x15, 0x16, 0x17, 0x18, 0x26, 0x27, 0x28, 0x29, 0x16, 0x17, 0x18, 0x19, 0x27, 0x28, 0x29, 0x2a},
+    {0x12, 0x22, 0x11, 0x21, 0x11, 0x21, 0x10, 0x20, 0x10, 0x20, 0x00, 0x00, 0x00, 0x00, 0x00, 0x00}};
+// The 10 wavefront steps of a macroblock's blocks (raster, -1 none): a block follows its left, above-left, above and
+// above-right neighbours, so step bx + 2 by holds every block that can go.
+__constant__ signed char WAVE[10][2] = {{0, -1}, {1, -1}, {2, 4}, {3, 5}, {6, 8}, {7, 9}, {10, 12}, {11, 13},
+                                        {14, -1}, {15, -1}};
+constexpr unsigned AR_AVAIL = 0x5750;      // raster blocks whose above-right block is coded before them (6.4.11.4)
+// luma4x4BlkIdx -> raster block, and (being its own inverse) raster -> luma4x4BlkIdx
+__constant__ unsigned char BLK_RASTER[16] = {0, 1, 4, 5, 2, 3, 6, 7, 8, 9, 12, 13, 10, 11, 14, 15};
+__constant__ unsigned char SCAN_OF[16] = {0, 1, 5, 6, 2, 4, 7, 12, 3, 8, 11, 13, 9, 10, 14, 15};   // raster -> scan
+constexpr int C_I4 = 6;                    // an I_NxN macroblock's J4 is charged C_I4 lambda(qp) more (pm_emage.h)
+
 __device__ __forceinline__ int se_bits(int v) { return ue_bits(v > 0 ? 2 * v - 1 : -2 * v); }
 
 __device__ __forceinline__ int clip255(int v) { return min(255, max(0, v)); }
@@ -362,13 +403,18 @@ __device__ __forceinline__ void rgb(const unsigned char* p, int& r, int& g, int&
 // GOP_ZERO: the warp codes the row of each of the chain's frames in turn, the IDR frame first, and keeps the row's
 // reconstruction in J.recon for the next frame's P slice.  GOP_ME: the warp codes the row of the chain's frame J.k
 // only, against the whole reconstruction of frame k - 1, with the vectors h264_search_kernel chose, and writes frame
-// k's reconstruction to the other buffer; kernel boundaries order the frames.
-template <Mode MODE>
-__global__ void __launch_bounds__(32 * WARPS) h264_encode_kernel(Job J) {
+// k's reconstruction to the other buffer; kernel boundaries order the frames.  I4: each coded macroblock also gets
+// the I_NxN candidate, its blocks in 10 wavefront steps (lanes per (block, mode) for the costs, one per block for the
+// transform), the candidate's luma reconstruction in shared memory.
+// (The I4 instances ask for one CTA per SM at least, which lets the GOP_ZERO one keep its state in registers; the bound
+// is 0, no request, for the others.)
+template <Mode MODE, bool I4>
+__global__ void __launch_bounds__(32 * WARPS, I4 ? 1 : 0) h264_encode_kernel(Job J) {
   constexpr bool GOP = MODE != INTRA, ME = MODE == GOP_ME;
-  __shared__ Warp<GOP> WS[WARPS];
+  using W = std::conditional_t<I4, WarpI4<GOP>, Warp<GOP>>;
+  __shared__ W WS[WARPS];
   const int lane = threadIdx.x & 31;
-  Warp<GOP>& S = WS[threadIdx.x >> 5];
+  W& S = WS[threadIdx.x >> 5];
   const int mbw = J.w >> 4, mbh = J.h >> 4;
   const long long slice = (long long)blockIdx.x * WARPS + (threadIdx.x >> 5);
   const long long chains = GOP ? (long long)(J.n_frames / J.clip_len) * J.chains_per_clip : J.n_frames;
@@ -603,6 +649,9 @@ __global__ void __launch_bounds__(32 * WARPS) h264_encode_kernel(Job J) {
             S.lc[k][r] = S.ref(k, 8 * r + 7);
           }
           if (lane < 8) S.lnz[lane] = 0;
+          if constexpr (I4) {
+            if (lane < 4) S.lm4[lane] = 2;
+          }
           __syncwarp();
           continue;
         }
@@ -647,21 +696,131 @@ __global__ void __launch_bounds__(32 * WARPS) h264_encode_kernel(Job J) {
       sad_dc = warp_sum(sad_dc);
       sad_h = warp_sum(sad_h);
       use_h = have_left && sad_h < sad_dc;
-      // inter when the zero-motion residual's luma SAD is at most the Intra16x16 candidate's
-      const bool inter = pf && warp_sum(sad_p) <= (use_h ? sad_h : sad_dc);
+      int j_intra = 0;                                     // I4: the intra candidate's cost
+      bool nxn = false;                                    // I4: the I_NxN candidate is the intra choice
+      if constexpr (I4) {
+        // ---- the I_NxN candidate: per wavefront step, lane 9 s + m costs mode m of the step's block s, then lane s
+        // transforms, quantises and reconstructs block s by its lowest-J mode ----
+        const int lam = LAMBDA[qp];
+        int jsum = 0;
+        for (int step = 0; step < 10; ++step) {
+          const int slot = lane / 9, m = lane - 9 * slot;
+          const int blk = slot < 2 ? WAVE[step][slot] : -1;
+          const int bx = blk & 3, by = blk >> 2, X = 4 * bx, Y = 4 * by;
+          const bool la = bx > 0 || have_left, ua = by > 0, ar = (AR_AVAIL >> blk) & 1;
+          // E[c] of the block's edge (clamped to 0..12); only the samples its candidate modes read
+          auto edge = [&](int c) -> int {
+            c = min(12, max(0, c));
+            if (c < 5) return bx ? S.rec4[(Y + 3 - c) * 16 + X - 1] : S.ly[Y + 3 - c];
+            const int x = c > 8 && !ar ? 3 : c - 5;
+            return S.rec4[(Y - 1) * 16 + X + x];
+          };
+          auto pred = [&](int mode, int i, int dc) -> int {
+            if (mode == 2) return dc;
+            const int t = PRED4[mode][i], c = t & 15;
+            if (t >> 4 == 0) return edge(c);
+            if (t >> 4 == 1) return (edge(c) + edge(c + 1) + 1) >> 1;
+            return (edge(c - 1) + 2 * edge(c) + edge(c + 1) + 2) >> 2;
+          };
+          auto dc_of = [&]() -> int {
+            int sa = 0, sl = 0;
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+              if (ua) sa += edge(5 + i);
+              if (la) sl += edge(3 - i);
+            }
+            return la && ua ? (sa + sl + 4) >> 3 : (la ? (sl + 2) >> 2 : (ua ? (sa + 2) >> 2 : 128));
+          };
+          if (blk >= 0) {
+            // 8.3.1.1: DC when the block to the left or above is not available; a left macroblock not I_NxN counts as 2
+            const int pm = la && ua ? min(bx ? (int)S.m4[blk - 1] : (int)S.lm4[by], (int)S.m4[blk - 4]) : 2;
+            const bool cand = m == 2 || (m == 0 || m == 3 || m == 7 ? ua : (m == 1 || m == 8 ? la : la && ua));
+            int j = 0x7fffffff;
+            if (cand) {
+              const int dc = m == 2 ? dc_of() : 0;
+              int sad = 0;
+#pragma unroll 4
+              for (int i = 0; i < 16; ++i) sad += abs((int)S.y[(Y + (i >> 2)) * 16 + X + (i & 3)] - pred(m, i, dc));
+              j = sad + lam * (m == pm ? 1 : 4);
+            }
+            S.j4[lane] = j;
+            if (m == 0) S.pm4[blk] = (unsigned char)pm;
+          }
+          __syncwarp();
+          if (blk >= 0 && m == 0) {                        // lanes 0 and 9: the step's blocks
+            int best = 0, bj = S.j4[lane];
+#pragma unroll
+            for (int k = 1; k < 9; ++k)
+              if (S.j4[lane + k] < bj) { bj = S.j4[lane + k]; best = k; }
+            jsum += bj;
+            S.m4[blk] = (unsigned char)best;
+            const int dc = best == 2 ? dc_of() : 0;
+            int x[16];
+#pragma unroll
+            for (int i = 0; i < 16; ++i) x[i] = (int)S.y[(Y + (i >> 2)) * 16 + X + (i & 3)] - pred(best, i, dc);
+            fdct(x);
+            const int b16 = BLK_RASTER[blk];
+            int total = 0;
+#pragma unroll
+            for (int i = 0; i < 16; ++i) {
+              const int l = quant(x[i], MF[qp % 6][pos_class(i)], fq, qbits);
+              S.lev4[b16][SCAN_OF[i]] = l;
+              total += l != 0;
+              const int ls = 16 * VS[qp % 6][pos_class(i)];
+              x[i] = qp >= 24 ? (l * ls) << (qp / 6 - 4) : (l * ls + (1 << (3 - qp / 6))) >> (4 - qp / 6);
+            }
+            S.tc4[blk] = total;
+            idct(x);
+#pragma unroll
+            for (int i = 0; i < 16; ++i)
+              S.rec4[(Y + (i >> 2)) * 16 + X + (i & 3)] = (unsigned char)min(255, max(0, pred(best, i, dc) + x[i]));
+          }
+          __syncwarp();
+        }
+        const int j4 = warp_sum(jsum) + C_I4 * lam;
+        nxn = j4 < (use_h ? sad_h : sad_dc);
+        j_intra = nxn ? j4 : (use_h ? sad_h : sad_dc);
+      }
+      // inter when the inter candidate's luma SAD is at most the intra candidate's cost
+      const bool inter = pf && warp_sum(sad_p) <= (I4 ? j_intra : (use_h ? sad_h : sad_dc));
+      if (I4 && inter) nxn = false;
       if (!inter) cdc_nz = transform(false);
+      if constexpr (I4) {
+        if (nxn) {                                         // the I_NxN luma levels replace the Intra16x16 ones
+          __syncwarp();
+          if (lane < 16) {
+            const int b16 = BLK_RASTER[lane];
+#pragma unroll
+            for (int s = 0; s < 16; ++s) S.lev[1 + b16][s] = S.lev4[b16][s];
+            S.tc[lane] = S.tc4[lane];
+          }
+          __syncwarp();
+        }
+      }
       const bool cbp_l = __ballot_sync(0xffffffffu, lane < 16 && S.tc[lane] > 0) != 0;
       const bool ac_c = __ballot_sync(0xffffffffu, lane >= 16 && lane < 24 && S.tc[lane] > 0) != 0;
       const bool dc_c = __ballot_sync(0xffffffffu, cdc_nz) != 0;
       const int cbp_c = ac_c ? 2 : (dc_c ? 1 : 0);
       // an inter macroblock's CodedBlockPatternLuma: bit b8 when a 4x4 block of 8x8 block b8 has a level
       int cbp8 = 0;
-      if (inter)
+      if (inter || (I4 && nxn))
         cbp8 = (int)__reduce_or_sync(0xffffffffu, lane < 16 && S.tc[lane] > 0
                                                       ? 1u << (((lane >> 3) << 1) | ((lane & 3) >> 1)) : 0u);
       __syncwarp();
-      // ---- reconstruction: GOP every block into J.recon, else the right column (luma bx = 3, chroma bx = 1) ----
-      if (GOP ? lane < 24 : ((lane < 16 && (lane & 3) == 3) || (lane >= 16 && lane < 24 && (lane & 1) == 1))) {
+      // ---- reconstruction: GOP every block into J.recon, else the right column (luma bx = 3, chroma bx = 1); an
+      // I_NxN macroblock's luma is the candidate's ----
+      if constexpr (I4) {
+        if (nxn) {
+          for (int p = lane; p < 256; p += 32) {
+            const int v = S.rec4[p];
+            if constexpr (ME) rrow[yo(p >> 4, mx, p & 15)] = (unsigned char)v;
+            else if constexpr (GOP) rrow[(p >> 4) * J.w + 16 * mx + (p & 15)] = (unsigned char)v;
+            if ((p & 15) == 15) S.ny[p >> 4] = v;
+          }
+        }
+      }
+      if ((GOP ? lane < 24 : ((lane < 16 && (lane & 3) == 3) || (lane >= 16 && lane < 24 && (lane & 1) == 1)))
+          && !(I4 && nxn && lane < 16)) {
         const bool luma = lane < 16;
         const int k = luma ? 0 : (lane - 16) >> 2, bi = luma ? lane : (lane - 16) & 3;
         const int by = luma ? bi >> 2 : bi >> 1, bx = GOP ? (luma ? bi & 3 : bi & 1) : (luma ? 3 : 1);
@@ -722,6 +881,18 @@ __global__ void __launch_bounds__(32 * WARPS) h264_encode_kernel(Job J) {
             b.se(ME ? mv.y - lmv.y : 0);
             b.ue(INTER_CODE[cbp8 | cbp_c << 4]);           // coded_block_pattern
             if (cbp8 | cbp_c) b.se(0);                     // mb_qp_delta
+          } else if (I4 && nxn) {
+            if constexpr (I4) {
+              b.ue(pf ? 5 : 0);                            // mb_type I_NxN
+              for (int k = 0; k < 16; ++k) {               // luma4x4BlkIdx order
+                const int r = BLK_RASTER[k], m = S.m4[r], pm = S.pm4[r];
+                if (m == pm) b.put(1, 1);                  // prev_intra4x4_pred_mode_flag
+                else b.put((unsigned)(m < pm ? m : m - 1), 4);   // 0, rem_intra4x4_pred_mode
+              }
+              b.ue(0);                                     // intra_chroma_pred_mode: DC
+              b.ue(INTRA_CODE[cbp8 | cbp_c << 4]);         // coded_block_pattern
+              if (cbp8 | cbp_c) b.se(0);                   // mb_qp_delta
+            }
           } else {
             b.ue((unsigned)((pf ? 5 : 0) + 1 + (use_h ? 1 : 2) + 4 * cbp_c + (cbp_l ? 12 : 0)));
             b.ue(0);                                       // intra_chroma_pred_mode: DC
@@ -729,16 +900,16 @@ __global__ void __launch_bounds__(32 * WARPS) h264_encode_kernel(Job J) {
           }
           return true;
         }
-        if (u == 1) return inter || residual_block(b, S.lev[0], 16, have_left ? S.lnz[0] : 0);
+        if (u == 1) return inter || (I4 && nxn) || residual_block(b, S.lev[0], 16, have_left ? S.lnz[0] : 0);
         if (u < 18) {
           const int blk = u - 2;
-          if (inter ? !((cbp8 >> (blk >> 2)) & 1) : !cbp_l) return true;
+          if (inter || (I4 && nxn) ? !((cbp8 >> (blk >> 2)) & 1) : !cbp_l) return true;
           const int by = ((blk >> 3) << 1) | ((blk >> 1) & 1), bx = (((blk >> 2) & 1) << 1) | (blk & 1);
           const bool ha = bx > 0 || have_left, hb = by > 0;
           const int na = bx > 0 ? S.tc[4 * by + bx - 1] : (have_left ? S.lnz[by] : 0);
           const int nb = hb ? S.tc[4 * (by - 1) + bx] : 0;
           const int nc = ha && hb ? (na + nb + 1) >> 1 : (ha ? na : nb);
-          return residual_block(b, S.lev[u - 1], inter ? 16 : 15, nc);
+          return residual_block(b, S.lev[u - 1], inter || (I4 && nxn) ? 16 : 15, nc);
         }
         if (u < 20) return cbp_c ? residual_block(b, S.lev[u - 1], 4, -1) : true;
         if (u < 28) {
@@ -829,6 +1000,9 @@ __global__ void __launch_bounds__(32 * WARPS) h264_encode_kernel(Job J) {
           v = S.tc[16 + 4 * k + 2 * by + 1];
         }
         S.lnz[lane] = v;
+      }
+      if constexpr (I4) {
+        if (lane < 4) S.lm4[lane] = nxn && !pcm ? S.m4[4 * lane + 3] : 2;
       }
       __syncwarp();
     }
@@ -993,17 +1167,27 @@ bool shape_ok(int frames, int h, int w) {
   return mbh * mbw <= 36864 && mbh <= 543 && mbw <= 543;
 }
 
+// qp's bits above the quantiser: PM_H264_I4X4 or nothing.
+bool split_qp(int& qp, bool& i4) {
+  i4 = (qp & PM_H264_I4X4) != 0;
+  qp &= ~PM_H264_I4X4;
+  return qp >= 0 && qp <= 51;
+}
+
 }  // namespace
 
 extern "C" int pm_h264_encode(const unsigned char* frames, long long f_fs, int n_frames, int clip_len, int h, int w,
                               int qp, unsigned char* scratch, long long slice_cap, int* slice_bytes, void* stream) {
-  PM_REQUIRE(shape_ok(n_frames, h, w) && frames && scratch && slice_bytes && f_fs >= 3LL * w * h && clip_len >= 1
-             && qp >= 0 && qp <= 51 && slice_cap >= slice_bound(w));
+  bool i4;
+  PM_REQUIRE(split_qp(qp, i4) && shape_ok(n_frames, h, w) && frames && scratch && slice_bytes && f_fs >= 3LL * w * h
+             && clip_len >= 1 && slice_cap >= slice_bound(w));
   const long long slices = (long long)n_frames * (h / 16);
   if (slices == 0) return PM_OK;
   PM_REQUIRE(slices / WARPS < 0x7fffffffLL);
-  h264_encode_kernel<INTRA><<<(unsigned)((slices + WARPS - 1) / WARPS), 32 * WARPS, 0, (cudaStream_t)stream>>>(
-      Job{frames, f_fs, n_frames, clip_len, h, w, qp, scratch, slice_cap, slice_bytes, 1, 1, nullptr, 0});
+  const Job j{frames, f_fs, n_frames, clip_len, h, w, qp, scratch, slice_cap, slice_bytes, 1, 1, nullptr, 0};
+  const unsigned grid = (unsigned)((slices + WARPS - 1) / WARPS);
+  if (i4) h264_encode_kernel<INTRA, true><<<grid, 32 * WARPS, 0, (cudaStream_t)stream>>>(j);
+  else h264_encode_kernel<INTRA, false><<<grid, 32 * WARPS, 0, (cudaStream_t)stream>>>(j);
   PM_LAUNCH_CHECK();
 }
 
@@ -1013,16 +1197,19 @@ extern "C" int pm_h264_encode_gop(const unsigned char* frames, long long f_fs, i
   PM_REQUIRE(gop >= 1);
   if (gop == 1) return pm_h264_encode(frames, f_fs, n_frames, clip_len, h, w, qp, scratch, slice_cap, slice_bytes,
                                       stream);
-  PM_REQUIRE(shape_ok(n_frames, h, w) && frames && scratch && slice_bytes && recon && f_fs >= 3LL * w * h
-             && clip_len >= 1 && n_frames % clip_len == 0 && gop <= clip_len && qp >= 0 && qp <= 51
+  bool i4;
+  PM_REQUIRE(split_qp(qp, i4) && shape_ok(n_frames, h, w) && frames && scratch && slice_bytes && recon
+             && f_fs >= 3LL * w * h && clip_len >= 1 && n_frames % clip_len == 0 && gop <= clip_len
              && slice_cap >= slice_bound_gop(w) && recon_stride >= 24LL * w);
   const int chains_per_clip = (int)(((long long)clip_len + gop - 1) / gop);
   const long long slices = (long long)(n_frames / clip_len) * chains_per_clip * (h / 16);
   if (slices == 0) return PM_OK;
   PM_REQUIRE(slices / WARPS < 0x7fffffffLL);
-  h264_encode_kernel<GOP_ZERO><<<(unsigned)((slices + WARPS - 1) / WARPS), 32 * WARPS, 0, (cudaStream_t)stream>>>(
-      Job{frames, f_fs, n_frames, clip_len, h, w, qp, scratch, slice_cap, slice_bytes, gop, chains_per_clip, recon,
-          recon_stride});
+  const Job j{frames, f_fs, n_frames, clip_len, h, w, qp, scratch, slice_cap, slice_bytes, gop, chains_per_clip, recon,
+              recon_stride};
+  const unsigned grid = (unsigned)((slices + WARPS - 1) / WARPS);
+  if (i4) h264_encode_kernel<GOP_ZERO, true><<<grid, 32 * WARPS, 0, (cudaStream_t)stream>>>(j);
+  else h264_encode_kernel<GOP_ZERO, false><<<grid, 32 * WARPS, 0, (cudaStream_t)stream>>>(j);
   PM_LAUNCH_CHECK();
 }
 
@@ -1030,8 +1217,9 @@ extern "C" int pm_h264_encode_me(const unsigned char* frames, long long f_fs, in
                                  int w, int qp, unsigned char* scratch, long long slice_cap, int* slice_bytes, int gop,
                                  unsigned char* recon, long long recon_stride, int search, short* mv,
                                  long long mv_len, void* stream) {
-  PM_REQUIRE(shape_ok(n_frames, h, w) && frames && scratch && slice_bytes && recon && mv && f_fs >= 3LL * w * h
-             && clip_len >= 1 && n_frames % clip_len == 0 && gop >= 2 && gop <= clip_len && qp >= 0 && qp <= 51
+  bool i4;
+  PM_REQUIRE(split_qp(qp, i4) && shape_ok(n_frames, h, w) && frames && scratch && slice_bytes && recon && mv
+             && f_fs >= 3LL * w * h && clip_len >= 1 && n_frames % clip_len == 0 && gop >= 2 && gop <= clip_len
              && search >= 1 && search <= MAX_SEARCH && slice_cap >= slice_bound_gop(w) && recon_stride >= 3LL * h * w);
   const int chains_per_clip = (int)(((long long)clip_len + gop - 1) / gop);
   const long long chains = (long long)(n_frames / clip_len) * chains_per_clip, slices = chains * (h / 16);
@@ -1042,9 +1230,11 @@ extern "C" int pm_h264_encode_me(const unsigned char* frames, long long f_fs, in
   Job j{frames, f_fs, n_frames, clip_len, h, w, qp, scratch, slice_cap, slice_bytes, gop, chains_per_clip, recon,
         recon_stride, 0, search, reinterpret_cast<short2*>(mv)};
   const cudaStream_t st = (cudaStream_t)stream;
+  const unsigned grid = (unsigned)((slices + WARPS - 1) / WARPS);
   for (j.k = 0; j.k < gop; ++j.k) {
     if (j.k) h264_search_kernel<<<(unsigned)mbs, SEARCH_THREADS, 0, st>>>(j);
-    h264_encode_kernel<GOP_ME><<<(unsigned)((slices + WARPS - 1) / WARPS), 32 * WARPS, 0, st>>>(j);
+    if (i4) h264_encode_kernel<GOP_ME, true><<<grid, 32 * WARPS, 0, st>>>(j);
+    else h264_encode_kernel<GOP_ME, false><<<grid, 32 * WARPS, 0, st>>>(j);
   }
   PM_LAUNCH_CHECK();
 }

@@ -721,20 +721,27 @@ def png_encode(frames, data, nbytes, row_bits, row_adler):
 # ------------------------------------------------------------------------------------------------------
 
 
-def h264_encode(frames, clip_len, qp, data, nbytes, scratch, sizes, gop=1, recon=None, search=0, mv=None):
+H264_I4X4 = 0x100                         # include/pm_emage.h PM_H264_I4X4: the qp flag that adds Intra 4x4
+
+
+def h264_encode(frames, clip_len, qp, data, nbytes, scratch, sizes, gop=1, recon=None, search=0, mv=None,
+                intra4x4=False):
     """The H.264 samples of frames (N, H, W, 3) uint8, each frame dense, any stride apart, frame i at index i % clip_len
     of its clip, into the slots of data (N, cap) uint8 with their sizes in nbytes (N,) int64 (include/pm_emage.h
     pm_h264_*).  scratch (N, H / 16, slice_cap) uint8 and sizes (N, H / 16) int32: workspace, one slice per row.
     gop: frames per group of pictures, 1 <= gop <= clip_len; gop > 1 needs recon (GOPs, H / 16, >= 24 W) uint8, one macroblock row's
     reconstruction per (GOP, row), written by each GOP's IDR frame before its P frames read it.  search: the motion
     search range in whole pixels, 0..32; search > 0 with gop > 1 runs pm_h264_encode_me and needs recon (GOPs, >= 3 H W)
-    uint8, two whole-frame reconstructions per GOP, and mv (GOPs, H / 16, W / 16, 2) int16, the searched vectors.  The
-    slots are cleared first by a memset (a memset node under graph capture), then the launches."""
+    uint8, two whole-frame reconstructions per GOP, and mv (GOPs, H / 16, W / 16, 2) int16, the searched vectors.
+    intra4x4: add Intra 4x4 macroblocks (qp | PM_H264_I4X4 on every path).  The slots are cleared first by a memset (a
+    memset node under graph capture), then the launches."""
     _chk(frames, torch.uint8), _chk(data, torch.uint8), _chk(nbytes, torch.int64)
     _chk(scratch, torch.uint8), _chk(sizes, torch.int32)
     n, h, w, _ = frames.shape
     assert data.is_contiguous() and nbytes.is_contiguous() and scratch.is_contiguous() and sizes.is_contiguous()
     cap, fs, slice_cap = data.shape[1], frames.stride(0) if n > 1 else 3 * h * w, scratch.shape[2]
+    assert 0 <= qp <= 51
+    qp = qp | H264_I4X4 if intra4x4 else qp
     _lib.call("pm_memset_async", data.data_ptr(), 0, data.numel(), _stream())
     if gop == 1:
         _call("pm_h264_encode", frames.data_ptr(), fs, n, clip_len, h, w, qp, scratch.data_ptr(), slice_cap,

@@ -9,7 +9,10 @@ same sample alone or in any batch at the same index parity.  With a keyframe int
 every gop-th frame is an IDR frame and the frames between are P frames of P_Skip, zero-motion inter, Intra16x16 or
 I_PCM macroblocks, each coded against the frame before it; a GOP's bytes depend only on its frames, qp, gop and the
 parity of its index in the clip.  With a motion search range search > 0 (encode(..., gop=30, search=16)) the inter
-macroblocks carry quarter-pel motion vectors searched against the whole previous frame.
+macroblocks carry quarter-pel motion vectors searched against the whole previous frame.  With intra4x4=True
+(encode(..., intra4x4=True)) any intra macroblock of an I or P slice may also be Intra 4x4 (I_NxN): its 16 4x4 blocks
+each predicted by one of the nine modes from the reconstructed samples next to it, chosen by SAD and mode bits; off,
+the default, every byte is as before.
 
     data, nbytes = video.encode(renderer.render_sequence(poses, expression, trans))   # (B*T, cap) uint8, (B*T,) int64
     video.write_mp4(frames[0], "out/clip.mp4", fps=30)                                 # one silent clip
@@ -86,6 +89,12 @@ def _search(search) -> int:
     return search
 
 
+def _intra4x4(intra4x4) -> bool:
+    if not isinstance(intra4x4, bool):
+        raise ValueError(f"intra4x4 must be a bool, got {intra4x4!r}")
+    return intra4x4
+
+
 def _fps(fps) -> Fraction:
     """The frame rate as the MP4 file states it: timescale / sample duration, a denominator of at most 1001."""
     if isinstance(fps, bool) or not isinstance(fps, (int, float, Fraction)) or not fps > 0:
@@ -156,7 +165,7 @@ def pps() -> bytes:
 # ---- encoding on the GPU ----
 
 @torch.no_grad()
-def encode(frames, qp=20, out=None, gop=1, search=0):
+def encode(frames, qp=20, out=None, gop=1, search=0, intra4x4=False):
     """H.264 samples of frames (N, H, W, 3) or (B, T, H, W, 3) uint8 CUDA, each frame dense (a MeshRenderer result is
     read in place), H and W multiples of 16.  gop: frames per group of pictures.  Frame t of a clip (t, or n for
     (N, ...) input) is an IDR frame with idr_pic_id (t div gop) mod 2 when t mod gop == 0, else a P frame coded
@@ -166,14 +175,16 @@ def encode(frames, qp=20, out=None, gop=1, search=0):
     zero motion; search > 0 gives their inter macroblocks the quarter-pel vector of the lowest SAD + lambda(qp) x
     vector bits within +-search pixels of zero, against the whole previous frame (DESIGN.md section 12).  It trades
     encode time for size and changes no SPS, PPS or MP4 box; with gop 1 (or T = 1) there are no P frames and the
-    output is the gop 1 output.  Returns (data, nbytes): data (N, cap) uint8 holds sample i (its slices, each
+    output is the gop 1 output.  intra4x4: also code intra macroblocks as Intra 4x4 (I_NxN) where its cost
+    J4 + 6 lambda(qp) is below the Intra16x16 SAD (DESIGN.md section 12); the SPS, PPS, MP4 boxes and size bounds are
+    unchanged, and False gives the bytes of the rule without it.  Returns (data, nbytes): data (N, cap) uint8 holds sample i (its slices, each
     prefixed by its 4-byte big-endian length) in data[i, :nbytes[i]] (zeros after it), nbytes (N,) int64, both on the
     frames' device.  out: an optional (data, nbytes) pair to fill, data (N, cap) uint8 contiguous with
     cap >= slot_bytes(H, W, gop) and a multiple of 4, nbytes (N,) int64 contiguous.  No host synchronisation; with
     out given the call can be captured in a CUDA graph.  Raises ValueError on a CPU tensor, a wrong dtype or shape,
     H or W not a multiple of 16, a frame past level 5.1, frames that are not dense, qp outside 0..51, gop not an int
-    >= 1, search not an int in 0..32 or an out too small (cap >= slot_bytes(H, W, gop))."""
-    qp, gop, search = _qp(qp), _gop(gop), _search(search)
+    >= 1, search not an int in 0..32, intra4x4 not a bool or an out too small (cap >= slot_bytes(H, W, gop))."""
+    qp, gop, search, intra4x4 = _qp(qp), _gop(gop), _search(search), _intra4x4(intra4x4)
     frames, clip_len = slots.frames(frames)
     n, h, w, _ = frames.shape
     check_size(h, w)
@@ -186,16 +197,17 @@ def encode(frames, qp=20, out=None, gop=1, search=0):
     # a gop past the clip length gives the gop = T bytes (the same idr_pic_id and frame_num); the kernel takes at most T
     kgop = min(gop, clip_len)
     recon = None
+    i4 = {"intra4x4": True} if intra4x4 else {}         # without the switch the call is exactly as before
     chains = n // clip_len * -(-clip_len // kgop)
     if kgop > 1 and search > 0:           # two whole-frame reconstructions per GOP, and frame k's vectors
         recon = torch.empty(chains, 3 * h * w, dtype=torch.uint8, device=dev)
         mv = torch.empty(chains, h // 16, w // 16, 2, dtype=torch.int16, device=dev)
         ops.h264_encode(frames, clip_len, qp, data, nbytes, scratch, sizes, gop=kgop, recon=recon, search=search,
-                        mv=mv)
+                        mv=mv, **i4)
         return data, nbytes
     if kgop > 1:                          # one macroblock row's reconstruction per (GOP, row), updated frame by frame
         recon = torch.empty(chains, h // 16, RECON_ROW_BYTES * w, dtype=torch.uint8, device=dev)
-    ops.h264_encode(frames, clip_len, qp, data, nbytes, scratch, sizes, gop=kgop, recon=recon)
+    ops.h264_encode(frames, clip_len, qp, data, nbytes, scratch, sizes, gop=kgop, recon=recon, **i4)
     return data, nbytes
 
 
@@ -330,9 +342,9 @@ def mp4_bytes(samples, h: int, w: int, fps=30, audio=None, gop=1) -> bytes:
     return ftyp + moov(head) + struct.pack(">I", 8 + total - head) + b"mdat" + body
 
 
-def write_mp4(frames, path, fps=30, qp=20, audio=None, gop=1, search=0):
-    """Encode one clip (T, H, W, 3) uint8 CUDA frames with keyframe interval gop and motion search range search
-    (encode) and write it to path as an MP4 file.  audio: None (one silent video track), or (pcm, rate): pcm (n, C) CUDA int16 or int32 (24-bit) samples
+def write_mp4(frames, path, fps=30, qp=20, audio=None, gop=1, search=0, intra4x4=False):
+    """Encode one clip (T, H, W, 3) uint8 CUDA frames with keyframe interval gop, motion search range search and the
+    Intra 4x4 switch intra4x4 (encode) and write it to path as an MP4 file.  audio: None (one silent video track), or (pcm, rate): pcm (n, C) CUDA int16 or int32 (24-bit) samples
     at rate Hz, coded as a FLAC track (flac.encode) and trimmed to the video's duration: the first
     min(n, floor(T rate / fps)) samples.  That matches ffmpeg's -shortest when the audio is the longer stream; shorter
     audio is kept whole, and the video plays on past its end in silence.  Both streams are encoded on the current
@@ -341,7 +353,7 @@ def write_mp4(frames, path, fps=30, qp=20, audio=None, gop=1, search=0):
     if torch.is_tensor(frames) and frames.dim() != 4:
         raise ValueError(f"write_mp4 takes one clip (T, H, W, 3), got {tuple(frames.shape)}")
     frame_rate = _fps(fps)
-    gop, search = _gop(gop), _search(search)
+    gop, search, intra4x4 = _gop(gop), _search(search), _intra4x4(intra4x4)
     if audio is not None:
         pcm, rate = audio
         flac._rate(rate)
@@ -351,7 +363,7 @@ def write_mp4(frames, path, fps=30, qp=20, audio=None, gop=1, search=0):
         if keep < 1:
             raise ValueError(f"write_mp4: {frames.shape[0]} frames at {fps} fps hold no sample at {rate} Hz")
         pcm = pcm[:keep]
-    data, nbytes = encode(frames, qp=qp, gop=gop, search=search)
+    data, nbytes = encode(frames, qp=qp, gop=gop, search=search, intra4x4=intra4x4)
     h, w = frames.shape[1:3]
     if audio is None:
         (pieces,) = slots.to_host((data, nbytes.tolist()))

@@ -3,7 +3,7 @@
 
     python tools/bench_video.py OUT.json [--reps 5] [--stage-reps 3] [--psnr-frames 30] [--no-mb-types] [--gop-only]
                                          [--baseline-lib PARENT/pantomatrix_b200/libpm_emage.so]
-                                         [--me-only [--me-mb-frames 4]]
+                                         [--me-only [--me-mb-frames 4]] [--i4-only [--i4-mb-frames 2]]
 
 Inputs: the frames tools/bench_png.py uses: render_sequence of EMAGE generate() output (synthetic weights, full-size
 synthetic surface model), 1 x 300 and 8 x 300 frames of 960 x 720, and render_body(upsample=2) of CaMN forward()
@@ -30,6 +30,12 @@ first --psnr-frames frames, and the time of one call's search and code kernels f
 EMAGE clip also the macroblock shares over the first --me-mb-frames frames of the first GOP at gop 30, with P split
 into zero and non-zero vectors, counted by the CPU restatement (tests/h264_me_ref.py; the whole 30-frame GOP takes it
 too long at 960 x 720); and the output stage (render + write_mp4) at gop 30 with search 0 against search 16.
+Intra 4x4 arms (--i4-only runs only these): gop 1 and 30, search 0 and 16 (gop 30), qp 20 and 26, each with and
+without intra4x4, per input (the EMAGE 1 x 300 and CaMN 1 x 270 clips), all alternating in the timed loop: the
+video.encode call (median ms), bytes per frame (min, mean, max) and luma PSNR of the first --psnr-frames frames; for
+the EMAGE clip also, from the CPU restatement (tests/h264_i4_ref.py) over its first --i4-mb-frames frames at gop 30
+and search 0, the macroblock shares, the histogram of the nine modes, and the bytes for several values of the rule's
+constant c.
 The card's name, power limit and max SM clock are read in the same run.  Nothing is written except OUT."""
 import ctypes
 import argparse
@@ -57,6 +63,7 @@ from synthetic_models import build_lstm_product, build_product, smplx_surface_ar
 
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 import h264_gop_ref  # noqa: E402
+import h264_i4_ref  # noqa: E402
 import h264_me_ref  # noqa: E402
 
 QP = 20
@@ -293,8 +300,8 @@ def me_arms(frames, reps, psnr_frames, mb_frames, tmp):
     return out
 
 
-def _first_samples(clip, gop, search):
-    data, nbytes = video.encode(clip, qp=QP, gop=gop, search=search)
+def _first_samples(clip, gop, search, qp=QP, intra4x4=False):
+    data, nbytes = video.encode(clip, qp=qp, gop=gop, search=search, intra4x4=intra4x4)
     return [data[i, :k].cpu().numpy().tobytes() for i, k in enumerate(nbytes.tolist())]
 
 
@@ -335,6 +342,62 @@ def run_me(args, r, pred, res, tmp):
     del frames
     res["output_stage_me_1x300"] = output_stage_me(r, pred, args.stage_reps)
     print("output stage me", json.dumps(res["output_stage_me_1x300"]), flush=True)
+
+
+def i4_arms(frames, reps, psnr_frames, mb_frames, tmp):
+    """gop 1 / 30, search 0 / 16, qp 20 / 26, intra4x4 off / on, alternating in the timed loop: encode ms, bytes per
+    frame, luma PSNR; with mb_frames, the restatement's macroblock shares, mode histogram and c sweep."""
+    arms = [(g, s, q, i4) for g, s in ((1, 0), (30, 0), (30, 16)) for q in (20, 26) for i4 in (False, True)]
+    ms = {a: [] for a in arms}
+    for g, s, q, i4 in arms:
+        video.encode(frames, qp=q, gop=g, search=s, intra4x4=i4)   # warm-up
+    torch.cuda.synchronize()
+    for _ in range(reps):
+        for g, s, q, i4 in arms:
+            ms[(g, s, q, i4)].append(event_ms(lambda: video.encode(frames, qp=q, gop=g, search=s, intra4x4=i4)))
+    out = {}
+    clip = frames[0] if frames.dim() == 5 else frames
+    for g, s, q, i4 in arms:
+        sizes = video.encode(frames, qp=q, gop=g, search=s, intra4x4=i4)[1].cpu().numpy()
+        path = video.write_mp4(clip, os.path.join(tmp, f"g{g}s{s}q{q}i{int(i4)}.mp4"), fps=30, qp=q, gop=g, search=s,
+                               intra4x4=i4)
+        psnr_mean, psnr_min = luma_psnr(clip, path, psnr_frames)
+        a = out[f"gop{g}_search{s}_qp{q}_i4{int(i4)}"] = {
+            "encode_ms_median": statistics.median(ms[(g, s, q, i4)]), "encode_ms_all": ms[(g, s, q, i4)],
+            "bytes_per_frame_mean": float(sizes.mean()), "bytes_per_frame_min": int(sizes.min()),
+            "bytes_per_frame_max": int(sizes.max()), "luma_psnr_db_mean": psnr_mean, "luma_psnr_db_min": psnr_min}
+        print("  arm", g, s, q, i4, json.dumps({k: v for k, v in a.items() if k != "encode_ms_all"}), flush=True)
+    if mb_frames:
+        host = list(clip[:mb_frames].cpu().numpy())
+        for q in (20, 26):
+            enc = h264_i4_ref.encode_clip(host, q, 30, 0)
+            assert [e[0] for e in enc] == [bytes(x) for x in _first_samples(clip[:mb_frames], 30, 0, q, True)]
+            types = np.concatenate([e[2].reshape(-1) for e in enc])
+            modes = np.concatenate([e[3][e[2] == "I4"].reshape(-1) for e in enc])
+            sweep = {}
+            for c in (0, 3, 6, 12, 24):
+                sweep[c] = [len(e[0]) for e in h264_i4_ref.encode_clip(host, q, 30, 0, c=c)]
+            out[f"restatement_qp{q}"] = {
+                "frames": mb_frames, "c": h264_i4_ref.C_I4,
+                "mb_share": {k: float((types == k).mean()) for k in ("SKIP", "P", "DC", "H", "I4", "PCM")},
+                "mode_histogram": np.bincount(modes, minlength=9).tolist(),
+                "bytes_by_c": sweep, "bytes_without_i4": [len(e[0]) for e in h264_me_ref.encode_clip(host, q, 30, 0)]}
+            print("  restatement", q, json.dumps(out[f"restatement_qp{q}"]), flush=True)
+    return out
+
+
+def run_i4(args, r, pred, res, tmp):
+    frames = r.render_sequence(*(pred[k][:1] for k in ("motion_axis_angle", "expression", "trans")))
+    print("i4 emage", flush=True)
+    res["i4_emage_sequence_1x300"] = i4_arms(frames, args.reps, args.psnr_frames, args.i4_mb_frames, tmp)
+    del frames
+    camn = build_lstm_product("camn", device="cuda")
+    poses = camn(torch.from_numpy(synth_audio(1, 160000, 5)).cuda(),
+                 torch.zeros(1, 1, dtype=torch.long, device="cuda"))["motion_axis_angle"]
+    poses = poses.reshape(1, poses.shape[1], 165)
+    frames = r.render_body(poses, torch.zeros(1, poses.shape[1], 3, device="cuda"), upsample=2)
+    print("i4 camn", flush=True)
+    res["i4_camn_body_1x10s"] = i4_arms(frames, args.reps, args.psnr_frames, 0, tmp)
 
 
 def output_stage(r, pred, reps):
@@ -420,6 +483,8 @@ def main():
     ap.add_argument("--gop-only", action="store_true", help="only the GOP arms and the gop output stage")
     ap.add_argument("--me-only", action="store_true", help="only the motion search arms and their output stage")
     ap.add_argument("--me-mb-frames", type=int, default=4, help="frames the restatement counts macroblocks over")
+    ap.add_argument("--i4-only", action="store_true", help="only the Intra 4x4 arms")
+    ap.add_argument("--i4-mb-frames", type=int, default=2, help="frames the Intra 4x4 restatement counts over")
     args = ap.parse_args()
     assert torch.cuda.is_available(), "the video benchmark measures the GPU: no CUDA device found"
     torch.cuda.set_device(0)
@@ -429,7 +494,7 @@ def main():
     res = {"card": card()}
     tmp = tempfile.mkdtemp()
     try:
-        (run_me if args.me_only else run)(args, r, pred, res, tmp)
+        (run_i4 if args.i4_only else run_me if args.me_only else run)(args, r, pred, res, tmp)
     finally:
         shutil.rmtree(tmp, ignore_errors=True)
     res["card_after"] = card()
