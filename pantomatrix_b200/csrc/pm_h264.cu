@@ -11,8 +11,8 @@
 //   pm_h264_gather  one CTA per (frame, row): the slice's offset in the frame's sample, the copy, the frame's size.
 // A warp stages its bits in shared memory in stream byte order (pm_put_bits, as FLAC writes its slots), so whole
 // bytes leave the staging buffer as byte loads.
-// CPU restatement: oracle/h264_oracle.py, tests/h264_gop_ref.py for P frames, tests/h264_me_ref.py for motion,
-// tests/h264_i4_ref.py for Intra 4x4.  Every byte depends only on the frame (its GOP's frames), qp, gop, search, the
+// CPU restatement: oracle/h264_oracle.py for the intra rule, tests/h264_ref.py for P frames, motion and Intra 4x4.
+// Every byte depends only on the frame (its GOP's frames), qp, gop, search, the
 // Intra 4x4 switch and the parity of its index (t div gop).
 #include <cub/block/block_reduce.cuh>
 

@@ -1,4 +1,4 @@
-"""The H.264 GOP rule on the CPU (tests/h264_gop_ref.py, DESIGN.md section 12): clips of IDR and P frames decode with
+"""The H.264 GOP rule on the CPU (tests/h264_ref.py, DESIGN.md section 12): clips of IDR and P frames decode with
 OpenCV's FFmpeg to the restatement's reconstruction; gop 1 is the intra rule; the gop > 1 bound, SPS and stss box; and
 the ops wrapper's ctypes arguments for pm_h264_encode_gop.  The GPU's bytes are compared with these in
 tests/test_video_gop_gpu.py."""
@@ -10,7 +10,7 @@ import numpy as np
 import pytest
 import torch
 
-import h264_gop_ref as G
+import h264_ref as R
 from oracle import h264_oracle as O
 from pantomatrix_b200 import video
 from test_video import _boxes, _grad, decode
@@ -67,7 +67,30 @@ def gop_of(g, t):
 @functools.lru_cache(maxsize=None)
 def encoded(name, g):
     frames, qp = {c[0]: (c[1], c[2]) for c in gop_cases()}[name]
-    return G.encode_clip(frames, qp, gop_of(g, len(frames)))
+    return R.encode_clip(frames, qp, gop_of(g, len(frames)))
+
+
+@functools.lru_cache(maxsize=None)
+def every_qp(qp):
+    """The two-frame clip of test_every_qp_decodes_to_the_reconstruction at qp, gop 2."""
+    rng = np.random.default_rng(5)
+    a = rng.integers(0, 256, (32, 32, 3), dtype=np.uint8)
+    a[:16] = _grad(16, 32)
+    b = a.copy()
+    b[4:20, 6:30] = np.clip(b[4:20, 6:30].astype(int) + rng.integers(-12, 13, (16, 24, 3)), 0, 255)
+    return R.encode_clip([a, b], qp, 2)
+
+
+@functools.lru_cache(maxsize=None)
+def noise_bound(qp):
+    """The noise clip of test_bound_holds_on_noise_for_gop_above_1 at qp 0 or 51, gop 3."""
+    rng = np.random.default_rng(3)
+    for q in (0, 51):
+        a = rng.integers(0, 256, (48, 64, 3), dtype=np.uint8)
+        frames = [a, np.clip(a.astype(int) + rng.integers(-6, 7, a.shape), 0, 255).astype(np.uint8),
+                  rng.integers(0, 256, (48, 64, 3), dtype=np.uint8)]
+        if q == qp:
+            return R.encode_clip(frames, qp, 3)
 
 
 def check_clip(enc, h, w, gop, tmp_path, fps=30):
@@ -105,7 +128,7 @@ def test_every_macroblock_type_occurs():
     for name, _, _ in gop_cases():
         for e in encoded(name, 3):
             seen |= set(e[2].reshape(-1))
-    assert seen == {G.SKIP, G.INTER, "DC", "H", O.PCM}
+    assert seen == {R.SKIP, R.INTER, "DC", "H", O.PCM}
     # P frames of the noise clip at qp 0 hold I_PCM macroblocks
     assert any((e[2] == O.PCM).any() for e in encoded("noise_qp0", 3)[1:3])
 
@@ -114,13 +137,13 @@ def test_static_p_slices_are_a_header_and_one_skip_run():
     frames, qp = gop_cases()[0][1:]
     h, w, _ = frames[0].shape
     for e in encoded("static", 7)[1:]:
-        assert (e[2] == G.SKIP).all()
+        assert (e[2] == R.SKIP).all()
         ry = encoded("static", 7)[0][1]
         assert all(np.array_equal(a, b) for a, b in zip(e[1], ry))
     for t, e in enumerate(encoded("static", 7)[1:], 1):
         want = bytearray()
         for my in range(h // 16):
-            b = G.p_slice_header(my * (w // 16), t, qp)
+            b = R.p_slice_header(my * (w // 16), t, qp)
             b.ue(w // 16)
             b.trailing()
             nal = O.emulation_prevent(b.tobytes())
@@ -142,46 +165,37 @@ def test_p_slices_use_level_escapes_at_qp0():
 
     O.Bits.put = spy
     try:
-        _, _, types = G.encode_p(frames[1], ref, 0, 1)
+        types = R.encode_frame(frames[1], ref, 0, 1, 2).types
     finally:
         O.Bits.put = orig
-    assert (types == G.INTER).any() and seen
+    assert (types == R.INTER).any() and seen
 
 
 def test_every_qp_decodes_to_the_reconstruction(tmp_path):
-    rng = np.random.default_rng(5)
-    a = rng.integers(0, 256, (32, 32, 3), dtype=np.uint8)
-    a[:16] = _grad(16, 32)
-    b = a.copy()
-    b[4:20, 6:30] = np.clip(b[4:20, 6:30].astype(int) + rng.integers(-12, 13, (16, 24, 3)), 0, 255)
     for qp in range(52):
-        check_clip(G.encode_clip([a, b], qp, 2), 32, 32, 2, tmp_path)
+        check_clip(every_qp(qp), 32, 32, 2, tmp_path)
 
 
 def test_gop_1_is_the_intra_rule():
     for name, frames, qp in gop_cases()[:4]:
-        for t, e in enumerate(G.encode_clip(frames, qp, 1)):
+        for t, e in enumerate(R.encode_clip(frames, qp, 1)):
             want = O.encode(frames[t], qp, t)
             assert e[0] == want[0] and (e[2] == want[2]).all()
     # idr_pic_id = (t div gop) mod 2
     sq = gop_cases()[1][1]
-    enc = G.encode_clip(sq, 20, 2)
+    enc = R.encode_clip(sq, 20, 2)
     for t in (0, 2, 4):
         assert enc[t][0] == O.encode(sq[t], 20, t // 2)[0]
 
 
 def test_bound_holds_on_noise_for_gop_above_1():
-    rng = np.random.default_rng(3)
     for h, w in ((16, 16), (32, 96), (720, 960), (720, 480), (16 * 543, 16 * 64)):
         assert video.max_bytes(h, w) == O.max_bytes(h, w)
         for gop in (2, 30):
-            assert video.max_bytes(h, w, gop) == G.max_bytes(h, w, gop) > video.max_bytes(h, w)
+            assert video.max_bytes(h, w, gop) == R.max_bytes(h, w, gop) > video.max_bytes(h, w)
             assert video.slot_bytes(h, w, gop) % 4 == 0 and video.slot_bytes(h, w, gop) - video.max_bytes(h, w, gop) < 4
     for qp in (0, 51):
-        a = rng.integers(0, 256, (48, 64, 3), dtype=np.uint8)
-        frames = [a, np.clip(a.astype(int) + rng.integers(-6, 7, a.shape), 0, 255).astype(np.uint8),
-                  rng.integers(0, 256, (48, 64, 3), dtype=np.uint8)]
-        for e in G.encode_clip(frames, qp, 3):
+        for e in noise_bound(qp):
             assert len(e[0]) <= video.max_bytes(48, 64, 3)
 
 
@@ -195,7 +209,7 @@ def test_sps_differs_only_in_max_num_ref_frames():
     for h, w in ((16, 16), (720, 960), (720, 480), (16 * 543, 16 * 64)):
         one, many = _rbsp_bits(video.sps(h, w)), _rbsp_bits(video.sps(h, w, 30))
         assert video.sps(h, w, 1) == video.sps(h, w) == O.sps(h, w)
-        assert video.sps(h, w, 2) == video.sps(h, w, 30) == G.sps(h, w, 7)
+        assert video.sps(h, w, 2) == video.sps(h, w, 30) == R.sps(h, w, 7)
         # bits 32..36: seq_parameter_set_id, log2_max_frame_num_minus4, pic_order_cnt_type 2; then ue(0) -> ue(1)
         assert one[32:38] == "110111" and many[:37] + many[40:] == one[:37] + one[38:] and many[37:40] == "010"
 

@@ -1,5 +1,5 @@
 """H.264 GOP encoding on the H100 (pantomatrix_b200/video.py, gop > 1): the samples are byte for byte the CPU
-restatement's (tests/h264_gop_ref.py) on the CPU cases, every qp, random clips and rendered EMAGE and CaMN GOPs at qp 0,
+restatement's (tests/h264_ref.py) on the CPU cases, every qp, random clips and rendered EMAGE and CaMN GOPs at qp 0,
 20 and 51; each GOP encodes as it does alone at the same parity in (B, T, ...) and (N, ...) batches; calls are
 deterministic and capture in a CUDA graph; pm_h264_encode_gop at gop 1 is pm_h264_encode; a 300-frame gop 30
 write_mp4 file decodes to the restatement's reconstruction; bad gop values raise ValueError."""
@@ -7,7 +7,7 @@ import numpy as np
 import pytest
 import torch
 
-import h264_gop_ref as G
+import h264_ref as R
 from oracle.weights import synth_audio
 from pantomatrix_b200 import _lib, ops, video
 from pantomatrix_b200.body_model import SmplxBodyModel
@@ -51,7 +51,7 @@ def rendered_gop():
 def test_gop_cases_are_byte_identical_to_the_restatement(name, frames, qp, g):
     gop = gop_of(g, len(frames))
     got = samples(torch.as_tensor(np.stack(frames), device=DEV), qp, gop)
-    assert got == [e[0] for e in G.encode_clip(frames, qp, gop)]
+    assert got == [e[0] for e in R.encode_clip(frames, qp, gop)]
 
 
 def test_every_qp_is_byte_identical_to_the_restatement():
@@ -62,7 +62,7 @@ def test_every_qp_is_byte_identical_to_the_restatement():
     b[4:20, 6:30] = np.clip(b[4:20, 6:30].astype(int) + rng.integers(-12, 13, (16, 24, 3)), 0, 255)
     t = torch.as_tensor(np.stack([a, b]), device=DEV)
     for qp in range(52):
-        assert samples(t, qp, 2) == [e[0] for e in G.encode_clip([a, b], qp, 2)], qp
+        assert samples(t, qp, 2) == [e[0] for e in R.encode_clip([a, b], qp, 2)], qp
 
 
 def test_random_clips_are_byte_identical_to_the_restatement():
@@ -79,7 +79,7 @@ def test_random_clips_are_byte_identical_to_the_restatement():
             clip.append(f)
         for qp, gop in ((0, 3), (12, 4), (30, 6), (45, 2)):
             got = samples(torch.as_tensor(np.stack(clip), device=DEV), qp, gop)
-            want = G.encode_clip(clip, qp, gop)
+            want = R.encode_clip(clip, qp, gop)
             for i, (b, e) in enumerate(zip(got, want)):
                 assert b == e[0], (h, w, qp, gop, i)
                 assert len(b) <= video.max_bytes(h, w, gop)
@@ -90,7 +90,7 @@ def test_rendered_gops_are_byte_identical_to_the_restatement(rendered_gop, qp):
     emage, body = rendered_gop
     for clip, gop in ((emage[0, :10], 5), (body[1], 10)):
         got = samples(clip, qp, gop)
-        assert got == [e[0] for e in G.encode_clip(list(clip.cpu().numpy()), qp, gop)], qp
+        assert got == [e[0] for e in R.encode_clip(list(clip.cpu().numpy()), qp, gop)], qp
 
 
 def test_batch_encodes_each_gop_as_alone_at_the_same_parity(rendered_gop):
@@ -151,7 +151,7 @@ def test_write_mp4_gop_30_of_a_300_frame_render_decodes_to_the_reconstruction(re
     assert len(lumas) == 300 and fps == 30
     host = emage[0].cpu().numpy()
     for t0 in (0, 270):
-        for i, e in enumerate(G.encode_clip(list(host[t0:t0 + 3]), 20, 30)):
+        for i, e in enumerate(R.encode_clip(list(host[t0:t0 + 3]), 20, 30)):
             assert np.array_equal(lumas[t0 + i].reshape(-1)[:720 * 960].reshape(720, 960), e[1][0]), t0 + i
 
 

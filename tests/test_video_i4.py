@@ -1,18 +1,19 @@
-"""The H.264 Intra 4x4 rule on the CPU (tests/h264_i4_ref.py, DESIGN.md section 12): clips coded with intra4x4 decode
+"""The H.264 Intra 4x4 rule on the CPU (tests/h264_ref.py, DESIGN.md section 12): clips coded with intra4x4 decode
 with OpenCV's FFmpeg to the restatement's reconstruction, which anchors the nine prediction modes, the sample
 availability, the mode prediction, the Intra cbp mapping and nC beside every neighbour type; every mode, both
 prev_intra4x4_pred_mode_flag values, both intra macroblock types and I_NxN in P slices occur; bad intra4x4 values; and
 the ops wrapper's ctypes arguments.  The GPU's bytes are compared with these in tests/test_video_i4_gpu.py."""
 import ctypes
 import functools
+import hashlib
+import json
+import os
 
 import numpy as np
 import pytest
 import torch
 
-import h264_gop_ref as G
-import h264_i4_ref as I
-import h264_me_ref as M
+import h264_ref as R
 from oracle import h264_oracle as O
 from pantomatrix_b200 import video
 from test_video_gop import check_clip
@@ -80,7 +81,16 @@ def case(name):
 @functools.lru_cache(maxsize=None)
 def encoded(name, g):
     frames, qp, rng = case(name)
-    return I.encode_clip(frames, qp, gop_of(g, len(frames)), rng)
+    return R.encode_clip(frames, qp, gop_of(g, len(frames)), rng, True)
+
+
+@functools.lru_cache(maxsize=None)
+def noise_bound(gop):
+    """The clip of test_bound_holds_on_noise_at_qp_0 at gop 1 or 3."""
+    rng = np.random.default_rng(8)
+    frames = [rng.integers(0, 256, (32, 64, 3), dtype=np.uint8) for _ in range(3)]
+    frames[1][:, :32] = stripes(32, 32, 0.5, 4)
+    return R.encode_clip(frames, 0, gop, 0, True)
 
 
 @pytest.mark.parametrize("g", GOPS, ids=[str(g) for g in GOPS])
@@ -99,20 +109,20 @@ def test_every_mode_flag_and_macroblock_type_occurs():
     modes, flags, types, p_i4 = set(), set(), set(), False
     for e in _all():
         types |= set(e[2].reshape(-1))
-        m = e[3][e[2] == I.I4]
+        m = e.modes[e[2] == R.I4]
         modes |= set(m.reshape(-1).tolist())
-        p_i4 |= e[4] is not None and bool((e[2] == I.I4).any())
-        for my, mx in zip(*np.nonzero(e[2] == I.I4)):
-            lm = e[3][my, mx - 1] if mx and e[2][my, mx - 1] == I.I4 else np.full((4, 4), 2)
-            for by, bx in G.LUMA_BLK:
+        p_i4 |= e.mv is not None and bool((e[2] == R.I4).any())
+        for my, mx in zip(*np.nonzero(e[2] == R.I4)):
+            lm = e.modes[my, mx - 1] if mx and e[2][my, mx - 1] == R.I4 else np.full((4, 4), 2)
+            for by, bx in R.LUMA_BLK:
                 if by == 0 or (bx == 0 and mx == 0):
                     pm = 2
                 else:
-                    pm = min(e[3][my, mx, by, bx - 1] if bx else lm[by, 3], e[3][my, mx, by - 1, bx])
-                flags.add(bool(e[3][my, mx, by, bx] == pm))
+                    pm = min(e.modes[my, mx, by, bx - 1] if bx else lm[by, 3], e.modes[my, mx, by - 1, bx])
+                flags.add(bool(e.modes[my, mx, by, bx] == pm))
     assert modes == set(range(9)), sorted(modes)
     assert flags == {True, False}
-    assert {"DC", "H", I.I4, O.PCM, G.SKIP, G.INTER} <= types, types
+    assert {"DC", "H", R.I4, O.PCM, R.SKIP, R.INTER} <= types, types
     assert p_i4
 
 
@@ -120,32 +130,34 @@ def test_i_nxn_sits_right_of_every_macroblock_type():
     left = set()
     for e in _all():
         t = e[2]
-        left |= {t[my, mx - 1] for my, mx in zip(*np.nonzero(t == I.I4)) if mx}
-    assert {G.SKIP, G.INTER, I.I4, O.PCM} <= left and left & {"DC", "H"}, left     # DC, H: Intra16x16
+        left |= {t[my, mx - 1] for my, mx in zip(*np.nonzero(t == R.I4)) if mx}
+    assert {R.SKIP, R.INTER, R.I4, O.PCM} <= left and left & {"DC", "H"}, left     # DC, H: Intra16x16
 
 
-@pytest.mark.parametrize("name", [c[0] for c in i4_cases() if M.LAMBDA[c[2]] > 0])   # lambda 0: c lambda is 0
+@pytest.mark.parametrize("name", [c[0] for c in i4_cases() if R.LAMBDA[c[2]] > 0])   # lambda 0: c lambda is 0
 def test_a_constant_past_every_cost_is_the_rule_without_intra4x4(name):
+    """At gop > 1 the rule without intra4x4 is the candidate never computed, and the bytes the motion search rule's own
+    restatement coded, pinned by their digests."""
     frames, qp, rng = case(name)
+    with open(os.path.join(os.path.dirname(__file__), "golden", "h264_ref_digests.json")) as f:
+        pinned = json.load(f)["without_i4"]
     for gop in (1, 2, len(frames)):
-        off = [e[0] for e in I.encode_clip(frames, qp, gop, rng, c=1 << 40)]
+        off = [e[0] for e in R.encode_clip(frames, qp, gop, rng, True, c=1 << 40)]
         if gop == 1:
             assert off == [O.encode(f, qp, t)[0] for t, f in enumerate(frames)]
         else:
-            assert off == [e[0] for e in M.encode_clip(frames, qp, gop, rng)]
+            assert off == [e[0] for e in R.encode_clip(frames, qp, gop, rng, False)]
+            assert [hashlib.sha256(b).hexdigest() for b in off] == pinned[f"{name}/{gop}"]
 
 
 def test_intra_cbp_table_is_a_permutation():
-    assert sorted(I.INTRA_CBP) == list(range(48))
-    assert I.INTRA_CBP[:4] == [47, 31, 15, 0] and I.INTRA_CBP[-1] == 41
+    assert sorted(R.INTRA_CBP) == list(range(48))
+    assert R.INTRA_CBP[:4] == [47, 31, 15, 0] and R.INTRA_CBP[-1] == 41
 
 
 def test_bound_holds_on_noise_at_qp_0():
-    rng = np.random.default_rng(8)
-    frames = [rng.integers(0, 256, (32, 64, 3), dtype=np.uint8) for _ in range(3)]
-    frames[1][:, :32] = stripes(32, 32, 0.5, 4)
     for gop in (1, 3):
-        for e in I.encode_clip(frames, 0, gop, 0):
+        for e in noise_bound(gop):
             assert len(e[0]) <= video.max_bytes(32, 64, gop)
 
 

@@ -1,5 +1,5 @@
 """H.264 Intra 4x4 on the H100 (pantomatrix_b200/video.py, intra4x4=True): the samples are byte for byte the CPU
-restatement's (tests/h264_i4_ref.py) on the CPU cases, random clips and the first frames of rendered EMAGE and CaMN
+restatement's (tests/h264_ref.py) on the CPU cases, random clips and the first frames of rendered EMAGE and CaMN
 clips at qp 0, 20 and 51, through all three kernels (gop 1, gop > 1 with search 0, search > 0); each GOP encodes as it
 does alone at the same parity; calls are deterministic and capture in a CUDA graph; a 300-frame gop 30 write_mp4 file
 decodes to the restatement's reconstruction."""
@@ -7,7 +7,7 @@ import numpy as np
 import pytest
 import torch
 
-import h264_i4_ref as I
+import h264_ref as R
 from test_video import decode
 from test_video_gop_gpu import rendered_gop  # noqa: F401  (the module fixture)
 from test_video_i4 import GOPS, gop_of, i4_cases
@@ -29,7 +29,7 @@ def _samples(frames, qp, gop, search, intra4x4=True):
 def test_i4_cases_are_byte_identical_to_the_restatement(name, frames, qp, search, g):
     gop = gop_of(g, len(frames))
     got = _samples(torch.as_tensor(np.stack(frames), device=DEV), qp, gop, search)
-    assert got == [e[0] for e in I.encode_clip(frames, qp, gop, search)]
+    assert got == [e[0] for e in R.encode_clip(frames, qp, gop, search, True)]
 
 
 def test_random_clips_are_byte_identical_to_the_restatement():
@@ -45,7 +45,7 @@ def test_random_clips_are_byte_identical_to_the_restatement():
             clip.append(f)
         for qp, gop, search in ((0, 1, 0), (12, 3, 0), (30, 4, 7), (45, 2, 16)):
             got = _samples(torch.as_tensor(np.stack(clip), device=DEV), qp, gop, search)
-            want = I.encode_clip(clip, qp, gop, search)
+            want = R.encode_clip(clip, qp, gop, search, True)
             for i, (b, e) in enumerate(zip(got, want)):
                 assert b == e[0], (h, w, qp, gop, search, i)
                 assert len(b) <= video.max_bytes(h, w, gop)
@@ -57,7 +57,7 @@ def test_rendered_clips_are_byte_identical_to_the_restatement(rendered_gop, qp):
     for clip, gop, search in ((emage[0, :1], 1, 0), (emage[0, :3], 3, 0), (emage[0, :3], 3, 16),
                               (body[1, :1], 1, 0), (body[1, :3], 3, 0), (body[1, :3], 3, 16)):
         got = _samples(clip, qp, gop, search)
-        assert got == [e[0] for e in I.encode_clip(list(clip.cpu().numpy()), qp, gop, search)], (qp, gop, search)
+        assert got == [e[0] for e in R.encode_clip(list(clip.cpu().numpy()), qp, gop, search, True)], (qp, gop, search)
 
 
 @pytest.mark.parametrize("search", [0, 16])
@@ -101,5 +101,5 @@ def test_write_mp4_gop_30_intra4x4_of_a_300_frame_render_decodes_to_the_reconstr
     assert len(lumas) == 300 and fps == 30
     host = emage[0].cpu().numpy()
     for t0 in (0, 270):
-        for i, e in enumerate(I.encode_clip(list(host[t0:t0 + 3]), 20, 30, 0)):
+        for i, e in enumerate(R.encode_clip(list(host[t0:t0 + 3]), 20, 30, 0, True)):
             assert np.array_equal(lumas[t0 + i].reshape(-1)[:720 * 960].reshape(720, 960), e[1][0]), t0 + i

@@ -1,17 +1,20 @@
-"""The H.264 motion search rule on the CPU (tests/h264_me_ref.py, DESIGN.md section 12): clips coded with quarter-pel
+"""The H.264 motion search rule on the CPU (tests/h264_ref.py, DESIGN.md section 12): clips coded with quarter-pel
 motion decode with OpenCV's FFmpeg to the restatement's reconstruction, which anchors the interpolation and the vector
-predictor; translating clips get their true displacement; search 0 is the zero-motion rule; lambda(qp); the bound;
+predictor; translating clips get their true displacement; search 0 is the zero-motion rule (the bytes pinned in
+tests/golden/h264_ref_digests.json); lambda(qp); the bound;
 bad search values; and the ops wrapper's ctypes arguments for pm_h264_encode_me.  The GPU's bytes are compared with
 these in tests/test_video_me_gpu.py."""
 import ctypes
 import functools
+import hashlib
+import json
+import os
 
 import numpy as np
 import pytest
 import torch
 
-import h264_gop_ref as G
-import h264_me_ref as M
+import h264_ref as R
 from oracle import h264_oracle as O
 from pantomatrix_b200 import video
 from test_video_gop import check_clip
@@ -87,7 +90,17 @@ def case(name):
 @functools.lru_cache(maxsize=None)
 def encoded(name, g):
     frames, qp, rng, _ = case(name)
-    return M.encode_clip(frames, qp, gop_of(g, len(frames)), rng)
+    return R.encode_clip(frames, qp, gop_of(g, len(frames)), rng)
+
+
+@functools.lru_cache(maxsize=None)
+def noise_bound():
+    """The clip of test_bound_holds_on_noise_at_search_32_and_qp_0: gop 4, search 32, qp 0."""
+    rng = np.random.default_rng(4)
+    a = rng.integers(0, 256, (48, 64, 3), dtype=np.uint8)
+    frames = [a, np.roll(a, (3, -5), (0, 1)), np.clip(a.astype(int) + rng.integers(-30, 31, a.shape), 0, 255)
+              .astype(np.uint8), rng.integers(0, 256, (48, 64, 3), dtype=np.uint8)]
+    return R.encode_clip(frames, 0, 4, 32)
 
 
 @pytest.mark.parametrize("g", GOPS, ids=[str(g) for g in GOPS])
@@ -114,9 +127,9 @@ def test_translating_clips_get_the_true_displacement(name):
         else:                                            # where the true block lies inside the frame
             where = np.ones(enc[t][2].shape, bool)
             where[-1], where[:, 0] = False, False
-        coded = where & (enc[t][2] == G.INTER)
+        coded = where & (enc[t][2] == R.INTER)
         assert coded.sum() >= 2, (name, t)
-        assert (enc[t][3][coded] == truth[t - 1]).all(), (name, t, enc[t][3][coded].tolist(), truth[t - 1])
+        assert (enc[t].mv[coded] == truth[t - 1]).all(), (name, t, enc[t].mv[coded].tolist(), truth[t - 1])
 
 
 def test_every_macroblock_type_phase_and_predictor_occurs():
@@ -124,39 +137,40 @@ def test_every_macroblock_type_phase_and_predictor_occurs():
     for name, *_ in me_cases():
         for e in encoded(name, "T"):
             types |= set(e[2].reshape(-1))
-            if e[3] is None:
+            if e.mv is None:
                 continue
-            p = e[2] == G.INTER
-            phases |= {(int(x) & 3, int(y) & 3) for x, y in e[3][p]}
+            p = e[2] == R.INTER
+            phases |= {(int(x) & 3, int(y) & 3) for x, y in e.mv[p]}
             for my in range(p.shape[0]):
                 for mx in range(p.shape[1]):
                     if not p[my, mx]:
                         continue
-                    mvp = e[3][my, mx - 1] if mx and p[my, mx - 1] else np.zeros(2)
-                    mvd_nonzero |= bool((e[3][my, mx] != mvp).any())
+                    mvp = e.mv[my, mx - 1] if mx and p[my, mx - 1] else np.zeros(2)
+                    mvd_nonzero |= bool((e.mv[my, mx] != mvp).any())
                     left_pred |= bool(mvp.any())
-    assert types == {G.SKIP, G.INTER, "DC", "H", O.PCM}
+    assert types == {R.SKIP, R.INTER, "DC", "H", O.PCM}
     assert len(phases) == 16 and mvd_nonzero and left_pred
 
 
 @pytest.mark.parametrize("name", [c[0] for c in me_cases()])
 def test_search_0_is_the_zero_motion_rule(name):
+    """The bytes of search 0 are those the zero-motion rule's own restatement coded, pinned by their digests."""
     frames, qp, _, _ = case(name)
+    with open(os.path.join(os.path.dirname(__file__), "golden", "h264_ref_digests.json")) as f:
+        want = json.load(f)["zero_motion"]
     for gop in (2, len(frames)):
-        assert [e[0] for e in M.encode_clip(frames, qp, gop, 0)] == [e[0] for e in G.encode_clip(frames, qp, gop)]
+        enc = R.encode_clip(frames, qp, gop, 0)
+        assert [hashlib.sha256(e.data).hexdigest() for e in enc] == want[f"{name}/{gop}"]
+        assert all(e.mv is None or not e.mv.any() for e in enc)
 
 
 def test_lambda_table_is_the_formula():
-    assert M.LAMBDA == [M.lam(qp) for qp in range(52)]
-    assert M.LAMBDA[0] == 0 and M.LAMBDA[51] == 83
+    assert R.LAMBDA == [R.lam(qp) for qp in range(52)]
+    assert R.LAMBDA[0] == 0 and R.LAMBDA[51] == 83
 
 
 def test_bound_holds_on_noise_at_search_32_and_qp_0():
-    rng = np.random.default_rng(4)
-    a = rng.integers(0, 256, (48, 64, 3), dtype=np.uint8)
-    frames = [a, np.roll(a, (3, -5), (0, 1)), np.clip(a.astype(int) + rng.integers(-30, 31, a.shape), 0, 255)
-              .astype(np.uint8), rng.integers(0, 256, (48, 64, 3), dtype=np.uint8)]
-    enc = M.encode_clip(frames, 0, 4, 32)
+    enc = noise_bound()
     for e in enc:
         assert len(e[0]) <= video.max_bytes(48, 64, 4)
     assert any((e[2] == O.PCM).any() for e in enc[1:])

@@ -1,5 +1,5 @@
 """H.264 motion search on the H100 (pantomatrix_b200/video.py, gop > 1 and search > 0): the samples are byte for byte
-the CPU restatement's (tests/h264_me_ref.py) on the CPU cases, random clips and the first frames of rendered EMAGE and
+the CPU restatement's (tests/h264_ref.py) on the CPU cases, random clips and the first frames of rendered EMAGE and
 CaMN clips at qp 0, 20 and 51; a rendered frame shifted by (5, -3) pixels gets vector (20, -12) on at least 80 % of
 the body's moving macroblocks; each GOP encodes as it does alone at the same parity; calls are deterministic and
 capture in a CUDA graph; search 0 is pm_h264_encode_gop; gop T + 1 gives the gop T samples; a 300-frame gop 30 search
@@ -8,7 +8,7 @@ import numpy as np
 import pytest
 import torch
 
-import h264_me_ref as M
+import h264_ref as R
 from test_video import decode
 from test_video_gop_gpu import rendered_gop, samples  # noqa: F401  (the module fixture)
 from test_video_me import GOPS, gop_of, me_cases
@@ -30,7 +30,7 @@ def _samples(frames, qp, gop, search):
 def test_me_cases_are_byte_identical_to_the_restatement(name, frames, qp, search, truth, g):
     gop = gop_of(g, len(frames))
     got = _samples(torch.as_tensor(np.stack(frames), device=DEV), qp, gop, search)
-    assert got == [e[0] for e in M.encode_clip(frames, qp, gop, search)]
+    assert got == [e[0] for e in R.encode_clip(frames, qp, gop, search)]
 
 
 def test_random_clips_are_byte_identical_to_the_restatement():
@@ -45,7 +45,7 @@ def test_random_clips_are_byte_identical_to_the_restatement():
             clip.append(f)
         for qp, gop, search in ((0, 3, 32), (12, 4, 1), (30, 5, 7), (45, 2, 16)):
             got = _samples(torch.as_tensor(np.stack(clip), device=DEV), qp, gop, search)
-            want = M.encode_clip(clip, qp, gop, search)
+            want = R.encode_clip(clip, qp, gop, search)
             for i, (b, e) in enumerate(zip(got, want)):
                 assert b == e[0], (h, w, qp, gop, search, i)
                 assert len(b) <= video.max_bytes(h, w, gop)
@@ -56,7 +56,7 @@ def test_rendered_clips_are_byte_identical_to_the_restatement(rendered_gop, qp):
     emage, body = rendered_gop
     for clip, gop, search in ((emage[0, :4], 4, 16), (body[1, :4], 4, 16)):
         got = _samples(clip, qp, gop, search)
-        assert got == [e[0] for e in M.encode_clip(list(clip.cpu().numpy()), qp, gop, search)], qp
+        assert got == [e[0] for e in R.encode_clip(list(clip.cpu().numpy()), qp, gop, search)], qp
 
 
 def test_a_shifted_render_gets_the_shift_as_vector(rendered_gop):
@@ -64,10 +64,10 @@ def test_a_shifted_render_gets_the_shift_as_vector(rendered_gop):
     a = emage[0, 0]
     b = torch.zeros_like(a)
     b[3:, :-5] = a[:-3, 5:]                               # each sample of b is a's 5 to the right and 3 up
-    enc = M.encode_clip([a.cpu().numpy(), b.cpu().numpy()], 20, 2, 8)
+    enc = R.encode_clip([a.cpu().numpy(), b.cpu().numpy()], 20, 2, 8)
     got = _samples(torch.stack([a, b]), 20, 2, 8)
     assert got == [e[0] for e in enc]
-    types, mv = enc[1][2], enc[1][3]
+    types, mv = enc[1].types, enc[1].mv
     body = (types == "P") & (mv != 0).any(-1)
     hit = (mv[body] == (20, -12)).all(-1)
     # the others match another vector at no higher J: flat shading, where a shorter vector costs fewer bits
@@ -120,5 +120,5 @@ def test_write_mp4_gop_30_search_16_of_a_300_frame_render_decodes_to_the_reconst
     assert len(lumas) == 300 and fps == 30
     host = emage[0].cpu().numpy()
     for t0 in (0, 270):
-        for i, e in enumerate(M.encode_clip(list(host[t0:t0 + 3]), 20, 30, 16)):
+        for i, e in enumerate(R.encode_clip(list(host[t0:t0 + 3]), 20, 30, 16)):
             assert np.array_equal(lumas[t0 + i].reshape(-1)[:720 * 960].reshape(720, 960), e[1][0]), t0 + i

@@ -19,7 +19,7 @@ GOP arms (keyframe interval gop 1, 30 and T, the clip length), per input: the vi
 the three gops alternating), bytes per frame (min, mean, max), and luma PSNR of the first --psnr-frames frames decoded
 by OpenCV's FFmpeg from a write_mp4 file; for the 1 x 300 EMAGE clip also the share of P_Skip / inter / intra / I_PCM
 macroblocks over one whole GOP at gop 30 (frames 0..29: the IDR frame and 29 P frames), counted by the CPU
-restatement (tests/h264_gop_ref.py), whose bytes equal the GPU's; and the output stage (render + write_mp4) at gop 1
+restatement (tests/h264_ref.py), whose bytes equal the GPU's; and the output stage (render + write_mp4) at gop 1
 against gop 30, alternating.  --gop-only runs only the GOP arms and that output stage.
 --baseline-lib: the libpm_emage.so of another build (for instance the parent commit's, built from a checkout of it):
 pm_h264_encode of that library, pm_h264_encode of this tree and pm_h264_encode_gop(gop = 1) of this tree on the
@@ -28,14 +28,14 @@ Motion search arms (--me-only runs only these): gop 30 and T with search 0, 16 a
 alternating in the timed loop: the video.encode call (median ms), bytes per frame (min, mean, max), luma PSNR of the
 first --psnr-frames frames, and the time of one call's search and code kernels from torch.profiler; for the 1 x 300
 EMAGE clip also the macroblock shares over the first --me-mb-frames frames of the first GOP at gop 30, with P split
-into zero and non-zero vectors, counted by the CPU restatement (tests/h264_me_ref.py; the whole 30-frame GOP takes it
+into zero and non-zero vectors, counted by the CPU restatement (tests/h264_ref.py; the whole 30-frame GOP takes it
 too long at 960 x 720); and the output stage (render + write_mp4) at gop 30 with search 0 against search 16.
 Intra 4x4 arms (--i4-only runs only these): gop 1 and 30, search 0 and 16 (gop 30), qp 20 and 26, each with and
 without intra4x4, per input (the EMAGE 1 x 300 and CaMN 1 x 270 clips), all alternating in the timed loop: the
 video.encode call (median ms), bytes per frame (min, mean, max) and luma PSNR of the first --psnr-frames frames; for
-the EMAGE clip also, from the CPU restatement (tests/h264_i4_ref.py) over its first --i4-mb-frames frames at gop 30
+the EMAGE clip also, from the CPU restatement (tests/h264_ref.py) over its first --i4-mb-frames frames at gop 30
 and search 0, the macroblock shares, the histogram of the nine modes, and the bytes for several values of the rule's
-constant c.
+constant c and without intra4x4.
 The card's name, power limit and max SM clock are read in the same run.  Nothing is written except OUT."""
 import ctypes
 import argparse
@@ -61,10 +61,8 @@ from pantomatrix_b200.pipeline import generate  # noqa: E402
 from pantomatrix_b200.render import MeshRenderer  # noqa: E402
 from synthetic_models import build_lstm_product, build_product, smplx_surface_arrays  # noqa: E402
 
+# the CPU restatement tests/h264_ref.py is imported only by the arms that count macroblocks with it
 sys.path.insert(0, os.path.join(ROOT, "tests"))
-import h264_gop_ref  # noqa: E402
-import h264_i4_ref  # noqa: E402
-import h264_me_ref  # noqa: E402
 
 QP = 20
 
@@ -220,7 +218,8 @@ def gop_arms(frames, reps, psnr_frames, mb_types, tmp):
                           "bytes_per_frame_max": int(sizes.max()), "file_bytes_clip0": os.path.getsize(path),
                           "luma_psnr_db_mean": psnr_mean, "luma_psnr_db_min": psnr_min}
         if mb_types and g == 30 < t:
-            enc = h264_gop_ref.encode_clip(list(clip[:g].cpu().numpy()), QP, g)
+            import h264_ref
+            enc = h264_ref.encode_clip(list(clip[:g].cpu().numpy()), QP, g)
             types = np.concatenate([e[2].reshape(-1) for e in enc])
             out[f"gop{g}"]["mb_share_first_gop"] = {k: float((types == k).mean())
                                                     for k in ("SKIP", "P", "DC", "H", "PCM")}
@@ -287,9 +286,10 @@ def me_arms(frames, reps, psnr_frames, mb_frames, tmp):
             "luma_psnr_db_mean": psnr_mean, "luma_psnr_db_min": psnr_min,
             "kernel_ms": kernel_split(frames, g, s)}
         if mb_frames and g == 30:
-            enc = h264_me_ref.encode_clip(list(clip[:mb_frames].cpu().numpy()), QP, g, s)
+            import h264_ref
+            enc = h264_ref.encode_clip(list(clip[:mb_frames].cpu().numpy()), QP, g, s)
             types = np.concatenate([e[2].reshape(-1) for e in enc])
-            moved = np.concatenate([(e[3] if e[3] is not None else np.zeros(e[2].shape + (2,), int)).any(-1)
+            moved = np.concatenate([(e.mv if e.mv is not None else np.zeros(e.types.shape + (2,), int)).any(-1)
                                     .reshape(-1) for e in enc])
             share = {k: float((types == k).mean()) for k in ("SKIP", "DC", "H", "PCM")}
             share["P_zero"] = float(((types == "P") & ~moved).mean())
@@ -368,20 +368,21 @@ def i4_arms(frames, reps, psnr_frames, mb_frames, tmp):
             "bytes_per_frame_max": int(sizes.max()), "luma_psnr_db_mean": psnr_mean, "luma_psnr_db_min": psnr_min}
         print("  arm", g, s, q, i4, json.dumps({k: v for k, v in a.items() if k != "encode_ms_all"}), flush=True)
     if mb_frames:
+        import h264_ref
         host = list(clip[:mb_frames].cpu().numpy())
         for q in (20, 26):
-            enc = h264_i4_ref.encode_clip(host, q, 30, 0)
+            enc = h264_ref.encode_clip(host, q, 30, 0, True)
             assert [e[0] for e in enc] == [bytes(x) for x in _first_samples(clip[:mb_frames], 30, 0, q, True)]
             types = np.concatenate([e[2].reshape(-1) for e in enc])
-            modes = np.concatenate([e[3][e[2] == "I4"].reshape(-1) for e in enc])
+            modes = np.concatenate([e.modes[e.types == "I4"].reshape(-1) for e in enc])
             sweep = {}
             for c in (0, 3, 6, 12, 24):
-                sweep[c] = [len(e[0]) for e in h264_i4_ref.encode_clip(host, q, 30, 0, c=c)]
+                sweep[c] = [len(e[0]) for e in h264_ref.encode_clip(host, q, 30, 0, True, c)]
             out[f"restatement_qp{q}"] = {
-                "frames": mb_frames, "c": h264_i4_ref.C_I4,
+                "frames": mb_frames, "c": h264_ref.C_I4,
                 "mb_share": {k: float((types == k).mean()) for k in ("SKIP", "P", "DC", "H", "I4", "PCM")},
                 "mode_histogram": np.bincount(modes, minlength=9).tolist(),
-                "bytes_by_c": sweep, "bytes_without_i4": [len(e[0]) for e in h264_me_ref.encode_clip(host, q, 30, 0)]}
+                "bytes_by_c": sweep, "bytes_without_i4": [len(e[0]) for e in h264_ref.encode_clip(host, q, 30, 0)]}
             print("  restatement", q, json.dumps(out[f"restatement_qp{q}"]), flush=True)
     return out
 
